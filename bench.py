@@ -31,6 +31,35 @@ FS_BY = {"cfg2": 100e6, "cfg3": 200e6, "cfg4": 50e6, "cfg5": 100e6}
 NFFT_BY = {"cfg2": 65536, "cfg3": 65536, "cfg4": 32768, "cfg5": 65536}
 FS = 100e6     # replaced per workload in main()
 B_ALG = {"cfg2": 12.09, "cfg3": 14.41, "cfg4": 12.06, "cfg5": 12.0}     # SURVEY 8(d), bytes per input sample
+HBM_PEAK_GBS = 3350.0     # H100 SXM data sheet (HBM3); MEASURED_PEAKS.json hbm_gbs overrides it where present
+DUMP_STREAMS, DUMP_FRAMES, DUMP_SYMBOLS = 16, 4, 2048      # --dump-outputs sample: at most 42 MB at N = 65536
+
+
+def dump_outputs(d, arrays):
+    """Writes each array as d/<name>.npy (float32, or float64 where the values are counts)."""
+    os.makedirs(d, exist_ok=True)
+    for k, v in arrays.items():
+        np.save(os.path.join(d, k + ".npy"), np.ascontiguousarray(v))
+
+
+def engine_outputs(e, hs):
+    """PSD frames and soft / hard symbols of the last feed for a fixed, seeded sample of the streams (a full step of
+    the default workload is 0.3 GB of PSD alone)."""
+    S = e.n_streams
+    pick = np.sort(np.random.default_rng(0).choice(S, min(DUMP_STREAMS, S), replace=False))
+    psd = e.read_psd()[pick, -DUMP_FRAMES:]
+    soft, hard, counts = [], [], np.zeros((len(pick), len(hs)), np.float64)
+    for i, s in enumerate(pick):
+        for j, h in enumerate(hs):
+            sf, hd = e.read_symbols(int(s), h)
+            sf, hd = sf[-DUMP_SYMBOLS:], hd[-DUMP_SYMBOLS:]
+            soft.append(sf.view(np.float32).reshape(-1, 2))
+            hard.append(hd.astype(np.float32))
+            counts[i, j] = len(hd)
+    out = {"streams": pick.astype(np.float64), "psd": psd, "symbol_counts": counts}
+    if hs:
+        out.update(soft=np.concatenate(soft), hard=np.concatenate(hard))
+    return out
 
 
 # --------------------------------------------------------------------------------------------------
@@ -100,7 +129,7 @@ def make_base_signal(name, n, seed):
 
 
 # --------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md recipe)
+# clocks sampler: SM clock and throttle reasons over the timed region
 # --------------------------------------------------------------------------------------------------
 class Clocks:
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -486,7 +515,7 @@ def run_cuda_cfg5(args):
     det = dict(alpha=1.0, gamma=0.5, snr=6.0, min_bins=2)
     p = sdb.Panoramic(N_FFT, "blackmann_harris", FS, (fmin, fmax), rel_bw, device=local, rank=rank, world=world,
                       unique_id=panoramic.exchange_unique_id(sdb, torch, dist), detect=det)
-    flush = torch.empty(160 << 20, dtype=torch.uint8, device="cuda")      # > 126 MB L2
+    flush = torch.empty(160 << 20, dtype=torch.uint8, device="cuda")      # > the H100's 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -521,6 +550,8 @@ def run_cuda_cfg5(args):
     samples = CFG5_HOPS * N_FFT
     value = samples * args.steps / (ms * 1e-3) / 1e6
     tm = p.timing()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(zip(("view_psd", "view_accum", "view_count"), p.read())))
     # end to end: pinned host hop buffers -> H2D -> sweep -> D2H of the stitched view (+ channel lists) on rank 0
     def step_e2e():
         p.reset()
@@ -545,7 +576,7 @@ def run_cuda_cfg5(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
     # dominant kernels: the two passes of the hop PSDs (inside psd_project_ms); B_alg = 8 B in + 4 B out per sample
     ach = B_ALG["cfg5"] * (hi - lo) * N_FFT / (tm["psd_project_ms"] * 1e-3) / 1e9 if tm["psd_project_ms"] > 0 else 0.0
     try:
@@ -699,10 +730,12 @@ def run_cuda(args):
         ms = timed(step_dev, args.steps)
     launches = e.launches - l0
     value = samples_step * world * args.steps / (ms * 1e-3) / 1e6
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, engine_outputs(e, hs))
 
     # ---- per-kernel device times: a separate pass in the engine's timing mode, which queues every kernel on ONE
     # stream (no two kernels overlap), so the CUDA-event spans recorded on that stream are the kernels' own warm
-    # durations; the ncu launch list of the same command is committed under profiles/ (shares must agree)
+    # durations
     e.timing(True)
     timed_steps = 2
     for _ in range(timed_steps):
@@ -721,53 +754,22 @@ def run_cuda(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
     launches_dom = max(1.0, fam[dom][1] / timed_steps)                     # launches per step
     alg_launch = B_ALG[name] * samples_step / launches_dom
     ach = alg_launch / (fam[dom][0] * 1e-3) / 1e9 if fam[dom][0] > 0 else 0.0
-    traffic = None
-    try:   # DRAM bytes per launch of that kernel from the committed single-pass ncu capture of this workload
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        if tr.get("workload") == name and dom in tr.get("kernels", {}):
-            traffic = tr["kernels"][dom]["dram_bytes_per_launch"]
-            # the capture was taken at tr["streams_per_gpu"] streams; the inspector / inverse-transform kernels
-            # cover every stream in one launch, so their per-launch traffic scales with the stream count
-            if dom in ("inspector", "chan_ifft") and tr.get("streams_per_gpu"):
-                traffic = int(traffic * S / tr["streams_per_gpu"])
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak, "unit": "GB/s",
-                "frac": ach / peak, "traffic": traffic,
+                "frac": ach / peak, "traffic": None,
                 "algorithmic_bytes_per_launch": alg_launch, "launch_ms": fam[dom][0],
                 "note": "B_alg (SURVEY 8d) x input samples covered by one launch / its duration; durations are "
-                        "CUDA-event spans of a serialised pass (one stream, no overlap). The kernel is bound by "
-                        "instruction issue / recurrence latency, not by DRAM (profiles/r02_*.md)",
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s",
+                        "CUDA-event spans of a serialised pass (one stream, no overlap)",
+                "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, %g GB/s" % HBM_PEAK_GBS,
                 "kernel_share_of_device_time": tot[dom] / max(1e-9, sum(tot.values())),
                 "device_ms_per_step": {f: round(tot[f], 4) for f in tot},
                 "launch_ms_avg": {f: round(fam[f][0], 4) for f in fam},
                 "path": {"b_alg_bytes_per_sample": B_ALG[name],
                          "achieved": B_ALG[name] * value * 1e6 / world / 1e9,
                          "frac": B_ALG[name] * value * 1e6 / world / 1e9 / peak}}
-    # The path's other roofline: instruction issue.  Every input sample costs a fixed number of warp instructions
-    # (64 inspectors' recurrences, filters and transforms; counted by ncu, profiles/r02_traffic.json), and an SM issues
-    # at most 4 warp instructions per clock: the ceiling that count sets, whatever the memory system does.
-    try:
-        wi = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        if wi.get("workload") == name and "warp_instructions" in wi:
-            w = wi["warp_instructions"]
-            per_sample = sum(w["per_step_148_streams"].values()) / float(w["input_samples_per_step"])
-            sm_clock = (clk.summary().get("sm_mhz") or 1965.0) * 1e6
-            ceiling = 148 * 4 * sm_clock / per_sample / 1e6          # MS/s per GPU
-            roofline["issue"] = {"warp_instructions_per_input_sample": round(per_sample, 2),
-                                 "ceiling_msps_per_gpu": round(ceiling, 1),
-                                 "frac": round(value / world / ceiling, 4),
-                                 "ceiling_as_hbm_frac": round(B_ALG[name] * ceiling * 1e6 / 1e9 / peak, 4),
-                                 "note": "148 SMs x 4 warp instructions per clock / instructions per sample: even a "
-                                         "perfectly issue-bound run of this instruction stream stays below this "
-                                         "fraction of the HBM roofline"}
-    except Exception:
-        pass
     if os.environ.get("SDB_LIB"):      # instrumented twin: busy cycles per role warp per chunk sample
         sdb.stage_cycles(reset=True)
         step_dev(); e.sync()
@@ -908,17 +910,17 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-single", action="store_true")
     ap.add_argument("--no-formats", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed (a fixed, seeded sample) as DIR/<name>.npy")
     args = ap.parse_args()
     global FS, N_FFT
     FS = FS_BY[args.workload]
     N_FFT = NFFT_BY[args.workload]
     if args.streams == 0:
         # cfg2: the (latency-bound) inspector kernel of 1024 single-channel streams takes about as long as their
-        # transforms; 2048 streams put the transforms on the critical path (33.9 / 53.3 / 64.5 GS/s at 512 / 1024 /
-        # 2048 streams on one B200, profiles/r01_batch.md)
-        # cfg3: 148 streams are one wave of inspector CTAs (2 per SM); with 296 the CTAs of the faster inspector
-        # classes are back-filled as they retire (15.2 / 15.8 / 16.1 / 16.1 GS/s at 148 / 222 / 296 / 444 streams,
-        # profiles/r02_summary.md)
+        # transforms; 2048 streams put the transforms on the critical path.
+        # cfg3: the inspector kernel runs 2 CTAs per SM; more streams than one wave let the CTAs of the faster
+        # inspector classes be back-filled as they retire.
         args.streams = {"cfg2": 2048, "cfg3": 296, "cfg4": 1024, "cfg5": 0}[args.workload]
     if args.impl == "reference":
         run_reference(args)

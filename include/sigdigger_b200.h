@@ -1,9 +1,9 @@
 /*
- * sigdigger_b200.h -- C-ABI of libsigdigger_b200.so: the B200-native replacement of the suscan /
+ * sigdigger_b200.h -- C-ABI of libsigdigger_b200.so: the H100-native replacement of the suscan /
  * sigutils analyzer hot path that BatchDrake/SigDigger drives (SURVEY.md section 8).
  *
  * Plain C, plain pointers and sizes, no CUDA or torch types.  Every entry point names the reference
- * interface it replaces (file:line under /root/reference).  `const sdb_complex *` has the layout of
+ * interface it replaces (file:line in the SigDigger sources).  `const sdb_complex *` has the layout of
  * SUCOMPLEX (interleaved float32 re, im).  Functions return 0 / a non-negative value on success and -1
  * on failure (SUBOOL-style callers map that to SU_FALSE; message via sdb_last_error(), which plays
  * the role of the sigutils log sink, include/Suscan/Logger.h:55).  There is NO CPU fallback: without a

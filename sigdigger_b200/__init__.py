@@ -1,6 +1,6 @@
 """sigdigger_b200 -- Python host mirror of the C-ABI in include/sigdigger_b200.h.
 
-The product is libsigdigger_b200.so (hand-written CUDA for sm_100a + a C++ host runtime); this module
+The product is libsigdigger_b200.so (hand-written CUDA for sm_90a + a C++ host runtime); this module
 is a thin ctypes binding used by the tests and the benchmark.  It fails loudly when the native library
 is missing or no CUDA device is present: there is no CPU path.
 """
@@ -417,7 +417,7 @@ def load_library():
     global _lib
     if _lib is None:
         # SDB_LIB selects the instrumented twin (libsigdigger_b200_prof.so: per-role cycle counters compiled into
-        # the inspector kernel) for profiles/; the product library is the default and the only one tests load
+        # the inspector kernel); the product library is the default and the only one tests load
         path = os.environ.get("SDB_LIB") or LIB_PATH
         if not os.path.exists(path):
             raise RuntimeError("native library %s missing: run `python __graft_entry__.py` (build())" % path)

@@ -36,19 +36,13 @@
 //   5     6-9    demod     ask: exp(-i phase), mix, component (|.| / I / Q), in place in ringB -- feed-forward
 //                          once the phases are known (4 samples per warp)                        ringB
 //   6     6-9    filter    matched filter: 4 outputs per warp straight off ringB (its history IS
-//                          the filter line), one FFMA2 per complex sample x tap; audio LPF (IIR, 1 warp) ringC[2]
+//                          the filter line), two FFMAs per complex sample x tap; audio LPF (IIR, 1 warp) ringC[2]
 //   7     10     clock     Gardner | sampler | resampler, CMA (recurrence)                       sym[2], cnt[2]
 //   8     11     out       x0.75, decision (atan2 / modulus quantiser), symbol stores            global
 //
-// Round 1 ran four stage-warps per CTA (8 warps per SM: issue slots 10 % busy, half of all stall samples on
-// the barrier behind the slowest stage, profiles/r01_inspector_stages.md); the feed-forward work (two logarithm /
-// exponential evaluations, the 19...75-tap FIR, the decision) now runs beside the recurrences instead of in series
-// with them.  Loop state lives in registers for the whole feed; the per-chain lines (AGC delay line + magnitude
-// history, CMA) in shared memory sized from the channel plan (SdbInspDyn).  Two other mappings were built, measured
-// and dropped this round (profiles/r02_inspector.md): 6 warps x chunks of 8 with the roles specialised per inspector
-// class, and the same with every chunk loop unrolled over register arrays -- both correct, both slower: the kernel
-// grew to 360 KB / 676 KB of code and every role warp starved on instruction fetch.  The recurrences run at about
-// six cycles per instruction whatever the mapping, so this kernel keeps its loops rolled and its code small (84 KB).
+// Feed-forward work runs beside the recurrences, not in series with them.  Loop state lives in registers for the
+// whole feed, the per-chain lines in shared memory sized from the channel plan (SdbInspDyn).  Loops stay rolled:
+// unrolled or per-class variants grow the code several-fold and starve the role warps on instruction fetch.
 #define CH 16
 enum { INSP_WARPS = 12 };              // role of each warp: see the dispatch at the end of k_inspectors
 #define INSP_STEPS 8          // pipeline depth after the load: a chunk loaded in iteration c leaves in iteration c + 8
@@ -186,7 +180,7 @@ static __device__ void role_track(const ICtx &c, const float2 *chan_row)
   float *dl = nullptr, *mh = nullptr; bool in_smem = false;
   // the delay line is a pure delay (feed-forward): with the lines in shared memory and at least a chunk long, the
   // two pre warps swap their own samples through it (distinct slots within a chunk) and this warp keeps only the
-  // level tracker, the recurrence (role_pre; 546 -> see profiles/r02_summary.md cycles per sample)
+  // level tracker, the recurrence (role_pre)
   bool dl_in_pre = false; unsigned dl_ptr0 = 0;
   if (have_agc) {
     far_ = cp->far_; faf = cp->faf; sar = cp->sar; saf = cp->saf;
@@ -590,7 +584,7 @@ static __device__ void role_carrier(const ICtx &c)
 // The carrier ring IS the filter line: output p needs x[p - t], t < mf_n, which are the mf_n most recent ring
 // entries (the last mf_n - 1 samples of the previous feed are put back in front of position 0 at kernel start).
 // One thread produces 4 consecutive outputs of its chain from a sliding register window: per tap one ring load,
-// one tap load and four packed FFMA2 (complex sample x real tap, SPEC I.1: ascending taps, fused terms).
+// one tap load and four complex-by-real FMAs (complex sample x real tap, SPEC I.1: ascending taps, fused terms).
 static __device__ void role_filter(const ICtx &c, int part, const float *taps_pool)
 {
   ChainSmem &sm = *c.sm;
@@ -912,7 +906,7 @@ __global__ void __launch_bounds__(INSP_WARPS * 32, 2) k_inspectors(const SdbChai
 #endif
 
   // Role of each warp.  Warps go to the SM's four schedulers by warp index modulo 4, and the matched filter is the one
-  // role that can issue every cycle (independent FFMA2s): three of its four warps share scheduler 1 among themselves,
+  // role that can issue every cycle (independent FFMAs): three of its four warps share scheduler 1 among themselves,
   // so that the recurrence warps (track, carrier -- the roles that set the CTA's pace) never compete with one for
   // an issue slot:  scheduler 0: track, pre 0, out;  1: filter 0-2;  2: carrier, pre 1, post 0;  3: clock, post 1, filter 3
   // (one call site per role with the part as a run-time value: a call per warp index would inline four copies of the
@@ -971,7 +965,7 @@ cudaError_t sdb_launch_inspectors_n(const SdbLaunchCtx &c, const SdbChainCfg *cf
   const size_t smem = sdb_inspector_smem_bytes(dyn);
   if (!chain_map) n_ctas = (chains + 31) / 32;
   // SDB_INSP_PLACEMENT=linear: roles in warp order (track, pre x2, post x2, carrier, filter x4, clock, out), the
-  // placement of the first builds -- kept for A/B measurements (profiles/r02_inspector.md)
+  // placement of the first builds -- kept for A/B measurements
   static const bool linear = getenv("SDB_INSP_PLACEMENT") && !strcmp(getenv("SDB_INSP_PLACEMENT"), "linear");
   SdbInspDyn d2 = dyn;
   if (linear) { d2.role_lut = 0x653333244110ull; d2.part_lut = 0x3210010100ull; }

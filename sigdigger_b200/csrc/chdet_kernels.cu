@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(1024) k_chdet_find(const ChdetK p)
 // ---- k = r * 1024 + tid) from the exponential average (K.1, same expression and frame order as k_chdet_avg) through
 // ---- the four radix-select passes (K.2); the threshold test leaves a bit map in frequency order in shared memory
 // ---- (warp votes; ascending frequency j = k xor N/2), and the run events of K.3 are read off that map word by word.
-// ---- One read of the PSD frames, one read + one write of the average: 0.35 + 0.68 ms -> see profiles/r02_summary.md.
+// ---- One read of the PSD frames, one read + one write of the average.
 // ---- Same values as k_chdet_avg + k_chdet_find bit for bit (exact order statistic, ordered events).
 #define CHDET_RMAX 64
 #define CHDET_RREG 32                           // values per thread kept in registers; the rest in shared memory

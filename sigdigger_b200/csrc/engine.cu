@@ -1,4 +1,4 @@
-// engine.cu -- host runtime + C-ABI (include/sigdigger_b200.h) of the B200 analyzer engine.
+// engine.cu -- host runtime + C-ABI (include/sigdigger_b200.h) of the H100 analyzer engine.
 //
 // One engine = one channel plan applied to a batch of S independent IQ streams on one GPU.
 // feed(): main PSD over every psd_size frame (four-step FFT, two kernels), channeliser forward FFT
@@ -600,12 +600,17 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       if (cw < 1) cw = 1;
       if ((big == 65536 || big == 32768 || big == 16384 || big == 8192) && !getenv("SDB_SCRATCH_MB")) {
         // 65536 path: 16 (pass A, 4 CTAs/SM) and 8 (pass B, 2 CTAs/SM) CTAs per window, all of equal duration:
-        // one window per SM is exactly 4 waves of either kernel.  148 SMs -> 148 windows -> 77.6 MB, inside
-        // the 82.9 MB of L2 that can be set aside for persisting lines on B200.
-        int sms = 0;
+        // one window per SM is exactly 4 waves of either kernel.  On an H100 that is 132 windows, 69 MB, more than
+        // its 50 MB L2 can set aside for persisting lines, so the chunk is halved (whole waves still: 2 per kernel,
+        // 34.6 MB) until it fits the set-aside.  bench.py cfg3 on an H100 80GB HBM3 at 400 W: 10.6 GS/s with the
+        // halved chunk, 7.6 GS/s with one window per SM (SDB_CHUNK_WINDOWS=132).
+        int sms = 0, max_persist = 0;
         if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->prm.device) == cudaSuccess && sms > 0 &&
-            (size_t) sms * 65536 * sizeof(float2) <= (100u << 20))
-          cw = (size_t) sms * (65536 / big);          // the same 77.6 MB: two 32768-point windows per SM, ...
+            (size_t) sms * 65536 * sizeof(float2) <= (100u << 20)) {
+          cw = (size_t) sms * (65536 / big);          // the same bytes: two 32768-point windows per SM, ...
+          cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, e->prm.device);
+          while (max_persist > 0 && cw % 2 == 0 && cw * big * sizeof(float2) > (size_t) max_persist) cw /= 2;
+        }
         e->sm_count = sms;
       }
       if (const char *env = getenv("SDB_CHUNK_WINDOWS")) { long v = atol(env); if (v >= 1 && v <= 65536) cw = (size_t) v; }
@@ -617,8 +622,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
         CK(cudaEventCreateWithFlags(&e->ev_feed, cudaEventDisableTiming));
       }
       // Pin the scratch in L2.  Without this the streamed input and output evict it between the two passes
-      // and every window costs two extra HBM round trips (ncu: 266 MB of DRAM traffic per 148-window chunk
-      // against 116 MB algorithmic, profiles/r01_l2.md).  Accesses of the transform streams inside the window
+      // and every window costs two extra HBM round trips.  Accesses of the transform streams inside the window
       // are "persisting" (a set-aside part of L2 that normal traffic cannot evict); the kernels additionally
       // mark their one-shot outputs as streaming (st.global.cs).
       if ((big == 65536 || big == 32768 || big == 16384 || big == 8192) && !getenv("SDB_NO_L2_PIN")) {   // the set-aside is device-wide: only the big plans claim it

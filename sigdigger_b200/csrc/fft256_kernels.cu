@@ -11,7 +11,7 @@
 //       so that a warp holds 32 consecutive output bins -> 128-byte PSD / compacted-spectrum stores.
 //
 // Same mathematics as the generic path in fft_kernels.cu (which remains for every other size); results
-// are bit-identical to oracle/fft_spec.c (SPEC.md F.4).  Designs measured and rejected: profiles/r01_experiments.md.
+// are bit-identical to oracle/fft_spec.c (SPEC.md F.4).
 // Replaces the forward FFTs of su_specttuner
 // (Tasks/LPFTask.cpp:83-87) and of the PSD (Suscan/Messages/PSDMessage.cpp:26-39).
 #include "sdb_internal.h"
@@ -22,8 +22,7 @@
 #define S1 0.38268343236508977173f   // sin(pi/8)
 #define R2 0.70710678118654752440f
 
-// complex arithmetic (cadd, csub, cmulf = SPEC F.1 twiddle product, fft4) on the packed FP32x2 pipe:
-// sdb_cpx.h.  The unit is compiled with -fmad=false so nothing else is contracted.
+// complex arithmetic (cadd, csub, cmulf = SPEC F.1 twiddle product, fft4): sdb_cpx.h.  The unit is compiled with -fmad=false so nothing else is contracted.
 
 // forward 16-point DFT of v[0..15] (natural order in).  Result X[m + 4 q] is left in v[4 m + q].
 static __device__ __forceinline__ void fft16(float2 (&v)[16])

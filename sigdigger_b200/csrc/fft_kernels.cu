@@ -1,4 +1,4 @@
-// fft_kernels.cu -- cuFFT-free FFT machinery of the analyzer hot path, hand-written for sm_100a.
+// fft_kernels.cu -- cuFFT-free FFT machinery of the analyzer hot path, hand-written for sm_90a.
 //
 //   * block_fft_inplace: Stockham radix-4 (+ one radix-2) transform of M points held in shared
 //     memory, twiddles from a correctly rounded table (W_M^i computed in double on the host).
@@ -67,9 +67,8 @@ static __device__ __forceinline__ void block_fft_inplace(float2 *s, const int M,
       const int j = lane + b * nthr;
       if (j < q) {
         const int k = j & (Ns - 1);
-        // packed FP32x2 arithmetic (sdb_cpx.h): the same IEEE operations per component as the scalar statement of
-        // SPEC F.1 / F.2 (a complex add is one FADD2, the twiddle product one FMUL2 + one FFMA2), so the results
-        // are bit-identical and the butterfly issues ~14 instead of ~34 arithmetic instructions
+        // complex arithmetic of sdb_cpx.h: the same IEEE operations per component as the scalar statement of
+        // SPEC F.1 / F.2, so the results are bit-identical
         if (logNs > 0) {
           const int step = M >> (logNs + 2);
           float2 w1 = ldtw(tw, k * step), w2 = ldtw(tw, 2 * k * step), w3 = ldtw(tw, 3 * k * step);

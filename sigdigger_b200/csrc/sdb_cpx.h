@@ -1,55 +1,25 @@
-// sdb_cpx.h -- complex binary32 arithmetic on sm_100a's packed FP32x2 pipe.
+// sdb_cpx.h -- complex binary32 arithmetic for the FFT and chain kernels (sm_90a).
 //
-// Blackwell adds add/sub/mul/fma.rn.f32x2 (SASS FADD2 / FMUL2 / FFMA2): one instruction, two IEEE
-// round-to-nearest binary32 lanes held in an aligned register pair -- exactly the (re, im) layout of a
-// float2.  ptxas folds lane swaps (.LO_HI), broadcasts (.F32) and per-lane sign flips (.NP) into the
-// operand modifiers, so a complex add is ONE issue slot, the SPEC F.1 twiddle product is TWO and a
-// 4-point DFT is EIGHT (16 / 4 / 16 with scalar FADD / FMUL / FFMA).  Every lane result is bit-identical
-// to the scalar expression it replaces (same operation, same rounding), so the parity with
-// oracle/fft_spec.c is unchanged.  The FFT kernels are issue-bound, not FP-pipe-bound (profiles/), which is
-// why halving the instruction count matters.
+// One explicit round-to-nearest intrinsic per component, so the compiler can neither contract nor reorder a
+// rounding: the parity with oracle/fft_spec.c rests on these exact expressions.
 #pragma once
 #include <cuda_runtime.h>
 
-typedef unsigned long long sdb_u64;
-
-static __device__ __forceinline__ sdb_u64 sdb_pk(float lo, float hi)
-{
-  sdb_u64 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-static __device__ __forceinline__ float2 sdb_up(sdb_u64 v)
-{
-  float2 r;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
-  return r;
-}
 static __device__ __forceinline__ float2 sdb_add2(float2 a, float2 b)
 {
-  sdb_u64 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(sdb_pk(a.x, a.y)), "l"(sdb_pk(b.x, b.y)));
-  return sdb_up(r);
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 }
 static __device__ __forceinline__ float2 sdb_sub2(float2 a, float2 b)
 {
-  sdb_u64 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(sdb_pk(a.x, a.y)), "l"(sdb_pk(b.x, b.y)));
-  return sdb_up(r);
+  return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y));
 }
 static __device__ __forceinline__ float2 sdb_mul2(float2 a, float2 b)
 {
-  sdb_u64 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(sdb_pk(a.x, a.y)), "l"(sdb_pk(b.x, b.y)));
-  return sdb_up(r);
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
 static __device__ __forceinline__ float2 sdb_fma2(float2 a, float2 b, float2 c)
 {
-  sdb_u64 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(r)
-      : "l"(sdb_pk(a.x, a.y)), "l"(sdb_pk(b.x, b.y)), "l"(sdb_pk(c.x, c.y)));
-  return sdb_up(r);
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 static __device__ __forceinline__ float2 cadd(float2 a, float2 b) { return sdb_add2(a, b); }
@@ -58,37 +28,31 @@ static __device__ __forceinline__ float2 mul_mi(float2 a) { return make_float2(a
 static __device__ __forceinline__ float2 mul_pi(float2 a) { return make_float2(-a.y, a.x); }   // a * (+i)
 
 // SPEC F.1 twiddle product: re = fma(a.re, b.re, -(a.im b.im)), im = fma(a.re, b.im, a.im b.re).
-// p = (a.im b.im, a.im b.re) is one FMUL2; the sign of p.re rides on the FFMA2's addend modifier.
 static __device__ __forceinline__ float2 cmulf(float2 a, float2 b)
 {
-  const float2 p = sdb_mul2(make_float2(a.y, a.y), make_float2(b.y, b.x));
-  return sdb_fma2(make_float2(a.x, a.x), b, make_float2(-p.x, p.y));
+  return make_float2(__fmaf_rn(a.x, b.x, -__fmul_rn(a.y, b.y)), __fmaf_rn(a.x, b.y, __fmul_rn(a.y, b.x)));
 }
 // a * conj(b), same rounding pattern with b.im negated: re = fma(a.re, b.re, a.im b.im),
 // im = fma(a.re, -b.im, a.im b.re)
 static __device__ __forceinline__ float2 cmulf_conj(float2 a, float2 b)
 {
-  const float2 p = sdb_mul2(make_float2(a.y, a.y), make_float2(b.y, b.x));
-  return sdb_fma2(make_float2(a.x, a.x), make_float2(b.x, -b.y), p);
+  return make_float2(__fmaf_rn(a.x, b.x, __fmul_rn(a.y, b.y)), __fmaf_rn(a.x, -b.y, __fmul_rn(a.y, b.x)));
 }
 
-// forward 4-point DFT in place: (a, b, c, d) <- DFT4.  b and d need d0 -/+ i t with t = b - d:
-// d0 + (t.im, -t.re) written as fma((t.im, t.re), (1, -1), d0): the product by +-1 is exact, so the single
-// rounding equals that of the plain add / subtract.
+// forward 4-point DFT in place: (a, b, c, d) <- DFT4, b = d0 - i t and d = d0 + i t with t = b - d
+// (one rounded add or subtract per lane, as in oracle/fft_spec.c)
 static __device__ __forceinline__ void fft4(float2 &a, float2 &b, float2 &c, float2 &d)
 {
   const float2 s0 = cadd(a, c), d0 = csub(a, c), s1 = cadd(b, d), t = csub(b, d);
-  const float2 ts = make_float2(t.y, t.x);
   a = cadd(s0, s1); c = csub(s0, s1);
-  b = sdb_fma2(ts, make_float2(1.0f, -1.0f), d0);
-  d = sdb_fma2(ts, make_float2(-1.0f, 1.0f), d0);
+  b = make_float2(__fadd_rn(d0.x, t.y), __fsub_rn(d0.y, t.x));
+  d = make_float2(__fsub_rn(d0.x, t.y), __fadd_rn(d0.y, t.x));
 }
 // inverse 4-point DFT (kernel exp(+i...)): b = d0 + i t, d = d0 - i t
 static __device__ __forceinline__ void ifft4(float2 &a, float2 &b, float2 &c, float2 &d)
 {
   const float2 s0 = cadd(a, c), d0 = csub(a, c), s1 = cadd(b, d), t = csub(b, d);
-  const float2 ts = make_float2(t.y, t.x);
   a = cadd(s0, s1); c = csub(s0, s1);
-  b = sdb_fma2(ts, make_float2(-1.0f, 1.0f), d0);
-  d = sdb_fma2(ts, make_float2(1.0f, -1.0f), d0);
+  b = make_float2(__fsub_rn(d0.x, t.y), __fadd_rn(d0.y, t.x));
+  d = make_float2(__fadd_rn(d0.x, t.y), __fsub_rn(d0.y, t.x));
 }

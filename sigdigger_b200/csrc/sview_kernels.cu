@@ -445,7 +445,7 @@ cudaError_t sdb_launch_psd_shift_db(cudaStream_t s, const float *lin, float *db,
   const size_t total = n_frames * n;
   if (total == 0) return cudaSuccess;
   size_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;        // 16 CTAs on each of an H100's 132 SMs, grid-stride beyond
   k_psd_shift_db<<<(unsigned) blocks, 256, 0, s>>>(lin, db, total, n);
   return cudaGetLastError();
 }

@@ -528,7 +528,7 @@ cudaError_t sdb_launch_sym_pack(cudaStream_t stream, const uint32_t *counts, uns
 {
   if (chains == 0) return cudaSuccess;
   k_sym_offsets<<<1, 1024, 0, stream>>>(counts, chains, offsets);
-  const unsigned grid = (unsigned) (chains < 148 * 16 ? chains : 148 * 16);
+  const unsigned grid = (unsigned) (chains < 132 * 16 ? chains : 132 * 16);   // 16 CTAs on each of an H100's 132 SMs
   k_sym_pack<<<grid, 128, 0, stream>>>(counts, offsets, chains, soft, hard, cap, (float4 *) out_soft, (uint4 *) out_hard,
                                        cap_total);
   if (launch_counter) *launch_counter += 2;

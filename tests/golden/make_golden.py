@@ -277,7 +277,245 @@ def pins():
     return out
 
 
+def sview_cases():
+    """SpectrumView runs of tests/test_ref.py -> [(fmin, fmax, fft_bandwidth, feeds)]; the third re-feeds the first"""
+    fmin, fmax, fftbw, psize, feeds = sview_case()
+    rng = np.random.default_rng(3)
+    fmin2, fmax2 = 1.0e9, 1.0e9 + 65536 * 1000.0 * 40
+    feeds2 = [((rng.random(512).astype(np.float32) * 10 - 80), fmin2 + (5 + 37.3 * h) * 40e3, 30e3) for h in range(200)]
+    return [(fmin, fmax, fftbw, feeds), (fmin2, fmax2, feeds2[0][2], feeds2), (fmin - 10e6, fmax + 25e6, fftbw, None)]
+
+
+def ref_task_input(n, seed):
+    x, _ = synth.multi_carrier(n, 1.0, [("qpsk", 0.01, 0.1, -6.0, {})], noise_db=-40.0, seed=seed)
+    return np.ascontiguousarray(x, np.complex64)
+
+
+TV_CASES = ((False, 40), (True, 61))
+SNR_CASES = ((1, 256), (2, 256), (3, 400))
+CARRIER_CASES = ((5000, 0.0371, 0.0), (16384, -0.212, 0.0), (3000, 0.11, 0.05), (9000, -0.4, 0.02))
+
+
+def snr_histograms(bps, length, rng):
+    k = 1 << bps
+    centres = (rng.integers(0, k, 200000) + 0.5) / k
+    v = (centres + 0.03 * rng.standard_normal(200000)) % 1.0
+    return np.bincount((v * length).astype(int) % length, minlength=length).astype(np.uint32)
+
+
+def carrier_input(n, f0, rng):
+    t = np.arange(n)
+    return (np.exp(2j * np.pi * f0 * t) * (1 + 0.3 * np.cos(2 * np.pi * 0.001 * t))
+            + 0.05 * (rng.standard_normal(n) + 1j * rng.standard_normal(n)) + 0.5).astype(np.complex64)
+
+
+def compiled_reference():
+    """Outputs of the reference's sources compiled into oracle/_ref/ (`make -C oracle ref`) on the inputs of
+    tests/test_ref.py: SHA-256 of the bytes where that test compares bit for bit, arrays otherwise."""
+    import ctypes as C
+    import test_oracle_tv as T
+    L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libsdref.so"))
+    L2 = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libsdref_suscan.so"))
+    L.ref_sview_new.restype = C.c_void_p
+    L.ref_sview_read.restype = C.c_uint
+    L.ref_sview_set_range.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_float]
+    L.ref_sview_feed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulong, C.c_double, C.c_int]
+    L.ref_sview_feed_view.argtypes = [C.c_void_p, C.c_void_p]
+    L.ref_sview_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.ref_wave_sampler.restype = C.c_long
+    L.ref_wave_sampler.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
+                                   C.c_float, C.c_float, C.c_float, C.c_float, C.c_size_t, C.c_double, C.c_void_p,
+                                   C.c_void_p, C.c_size_t]
+    L.ref_quad_demod.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    L.ref_delayed_conj.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_ulong]
+    L.ref_averager.argtypes = [C.c_void_p, C.c_uint, C.c_uint, C.c_float, C.c_void_p]
+    out = {}
+
+    views = []
+    for i, (fmin, fmax, fftbw, feeds) in enumerate(sview_cases()):
+        v = C.c_void_p(L.ref_sview_new())
+        L.ref_sview_set_range(v, C.c_double(fmin), C.c_double(fmax), C.c_double(fftbw), C.c_float(0.5))
+        if feeds is None:
+            L.ref_sview_feed_view(v, views[0])
+        for psd, fc, bw in feeds or ():
+            p = np.ascontiguousarray(psd, np.float32)
+            L.ref_sview_feed(v, p.ctypes.data, None, C.c_ulong(len(p)), C.c_double(fc), 1)
+        views.append(v)
+        a = [np.zeros(65536, np.float32) for _ in range(3)]
+        n = L.ref_sview_read(v, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data)
+        out["sview%d_size" % i] = np.int64(n)
+        out["sview%d_sha" % i] = np.array([sha(q[:n]) for q in a])
+
+    c = timewindow_case()
+    x = c["tone"][:5000]
+    y = np.zeros_like(x)
+    L.ref_quad_demod(x.ctypes.data, y.ctypes.data, C.c_size_t(len(x)))
+    out["quad_demod"] = y
+    for delay in (7, 500):
+        x = c["tone"][:3000]
+        y = np.zeros_like(x)
+        L.ref_delayed_conj(x.ctypes.data, y.ctypes.data, C.c_size_t(len(x)), C.c_ulong(delay))
+        out["delayed_conj_%d" % delay] = y
+    for space, sig in (("amplitude", "ask"), ("phase", "psk"), ("frequency", "psk")):
+        x = np.ascontiguousarray(c[sig][:6000])
+        y = np.zeros(1024, np.complex64)
+        n = L.ref_wave_sampler(x.ctypes.data, C.c_size_t(len(x)), 0, O.SPACE[space], C.c_double(1.0), C.c_double(0.1),
+                               C.c_double(0.1), 0, C.c_float(0), C.c_float(0), C.c_float(1), C.c_float(0), C.c_size_t(5),
+                               C.c_double(487.3), y.ctypes.data, None, C.c_size_t(1024))
+        out["manual_" + space] = y[:n].copy()
+    for i, (sig, space, amp, thr, zc, bnor) in enumerate(ZC_CASES):
+        x = np.ascontiguousarray(c[sig])
+        sym = np.zeros(len(x), np.uint8)
+        n = L.ref_wave_sampler(x.ctypes.data, C.c_size_t(len(x)), 2, O.SPACE[space], C.c_double(1.0), C.c_double(bnor),
+                               C.c_double(0.1), int(amp), C.c_float(thr.real), C.c_float(thr.imag), C.c_float(np.real(zc)),
+                               C.c_float(np.imag(zc)), C.c_size_t(0), C.c_double(100.0), None, sym.ctypes.data,
+                               C.c_size_t(len(x)))
+        out["zero_crossing_%d" % i] = sym[:n].copy()
+    x = np.ascontiguousarray(c["psk"])
+    y = np.zeros(len(x), np.complex64)
+    n = L.ref_wave_sampler(x.ctypes.data, C.c_size_t(len(x)), 1, O.SPACE["frequency"], C.c_double(1.0),
+                           C.c_double(1.0 / 12), C.c_double(0.2), 0, C.c_float(0), C.c_float(0), C.c_float(1), C.c_float(0),
+                           C.c_size_t(0), C.c_double(100.0), y.ctypes.data, None, C.c_size_t(len(x)))
+    out["gardner_sha"] = np.array(sha(y[:n]))
+
+    frames = averager_frames()
+    for alpha in (0.25, 1.0):
+        y = np.zeros(4096, np.float32)
+        L.ref_averager(frames.ctypes.data, 7, 4096, C.c_float(alpha), y.ctypes.data)
+        out["averager_%g_sha" % alpha] = np.array(sha(y))
+
+    L.ref_tv_worker.restype = C.c_long
+    L.ref_tv_worker.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                C.c_void_p]
+    for interlace, lines in TV_CASES:
+        x, _, _ = T.toy_signal(lines, interlace, frames=10)
+        sp = T.toy_params(lines, interlace, 4, cls=T.ShimTvParams)
+        W, H, cap, block = int(np.floor(T.LINE)), lines, 16, 7000
+        y = np.zeros((cap, H, W), np.float32)
+        w, h = C.c_int(), C.c_int()
+        got = L.ref_tv_worker(C.byref(sp), x.ctypes.data, x.size, block, y.ctypes.data, cap, C.byref(w), C.byref(h))
+        out["tv_%d_%d" % (interlace, lines)] = np.array([got, w.value, h.value], np.int64)
+        out["tv_%d_%d_sha" % (interlace, lines)] = np.array(sha(y))
+
+    L2.ref_suscan_psd_message.restype = C.c_long
+    L2.ref_suscan_psd_message.argtypes = [C.c_void_p, C.c_ulong, C.c_double, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p]
+    lin = psd_message_input()
+    y = np.zeros(len(lin), np.float32)
+    fc, rate = C.c_double(), C.c_uint()
+    n = L2.ref_suscan_psd_message(lin.ctypes.data, len(lin), 433.92e6, 2000000, y.ctypes.data, C.byref(fc), C.byref(rate))
+    out["psd_message"] = y[:n].copy()
+    out["psd_message_meta"] = np.array([fc.value, rate.value])
+    # Suscan/MQ.cpp, SamplesMessage, StatusMessage over libsuscan.so
+    L2.ref_suscan_mq_samples.restype = C.c_long
+    L2.ref_suscan_mq_samples.argtypes = [C.c_void_p, C.c_ulong, C.c_uint, C.c_void_p, C.c_void_p]
+    L2.ref_suscan_status_message.argtypes = [C.c_int, C.c_char_p, C.c_char_p, C.c_size_t]
+    x = mq_input()
+    y = np.zeros_like(x)
+    iid = C.c_uint()
+    n = L2.ref_suscan_mq_samples(x.ctypes.data, x.size, 0xBEEF, y.ctypes.data, C.byref(iid))
+    out["mq_samples"] = np.array([n, iid.value], np.int64)
+    out["mq_samples_sha"] = np.array(sha(y))
+    status = []
+    for code, text in MQ_STATUS_CASES:
+        buf = C.create_string_buffer(64)
+        status += [str(L2.ref_suscan_status_message(code, text, buf, 64)), buf.value.decode()]
+    out["status_messages"] = np.array(status)
+
+    n = 2 * 4096 + 777
+    x = ref_task_input(n, 5)
+    y = np.zeros(n, np.complex64)
+    for kind in (1, 2, 3):
+        L.ref_task_costas.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_float, C.c_float, C.c_int]
+        assert L.ref_task_costas(x.ctypes.data, y.ctypes.data, n, C.c_float(10.0), C.c_float(2e-3), kind) == 0
+        out["task_costas_%d_sha" % kind] = np.array(sha(y))
+    L.ref_task_pll.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_float]
+    assert L.ref_task_pll(x.ctypes.data, y.ctypes.data, n, C.c_float(5e-3)) == 0
+    out["task_pll_sha"] = np.array(sha(y))
+    L.ref_task_agc.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_float]
+    assert L.ref_task_agc(x.ctypes.data, y.ctypes.data, n, C.c_float(20.0)) == 0
+    out["task_agc_sha"] = np.array(sha(y))
+    L.ref_task_xlate.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_float, C.c_float]
+    assert L.ref_task_xlate(x.ctypes.data, y.ctypes.data, n, C.c_float(0.0123), C.c_float(0.5)) == 0
+    out["task_xlate_sha"] = np.array(sha(y))
+
+    L.ref_task_histogram.restype = C.c_long
+    L.ref_task_histogram.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t]
+    n = 3 * 4096 + 55
+    x = ref_task_input(n, 8)
+    for space in (0, 1, 2):
+        y = np.zeros(n, np.float32)
+        k = L.ref_task_histogram(x.ctypes.data, n, space, y.ctypes.data, n)
+        out["histogram_%d" % space] = y[:k].copy()
+
+    L.ref_snr_estimator.argtypes = [C.c_uint, C.c_float, C.c_float, C.c_void_p, C.c_uint, C.c_uint, C.c_void_p,
+                                    C.c_void_p, C.c_void_p]
+    rng = np.random.default_rng(4)
+    for bps, length in SNR_CASES:
+        h = snr_histograms(bps, length, rng)
+        feeds = 6
+        hs = np.ascontiguousarray(np.tile(h, (feeds, 1)))
+        sig, snr, model = np.zeros(feeds, np.float32), np.zeros(feeds, np.float32), np.zeros(length, np.float32)
+        assert L.ref_snr_estimator(bps, C.c_float(0.5), C.c_float(0.0), hs.ctypes.data, length, feeds,
+                                   sig.ctypes.data, snr.ctypes.data, model.ctypes.data) == length
+        out["snr_%d_%d" % (bps, length)] = np.concatenate([sig, snr, model])
+
+    L.ref_carrier_detect.restype = C.c_float
+    L.ref_carrier_detect.argtypes = [C.c_void_p, C.c_size_t, C.c_double, C.c_double]
+    rng = np.random.default_rng(12)
+    peaks = []
+    for n, f0, notch in CARRIER_CASES:
+        x = carrier_input(n, f0, rng)
+        peaks.append(L.ref_carrier_detect(x.ctypes.data, n, 0.01, notch))
+    out["carrier_detect"] = np.array(peaks, np.float32)
+    return out
+
+
+ZC_CASES = [("ask", "amplitude", True, 0.6 + 0.1j, 1 + 0j, 1.0 / 12),
+            ("ask", "amplitude", False, 0.55 + 0.2j, np.exp(-0.3j), 1.0 / 12),
+            ("psk", "phase", False, 0j, np.exp(0.1j), 1.0 / 12), ("ask", "amplitude", True, 0.6 + 0.1j, 1 + 0j, 1.0)]
+LPF_N, LPF_SEED, LPF_BW = 5 * 4096 + 300, 9, 0.2
+
+
+MQ_STATUS_CASES = ((-1, b"source failed to start"), (0, None))
+
+
+def mq_input():
+    rng = np.random.default_rng(22)
+    return (rng.standard_normal(1000) + 1j * rng.standard_normal(1000)).astype(np.complex64)
+
+
+def averager_frames():
+    return np.random.default_rng(9).random((7, 4096)).astype(np.float32) * 40 - 100
+
+
+def psd_message_input():
+    rng = np.random.default_rng(21)
+    n = 8192
+    lin = (rng.standard_normal(n) ** 2 * 10.0 ** rng.uniform(-9, 1, n)).astype(np.float32)
+    lin[:4] = [0.0, 1e-12, 1.0, 123.5]
+    return lin
+
+
+def compiled_reference_gpu():
+    """Tasks/LPFTask.cpp of oracle/_ref/ over the GPU tuner of <sigutils/specttuner.h>: SHA-256 of its output."""
+    import ctypes as C
+    R = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libsdref.so"))
+    R.ref_task_lpf.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_float]
+    x = ref_task_input(LPF_N, LPF_SEED)
+    y = np.zeros(LPF_N, np.complex64)
+    assert R.ref_task_lpf(x.ctypes.data, y.ctypes.data, LPF_N, C.c_float(LPF_BW)) == 0
+    return {"task_lpf_sha": sha(y)}
+
+
 def main():
+    if "--compiled-reference" in sys.argv:
+        np.savez_compressed(os.path.join(HERE, "ref_compiled.npz"), **compiled_reference())
+        print("wrote ref_compiled.npz")
+        return
+    if "--compiled-reference-gpu" in sys.argv:
+        json.dump(compiled_reference_gpu(), open(os.path.join(HERE, "ref_compiled_gpu.json"), "w"), indent=1)
+        print("wrote ref_compiled_gpu.json")
+        return
     fmin, fmax, fftbw, psize, feeds = sview_case()
     psd, acc, cnt, size = _sview_literal(fmin, fmax, feeds)
     np.savez_compressed(os.path.join(HERE, "ref_spectrumview.npz"), psd=psd, count=cnt, size=size)

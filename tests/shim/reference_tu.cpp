@@ -10,7 +10,10 @@
 //   * AnalyzerSession -- Suscan/Analyzer.cpp:63-115 (reader loop, std::thread in place of QThread), :459-495
 //                        (open_ex / set_inspector_config / set_inspector_id), :601-638 (construction with a
 //                        caller-owned suscan_mq, halt, join, destroy) and the OPEN -> SET_ID handshake of
-//                        Suscan/AnalyzerRequestTracker.cpp:138-157.
+//                        Suscan/AnalyzerRequestTracker.cpp:138-157;
+//   * mq / messages   -- Suscan/MQ.cpp:28-43 (caller-owned queue: init, read, finalize), the shared_ptr deleter of
+//                        Suscan/Message.cpp:46 and the getters of Suscan/Messages/SamplesMessage.cpp and
+//                        StatusMessage.cpp (a status message is disposed as SUSCAN_ANALYZER_MESSAGE_TYPE_INTERNAL).
 // Every sigutils / suscan call below is written as the reference writes it; only the Qt scaffolding is gone.
 #include <sigutils/types.h>
 #include <sigutils/sampling.h>
@@ -26,6 +29,7 @@
 
 #include <algorithm>
 #include <condition_variable>
+#include <memory>
 #include <mutex>
 #include <stdexcept>
 #include <string>
@@ -485,4 +489,46 @@ extern "C" long tu_analyzer_session(const SUCOMPLEX *iq, size_t n, unsigned samp
     suscan_source_config_destroy(config);
     return result;
   } catch (std::exception &) { return -1; }
+}
+
+// A SAMPLES batch posted with suscan_mq_write comes back through the caller-owned queue and is released by the
+// message deleter.  Returns the sample count (< 0: failure code).
+extern "C" long tu_mq_samples(const SUCOMPLEX *samples, unsigned long n, unsigned inspector_id, SUCOMPLEX *out,
+                              unsigned *id_out)
+{
+  struct suscan_mq mq;
+  if (!suscan_mq_init(&mq)) return -3;
+  auto *m = (struct suscan_analyzer_sample_batch_msg *) calloc(1, sizeof(struct suscan_analyzer_sample_batch_msg));
+  m->inspector_id = inspector_id; m->sample_count = n;
+  m->samples = (SUCOMPLEX *) malloc(n * sizeof(SUCOMPLEX));
+  memcpy(m->samples, samples, n * sizeof(SUCOMPLEX));
+  long ret = -1;
+  if (!suscan_mq_write(&mq, SUSCAN_ANALYZER_MESSAGE_TYPE_SAMPLES, m)) {
+    suscan_analyzer_dispose_message(SUSCAN_ANALYZER_MESSAGE_TYPE_SAMPLES, m);
+  } else {
+    uint32_t type = 0;
+    void *p = suscan_mq_read(&mq, &type);
+    std::shared_ptr<void> msg(p, [=](void *ptr) { suscan_analyzer_dispose_message(type, ptr); });
+    if (type != SUSCAN_ANALYZER_MESSAGE_TYPE_SAMPLES || p != m) {
+      ret = -2;
+    } else {
+      auto *s = static_cast<struct suscan_analyzer_sample_batch_msg *>(p);
+      *id_out = s->inspector_id;
+      memcpy(out, s->samples, s->sample_count * sizeof(SUCOMPLEX));
+      ret = (long) s->sample_count;
+    }
+  }
+  suscan_mq_finalize(&mq);
+  return ret;
+}
+
+// StatusMessage: code and text (empty for a NULL err_msg), disposed by the deleter.  Returns the code.
+extern "C" int tu_status_message(int code, const char *text, char *text_out, size_t cap)
+{
+  auto *m = (struct suscan_analyzer_status_msg *) calloc(1, sizeof(struct suscan_analyzer_status_msg));
+  m->code = code; m->err_msg = text ? strdup(text) : nullptr;
+  std::shared_ptr<void> msg(m, [](void *ptr) { suscan_analyzer_dispose_message(SUSCAN_ANALYZER_MESSAGE_TYPE_INTERNAL, ptr); });
+  const std::string s = m->err_msg == nullptr ? "" : m->err_msg;
+  strncpy(text_out, s.c_str(), cap - 1); text_out[cap - 1] = 0;
+  return m->code;
 }

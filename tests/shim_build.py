@@ -30,6 +30,9 @@ def reference_tu():
         L.tu_agc_task.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_float]
         L.tu_xlate_task.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_float, C.c_float, C.c_int]
         L.tu_lpf_task.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_float]
+        L.tu_mq_samples.restype = C.c_long
+        L.tu_mq_samples.argtypes = [C.c_void_p, C.c_ulong, C.c_uint, C.c_void_p, C.c_void_p]
+        L.tu_status_message.argtypes = [C.c_int, C.c_char_p, C.c_char_p, C.c_size_t]
         L.tu_tv_worker.restype = C.c_long
         L.tu_tv_worker.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                    C.c_void_p]

@@ -1,4 +1,4 @@
-"""-m gpu: the analog-TV processor batch on the B200 (k_tv_feed, one warp per processor) against the oracle, bit for
+"""-m gpu: the analog-TV processor batch on the GPU (k_tv_feed, one warp per processor) against the oracle, bit for
 bit: frame counts, every frame still in the ring, the picture in progress, the loop estimates; block-size independence;
 the TV tab's input conversion.  Through the C-ABI (sdb_tv_processor_*)."""
 import ctypes as C

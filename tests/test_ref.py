@@ -1,10 +1,11 @@
 """CPU: the oracle pinned to the REFERENCE ITSELF where the reference contains the arithmetic.  oracle/_ref/libsdref.so
-is built by `make -C oracle ref` from the sources under /root/reference where they lie (Panoramic/Scanner.cpp:1-293,
+is built by `make -C oracle ref` from the reference's own sources where they lie (Panoramic/Scanner.cpp:1-293,
 Tasks/QuadDemodTask.cpp, Tasks/DelayedConjTask.cpp, Tasks/WaveSampler.cpp, Misc/Averager.cpp,
 Default/GenericInspector/TVProcessorWorker.cpp) behind no-behaviour Qt
 stubs (oracle/ref_shim/, oracle/ref_glue.cpp); nothing of the reference is copied.  The restatements of oracle/*.c are
 compared with it here; the Python transcriptions of tests/golden/make_golden.py stay as a second opinion.
-Skipped when the library was not built (no /root/reference and no prebuilt file)."""
+What the compiled reference computed on these inputs is stored in tests/golden/ref_compiled.npz (as SHA-256 of the
+bytes where the comparison is bit for bit; `python tests/golden/make_golden.py --compiled-reference` rewrites it)."""
 import ctypes as C
 import os
 import sys
@@ -13,44 +14,18 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "oracle", "_ref", "libsdref.so")
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+import make_golden as G     # noqa: E402
 
 
 @pytest.fixture(scope="module")
 def ref():
-    if not os.path.exists(REF) and os.path.isdir("/root/reference"):
-        import subprocess
-        subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "ref"], capture_output=True)
-    if not os.path.exists(REF):
-        pytest.skip("oracle/_ref/libsdref.so not built (needs /root/reference)")
-    L = C.CDLL(REF)
-    L.ref_sview_new.restype = C.c_void_p
-    L.ref_sview_read.restype = C.c_uint
-    L.ref_wave_sampler.restype = C.c_long
-    L.ref_wave_sampler.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
-                                   C.c_float, C.c_float, C.c_float, C.c_float, C.c_size_t, C.c_double, C.c_void_p,
-                                   C.c_void_p, C.c_size_t]
-    L.ref_sview_set_range.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_float]
-    L.ref_sview_feed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulong, C.c_double, C.c_int]
-    L.ref_sview_feed_view.argtypes = [C.c_void_p, C.c_void_p]
-    L.ref_sview_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.ref_quad_demod.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    L.ref_delayed_conj.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_ulong]
-    L.ref_averager.argtypes = [C.c_void_p, C.c_uint, C.c_uint, C.c_float, C.c_void_p]
-    return L
+    with np.load(os.path.join(ROOT, "tests", "golden", "ref_compiled.npz")) as z:
+        return {k: z[k] for k in z.files}
 
 
-def _sview_ref(L, fmin, fmax, feeds, rel_bw=0.5):
-    v = C.c_void_p(L.ref_sview_new())
-    L.ref_sview_set_range(v, C.c_double(fmin), C.c_double(fmax), C.c_double(feeds[0][2]), C.c_float(rel_bw))
-    for psd, fc, bw in feeds:
-        L.ref_sview_set_range  # (range fixed)
-        p = np.ascontiguousarray(psd, np.float32)
-        L.ref_sview_feed(v, p.ctypes.data, None, C.c_ulong(len(p)), C.c_double(fc), 1)
-    out = [np.zeros(65536, np.float32) for _ in range(3)]
-    n = L.ref_sview_read(v, out[0].ctypes.data, out[1].ctypes.data, out[2].ctypes.data)
-    return [o[:n].copy() for o in out], v
+def _bits(*arrays):
+    return [G.sha(a) for a in arrays]
 
 
 def _sview_oracle(oracle, fmin, fmax, feeds, rel_bw=0.5):
@@ -69,44 +44,30 @@ def _sview_oracle(oracle, fmin, fmax, feeds, rel_bw=0.5):
 
 def test_spectrumview_restatement_equals_the_compiled_reference(ref, oracle):
     """linear mode with revisits (forgetting rule, gap filling), histogram mode, and view-to-view feed"""
-    import make_golden as G
-    fmin, fmax, fftbw, psize, feeds = G.sview_case()
+    (fmin, fmax, fftbw, feeds), (fmin2, fmax2, _, feeds2), (fmin3, fmax3, _, _) = G.sview_cases()
     got, ov = _sview_oracle(oracle, fmin, fmax, feeds)
-    want, rv = _sview_ref(ref, fmin, fmax, feeds)
-    for a, b in zip(got, want):
-        assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+    assert len(got[0]) == ref["sview0_size"] and _bits(*got) == list(ref["sview0_sha"])
     # histogram mode: hops narrower than two destination bins
-    rng = np.random.default_rng(3)
-    fmin2, fmax2 = 1.0e9, 1.0e9 + 65536 * 1000.0 * 40
-    feeds2 = [((rng.random(512).astype(np.float32) * 10 - 80), fmin2 + (5 + 37.3 * h) * 40e3, 30e3) for h in range(200)]
     got, ov2 = _sview_oracle(oracle, fmin2, fmax2, feeds2)
-    want, rv2 = _sview_ref(ref, fmin2, fmax2, feeds2)
-    for a, b in zip(got, want):
-        assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+    assert len(got[0]) == ref["sview1_size"] and _bits(*got) == list(ref["sview1_sha"])
     # SpectrumView::feed(SpectrumView const &): zoom path of Scanner::setViewRange
     L = oracle.lib()
     wide_o = oracle.SpectrumView(); assert L.sdo_sview_init(C.byref(wide_o)) == 0
-    L.sdo_sview_set_range(C.byref(wide_o), fmin - 10e6, fmax + 25e6)
+    L.sdo_sview_set_range(C.byref(wide_o), fmin3, fmax3)
     wide_o.fft_bandwidth = fftbw; wide_o.fft_rel_bw = 0.5
     L.sdo_sview_feed_view(C.byref(wide_o), C.byref(ov))
     L.sdo_sview_interpolate(C.byref(wide_o))
-    wide_r = C.c_void_p(ref.ref_sview_new())
-    ref.ref_sview_set_range(wide_r, C.c_double(fmin - 10e6), C.c_double(fmax + 25e6), C.c_double(fftbw), C.c_float(0.5))
-    ref.ref_sview_feed_view(wide_r, rv)
-    out = [np.zeros(65536, np.float32) for _ in range(3)]
-    n = ref.ref_sview_read(wide_r, out[0].ctypes.data, out[1].ctypes.data, out[2].ctypes.data)
-    assert n == wide_o.spectrum_size
-    for a, q in zip(out, (wide_o.psd, wide_o.psd_accum, wide_o.psd_count)):
-        assert np.array_equal(a[:n].view(np.uint32), np.ctypeslib.as_array(q, shape=(65536,))[:n].view(np.uint32))
+    n = wide_o.spectrum_size
+    assert n == ref["sview2_size"]
+    assert _bits(*(np.ctypeslib.as_array(q, shape=(65536,))[:n] for q in (wide_o.psd, wide_o.psd_accum,
+                                                                         wide_o.psd_count))) == list(ref["sview2_sha"])
 
 
 def test_timewindow_tasks_equal_the_compiled_reference(ref, oracle):
-    import make_golden as G
     c = G.timewindow_case()
     # QuadDemodTask: the reference calls std::arg (libm), the oracle its SPEC M atan2: equal to rounding
     x = c["tone"][:5000]
-    y = np.zeros_like(x)
-    ref.ref_quad_demod(x.ctypes.data, y.ctypes.data, C.c_size_t(len(x)))
+    y = ref["quad_demod"]
     o = np.empty_like(x)
     prev = oracle.Cpx(0, 0); primed = C.c_int(0)
     oracle.lib().sdo_quad_demod(oracle.ptr(x), oracle.ptr(o), len(x), C.byref(prev), C.byref(primed))
@@ -114,29 +75,22 @@ def test_timewindow_tasks_equal_the_compiled_reference(ref, oracle):
     # DelayedConjTask: to one ulp of cabsf (libm's hypot vs sqrtf of the sum of squares)
     for delay in (7, 500):
         x = c["tone"][:3000]
-        y = np.zeros_like(x)
-        ref.ref_delayed_conj(x.ctypes.data, y.ctypes.data, C.c_size_t(len(x)), C.c_ulong(delay))
+        y = ref["delayed_conj_%d" % delay]
         o = oracle.delayed_conj(x, delay)
         assert np.max(np.abs(y - o)) <= 4e-7 * np.max(np.abs(y))
     # WaveSampler MANUAL in the three decision spaces: soft symbols bit for bit
     for space, sig in (("amplitude", "ask"), ("phase", "psk"), ("frequency", "psk")):
         x = np.ascontiguousarray(c[sig][:6000])
-        out = np.zeros(1024, np.complex64)
-        n = ref.ref_wave_sampler(x.ctypes.data, C.c_size_t(len(x)), 0, oracle.SPACE[space], C.c_double(1.0), C.c_double(0.1),
-                                 C.c_double(0.1), 0, C.c_float(0), C.c_float(0), C.c_float(1), C.c_float(0), C.c_size_t(5),
-                                 C.c_double(487.3), out.ctypes.data, None, C.c_size_t(1024))
+        out = ref["manual_" + space]
+        n = len(out)
         o = oracle.sample_manual(x, space, 487.3, 5)
         assert n == len(o) == 487
         assert np.array_equal(out[:n].view(np.uint32), o.view(np.uint32)), space
     # WaveSampler ZERO_CROSSING: recovered bit streams bit for bit
-    cases = [("ask", "amplitude", True, 0.6 + 0.1j, 1 + 0j, 1.0 / 12), ("ask", "amplitude", False, 0.55 + 0.2j, np.exp(-0.3j), 1.0 / 12),
-             ("psk", "phase", False, 0j, np.exp(0.1j), 1.0 / 12), ("ask", "amplitude", True, 0.6 + 0.1j, 1 + 0j, 1.0)]
-    for sig, space, amp, thr, zc, bnor in cases:
+    for i, (sig, space, amp, thr, zc, bnor) in enumerate(G.ZC_CASES):
         x = np.ascontiguousarray(c[sig])
-        sym = np.zeros(len(x), np.uint8)
-        n = ref.ref_wave_sampler(x.ctypes.data, C.c_size_t(len(x)), 2, oracle.SPACE[space], C.c_double(1.0), C.c_double(bnor),
-                                 C.c_double(0.1), int(amp), C.c_float(thr.real), C.c_float(thr.imag), C.c_float(np.real(zc)),
-                                 C.c_float(np.imag(zc)), C.c_size_t(0), C.c_double(100.0), None, sym.ctypes.data, C.c_size_t(len(x)))
+        sym = ref["zero_crossing_%d" % i]
+        n = len(sym)
         o, k = oracle.sample_zero_crossing(x, space, bnor, amp, thr, zc)
         assert n == k and np.array_equal(sym[:n], o), (sig, space, amp)
 
@@ -144,23 +98,15 @@ def test_timewindow_tasks_equal_the_compiled_reference(ref, oracle):
 def test_gardner_sampler_of_the_reference_over_the_clock_detector_shim(ref, oracle):
     """Tasks/WaveSampler.cpp sampleGardner() compiled from the reference, running on THIS repo's su_clock_detector
     (libsigutils.so): equal to the oracle's Gardner detector fed the same way."""
-    import make_golden as G
     import shim_build as SB
     x = np.ascontiguousarray(G.timewindow_case()["psk"])
-    out = np.zeros(len(x), np.complex64)
-    n = ref.ref_wave_sampler(x.ctypes.data, C.c_size_t(len(x)), 1, oracle.SPACE["frequency"], C.c_double(1.0),
-                             C.c_double(1.0 / 12), C.c_double(0.2), 0, C.c_float(0), C.c_float(0), C.c_float(1), C.c_float(0),
-                             C.c_size_t(0), C.c_double(100.0), out.ctypes.data, None, C.c_size_t(len(x)))
     want = SB.oracle_gardner_frequency(oracle, x, 0.2, 1.0 / 12)
-    assert n == len(want) and np.array_equal(out[:n].view(np.uint32), want.view(np.uint32))
+    assert G.sha(want) == ref["gardner_sha"]
 
 
 def test_averager_restatement_equals_the_compiled_reference(ref, oracle):
-    rng = np.random.default_rng(9)
-    frames = (rng.random((7, 4096)).astype(np.float32) * 40 - 100)
+    frames = G.averager_frames()
     for alpha in (0.25, 1.0):
-        out = np.zeros(4096, np.float32)
-        ref.ref_averager(frames.ctypes.data, 7, 4096, C.c_float(alpha), out.ctypes.data)
         last = frames[0].copy()
         L = oracle.lib()
         for f in range(1, 7):
@@ -168,7 +114,7 @@ def test_averager_restatement_equals_the_compiled_reference(ref, oracle):
                 L.sdo_averager_feed(oracle.ptr(last), oracle.ptr(np.ascontiguousarray(frames[f])), 4096, C.c_float(alpha))
             else:
                 last = frames[f].copy()
-        assert np.array_equal(out.view(np.uint32), last.view(np.uint32)), alpha
+        assert G.sha(last) == ref["averager_%g_sha" % alpha], alpha
 
 
 @pytest.mark.parametrize("interlace,lines", [(False, 40), (True, 61)])
@@ -178,20 +124,16 @@ def test_tv_worker_of_the_reference_over_the_tvproc_shim(ref, oracle, interlace,
     the frames it emits are, bit for bit, the oracle's (SPEC TV) and those of the reference-shaped TU."""
     import shim_build as SB
     import test_oracle_tv as T
-    ref.ref_tv_worker.restype = C.c_long
-    ref.ref_tv_worker.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
-                                  C.c_void_p]
     x, _, _ = T.toy_signal(lines, interlace, frames=10)
     sp = T.toy_params(lines, interlace, 4, cls=T.ShimTvParams)
     W, H, cap, block = int(np.floor(T.LINE)), lines, 16, 7000
     out = np.zeros((cap, H, W), np.float32)
     w, h = C.c_int(), C.c_int()
-    got = ref.ref_tv_worker(C.byref(sp), x.ctypes.data, x.size, block, out.ctypes.data, cap, C.byref(w), C.byref(h))
-    assert got >= 5 and (w.value, h.value) == (W, H)
-    out_tu = np.zeros_like(out)
-    assert SB.reference_tu().tu_tv_worker(C.byref(sp), x.ctypes.data, x.size, block, out_tu.ctypes.data, cap,
+    got, rw, rh = (int(v) for v in ref["tv_%d_%d" % (interlace, lines)])
+    assert got >= 5 and (rw, rh) == (W, H)
+    assert SB.reference_tu().tu_tv_worker(C.byref(sp), x.ctypes.data, x.size, block, out.ctypes.data, cap,
                                           C.byref(w), C.byref(h)) == got
-    assert np.array_equal(out.view(np.uint32), out_tu.view(np.uint32))
+    assert G.sha(out) == ref["tv_%d_%d_sha" % (interlace, lines)]
     t = T.OracleTv(T.toy_params(lines, interlace, 4))
     k = 0
     for p0 in range(0, x.size, block):
@@ -206,26 +148,7 @@ def test_tv_worker_of_the_reference_over_the_tvproc_shim(ref, oracle, interlace,
     t.close()
 
 
-REF2 = os.path.join(ROOT, "oracle", "_ref", "libsdref_suscan.so")
-
-
-@pytest.fixture(scope="module")
-def ref_suscan():
-    if not os.path.exists(REF2) and os.path.isdir("/root/reference"):
-        import subprocess
-        subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "ref"], capture_output=True)
-    if not os.path.exists(REF2):
-        pytest.skip("oracle/_ref/libsdref_suscan.so not built (needs /root/reference)")
-    L = C.CDLL(REF2)
-    L.ref_suscan_psd_message.restype = C.c_long
-    L.ref_suscan_psd_message.argtypes = [C.c_void_p, C.c_ulong, C.c_double, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.ref_suscan_mq_samples.restype = C.c_long
-    L.ref_suscan_mq_samples.argtypes = [C.c_void_p, C.c_ulong, C.c_uint, C.c_void_p, C.c_void_p]
-    L.ref_suscan_status_message.argtypes = [C.c_int, C.c_char_p, C.c_char_p, C.c_size_t]
-    return L
-
-
-def test_psd_message_of_the_reference_over_the_shim_headers(ref_suscan, oracle):
+def test_psd_message_of_the_reference_over_the_shim_headers(ref, oracle):
     """Suscan/Messages/PSDMessage.cpp + Suscan/Message.cpp COMPILED FROM THE REFERENCE against include/analyzer/msg.h:
     the constructor's fft-shift + SU_POWER_DB pass (:26-39) is the reference's own; the oracle's sdo_psd_shift_db
     (= the PSD kernels' SDB_FLAG_PSD_SHIFT_DB epilogue, bit for bit) is held to it -- the layout exactly, the values to
@@ -234,11 +157,8 @@ def test_psd_message_of_the_reference_over_the_shim_headers(ref_suscan, oracle):
     n = 8192
     lin = (rng.standard_normal(n) ** 2 * 10.0 ** rng.uniform(-9, 1, n)).astype(np.float32)
     lin[:4] = [0.0, 1e-12, 1.0, 123.5]
-    out = np.zeros(n, np.float32)
-    fc, rate = C.c_double(), C.c_uint()
-    assert ref_suscan.ref_suscan_psd_message(lin.ctypes.data, n, 433.92e6, 2000000, out.ctypes.data, C.byref(fc),
-                                             C.byref(rate)) == n
-    assert fc.value == 433920000.0 and rate.value == 2000000
+    out = ref["psd_message"]
+    assert len(out) == n and list(ref["psd_message_meta"]) == [433920000.0, 2000000]
     mine = lin.copy()
     oracle.lib().sdo_psd_shift_db(oracle.ptr(mine), n)
     assert np.all(np.isfinite(out)) and out.min() >= -80.0 - 1e-3          # the 1e-8 floor of SU_POWER_DB
@@ -247,20 +167,23 @@ def test_psd_message_of_the_reference_over_the_shim_headers(ref_suscan, oracle):
     assert np.max(np.abs(out - want)) < 2e-5
 
 
-def test_mq_and_message_wrappers_of_the_reference_over_libsuscan(ref_suscan):
+def test_mq_and_message_wrappers_of_the_reference_over_libsuscan(ref):
     """Suscan/MQ.cpp (caller-owned suscan_mq: init / read / finalize), SamplesMessage and StatusMessage over the shim
     library: payloads posted with suscan_mq_write come back through the reference's wrapper classes and are released by
-    their shared_ptr deleter (suscan_analyzer_dispose_message)."""
-    rng = np.random.default_rng(22)
-    x = (rng.standard_normal(1000) + 1j * rng.standard_normal(1000)).astype(np.complex64)
+    their shared_ptr deleter (suscan_analyzer_dispose_message): the same calls from the reference-shaped TU."""
+    import shim_build as SB
+    tu = SB.reference_tu()
+    x = G.mq_input()
     out = np.zeros_like(x)
     iid = C.c_uint()
-    assert ref_suscan.ref_suscan_mq_samples(x.ctypes.data, x.size, 0xBEEF, out.ctypes.data, C.byref(iid)) == x.size
+    assert tu.tu_mq_samples(x.ctypes.data, x.size, 0xBEEF, out.ctypes.data, C.byref(iid)) == x.size
     assert iid.value == 0xBEEF and np.array_equal(out, x)
-    buf = C.create_string_buffer(64)
-    assert ref_suscan.ref_suscan_status_message(-1, b"source failed to start", buf, 64) == -1
-    assert buf.value == b"source failed to start"
-    assert ref_suscan.ref_suscan_status_message(0, None, buf, 64) == 0 and buf.value == b""
+    assert list(ref["mq_samples"]) == [x.size, 0xBEEF] and G.sha(out) == ref["mq_samples_sha"]
+    status = []
+    for code, text in G.MQ_STATUS_CASES:
+        buf = C.create_string_buffer(64)
+        status += [str(tu.tu_status_message(code, text, buf, 64)), buf.value.decode()]
+    assert status == list(ref["status_messages"])
 
 
 def _qpsk(n, seed=5):
@@ -277,37 +200,25 @@ def test_tasks_of_the_reference_over_the_sigutils_shim(ref, oracle):
     import shim_build as SB
     n = 2 * 4096 + 777
     x = _qpsk(n)
-    y = np.zeros(n, np.complex64)
-    for fn, args in (("ref_task_costas", [C.c_float(10.0), C.c_float(2e-3), 2]),
-                     ("ref_task_pll", [C.c_float(5e-3)]), ("ref_task_agc", [C.c_float(20.0)]),
-                     ("ref_task_xlate", [C.c_float(0.0123), C.c_float(0.5)])):
-        getattr(ref, fn).argtypes = [C.c_void_p, C.c_void_p, C.c_size_t] + [type(a) if not isinstance(a, int) else C.c_int
-                                                                            for a in args]
     for kind in (1, 2, 3):
-        assert ref.ref_task_costas(x.ctypes.data, y.ctypes.data, n, C.c_float(10.0), C.c_float(2e-3), kind) == 0
-        assert np.array_equal(y.view(np.uint32), SB.oracle_costas(oracle, x, kind, 0.1, 2e-3).view(np.uint32))
-    assert ref.ref_task_pll(x.ctypes.data, y.ctypes.data, n, C.c_float(5e-3)) == 0
-    assert np.array_equal(y.view(np.uint32), SB.oracle_pll(oracle, x, 5e-3).view(np.uint32))
-    assert ref.ref_task_agc(x.ctypes.data, y.ctypes.data, n, C.c_float(20.0)) == 0
-    assert np.array_equal(y.view(np.uint32), SB.oracle_agc(oracle, x, 20.0).view(np.uint32))
-    assert ref.ref_task_xlate(x.ctypes.data, y.ctypes.data, n, C.c_float(0.0123), C.c_float(0.5)) == 0
-    assert np.array_equal(y.view(np.uint32), SB.oracle_xlate(oracle, x, 0.0123, 0.5).view(np.uint32))
+        assert G.sha(SB.oracle_costas(oracle, x, kind, 0.1, 2e-3)) == ref["task_costas_%d_sha" % kind]
+    assert G.sha(SB.oracle_pll(oracle, x, 5e-3)) == ref["task_pll_sha"]
+    assert G.sha(SB.oracle_agc(oracle, x, 20.0)) == ref["task_agc_sha"]
+    assert G.sha(SB.oracle_xlate(oracle, x, 0.0123, 0.5)) == ref["task_xlate_sha"]
 
 
 def test_histogram_feeder_of_the_reference(ref, oracle):
     """Tasks/HistogramFeeder.cpp compiled from the reference against the oracle's restatement (SPEC Y.2): amplitude
     exactly; phase / frequency to one ulp of libm's cargf against the SPEC M atan2."""
-    ref.ref_task_histogram.restype = C.c_long
-    ref.ref_task_histogram.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t]
     L = oracle.lib()
     L.sdo_histogram_feed.restype = C.c_size_t
     L.sdo_histogram_feed.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]
     n = 3 * 4096 + 55
     x = _qpsk(n, seed=8)
     for space, tol in ((0, 0.0), (1, 4e-7), (2, 4e-7)):
-        got = np.zeros(n, np.float32)
+        got = ref["histogram_%d" % space]
         mine = np.zeros(n, np.float32)
-        k = ref.ref_task_histogram(x.ctypes.data, n, space, got.ctypes.data, n)
+        k = len(got)
         m = L.sdo_histogram_feed(x.ctypes.data, mine.ctypes.data, n, space)
         assert k == m == (n - 1 if space == 2 else n)
         if tol == 0.0:
@@ -321,8 +232,6 @@ def test_histogram_feeder_of_the_reference(ref, oracle):
 def test_snr_estimator_restatement_tracks_the_compiled_reference(ref, oracle):
     """Misc/SNREstimator.cpp compiled from the reference against the oracle's restatement (SPEC Y.7): same trajectory
     of sigma over successive feeds and the same model histogram, to the difference between libm's exp and SPEC M's."""
-    ref.ref_snr_estimator.argtypes = [C.c_uint, C.c_float, C.c_float, C.c_void_p, C.c_uint, C.c_uint, C.c_void_p,
-                                      C.c_void_p, C.c_void_p]
     rng = np.random.default_rng(4)
     for bps, length in ((1, 256), (2, 256), (3, 400)):
         k = 1 << bps
@@ -330,10 +239,9 @@ def test_snr_estimator_restatement_tracks_the_compiled_reference(ref, oracle):
         v = (centres + 0.03 * rng.standard_normal(200000)) % 1.0
         h = np.bincount((v * length).astype(int) % length, minlength=length).astype(np.uint32)
         feeds = 6
-        hs = np.ascontiguousarray(np.tile(h, (feeds, 1)))
-        sig, snr, model = np.zeros(feeds, np.float32), np.zeros(feeds, np.float32), np.zeros(length, np.float32)
-        assert ref.ref_snr_estimator(bps, C.c_float(0.5), C.c_float(0.0), hs.ctypes.data, length, feeds,
-                                     sig.ctypes.data, snr.ctypes.data, model.ctypes.data) == length
+        r = ref["snr_%d_%d" % (bps, length)]
+        sig, snr, model = r[:feeds], r[feeds:2 * feeds], r[2 * feeds:]
+        assert len(model) == length
         e = oracle.SnrEstimator(bps, length, alpha=0.5)
         for f in range(feeds):
             e.feed(h)
@@ -347,14 +255,13 @@ def test_carrier_detector_restatement_tracks_the_compiled_reference(ref, oracle)
     """Tasks/CarrierDetector.cpp compiled from the reference (Blackman-Harris taps from this repo's <sigutils/taps.h>,
     its FFT through a binary64 stand-in for FFTW) against sdo_carrier_detect (SPEC Y.5, binary32 SPEC transform): the
     same peak to the transforms' rounding."""
-    ref.ref_carrier_detect.restype = C.c_float
-    ref.ref_carrier_detect.argtypes = [C.c_void_p, C.c_size_t, C.c_double, C.c_double]
     rng = np.random.default_rng(12)
-    for n, f0, notch in ((5000, 0.0371, 0.0), (16384, -0.212, 0.0), (3000, 0.11, 0.05), (9000, -0.4, 0.02)):
+    for (n, f0, notch), got in zip(((5000, 0.0371, 0.0), (16384, -0.212, 0.0), (3000, 0.11, 0.05), (9000, -0.4, 0.02)),
+                                   ref["carrier_detect"]):
         t = np.arange(n)
         x = (np.exp(2j * np.pi * f0 * t) * (1 + 0.3 * np.cos(2 * np.pi * 0.001 * t))
              + 0.05 * (rng.standard_normal(n) + 1j * rng.standard_normal(n)) + 0.5).astype(np.complex64)
-        got = float(ref.ref_carrier_detect(x.ctypes.data, n, 0.01, notch))
+        got = float(got)
         mine = float(oracle.carrier_detect(x, 0.01, notch))
         assert abs(got - mine) < 2e-5, (n, f0, got, mine)
         assert abs(got - 2 * np.pi * f0) < 2e-3 or notch > 0
