@@ -254,7 +254,8 @@ void    *sdb_engine_stream(const sdb_engine_t *e);
 uint64_t sdb_engine_launch_count(const sdb_engine_t *e);
 /* average device time (ms) of the named kernel family over the launches since the last reset, measured
  * with CUDA events on the engine stream; families: "fft_cols", "fft_rows_psd", "fft_rows_chan",
- * "chan_ifft", "inspector" */
+ * "chan_ifft", "inspector".  A 65536-point plan's fused forward transform counts as "fft_cols"; its
+ * "fft_rows_psd" / "fft_rows_chan" stay at zero launches */
 int      sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches);
 void     sdb_engine_timing(sdb_engine_t *e, int enable);
 /* inspector-kernel stage balance since the last reset: out[0..3] = busy SM cycles of the gain / carrier /

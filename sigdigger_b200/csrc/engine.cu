@@ -68,10 +68,11 @@ struct sdb_engine {
   SdbFourStep fs_psd{}, fs_st{};
   bool psd_small = false;
   float *d_window = nullptr;
+  // four-step scratch of the two-kernel transforms (every four-step size but 65536, which runs fused)
   float2 *d_scratch = nullptr; int chunk_windows = 1; size_t l2_pinned_bytes = 0; int sm_count = 0;
-  // The PSD transforms run on their own stream, concurrently with the channeliser transforms of the same
-  // group of streams (feed_device): the two kernel chains fill each other's launch gaps and partial waves,
-  // and both read the same input region while it is still in L2.
+  // Two-kernel sizes with Np == W: the PSD transforms run on their own stream, concurrently with the channeliser
+  // transforms of the same group of streams (feed_device): the two kernel chains fill each other's launch gaps
+  // and partial waves, and both read the same input region while it is still in L2.
   cudaStream_t psd_stream = nullptr; cudaEvent_t ev_feed = nullptr;
   float2 *d_xin = nullptr;              // staging for host feeds
   float2 *d_hist = nullptr;             // [S][W/2]
@@ -590,20 +591,19 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       if (!e->chdet) return fail("out of device memory (channel detector)");
     }
   }
-  // ---- four-step scratch: one window per SM, pinned in L2
+  // ---- four-step scratch of the two-kernel sizes: whole waves of both passes, pinned in L2.  65536-point windows
+  // keep their intermediate in the shared memory of a thread-block cluster and need none.
   {
-    unsigned big = std::max(Np > 4096 ? Np : 0u, K > 0 ? W : 0u);
+    unsigned big = std::max(Np > 4096 && Np != 65536 ? Np : 0u, K > 0 && W != 65536 ? W : 0u);
     if (big) {
       size_t scratch_mb = 64;
       if (const char *env = getenv("SDB_SCRATCH_MB")) { long v = atol(env); if (v >= 1 && v <= 4096) scratch_mb = (size_t) v; }
       size_t cw = (scratch_mb << 20) / ((size_t) big * sizeof(float2));
       if (cw < 1) cw = 1;
-      if ((big == 65536 || big == 32768 || big == 16384 || big == 8192) && !getenv("SDB_SCRATCH_MB")) {
-        // 65536 path: 16 (pass A, 4 CTAs/SM) and 8 (pass B, 2 CTAs/SM) CTAs per window, all of equal duration:
-        // one window per SM is exactly 4 waves of either kernel.  On an H100 that is 132 windows, 69 MB, more than
-        // its 50 MB L2 can set aside for persisting lines, so the chunk is halved (whole waves still: 2 per kernel,
-        // 34.6 MB) until it fits the set-aside.  bench.py cfg3 on an H100 80GB HBM3 at 400 W: 10.6 GS/s with the
-        // halved chunk, 7.6 GS/s with one window per SM (SDB_CHUNK_WINDOWS=132).
+      if ((big == 32768 || big == 16384 || big == 8192) && !getenv("SDB_SCRATCH_MB")) {
+        // SPEC F.5 path: 512 KB of windows per SM is whole waves of both passes (two 32768-point windows: 32
+        // k_cols16T CTAs at 8 per SM, 8 k_rows256 CTAs at 2 per SM).  On an H100 that is 69 MB, more than its
+        // 50 MB L2 can set aside for persisting lines, so the chunk is halved (whole waves still) until it fits.
         int sms = 0, max_persist = 0;
         if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->prm.device) == cudaSuccess && sms > 0 &&
             (size_t) sms * 65536 * sizeof(float2) <= (100u << 20)) {
@@ -617,7 +617,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       e->chunk_windows = (int) cw;
       e->d_scratch = e->dalloc<float2>((size_t) e->chunk_windows * big);
       if (!e->d_scratch) return fail("out of device memory (scratch)");
-      if (Np > 4096 && K > 0 && Np == W && !getenv("SDB_NO_PSD_STREAM")) {
+      if (Np > 4096 && Np != 65536 && K > 0 && Np == W && !getenv("SDB_NO_PSD_STREAM")) {
         CK(cudaStreamCreateWithFlags(&e->psd_stream, cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&e->ev_feed, cudaEventDisableTiming));
       }
@@ -625,7 +625,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       // and every window costs two extra HBM round trips.  Accesses of the transform streams inside the window
       // are "persisting" (a set-aside part of L2 that normal traffic cannot evict); the kernels additionally
       // mark their one-shot outputs as streaming (st.global.cs).
-      if ((big == 65536 || big == 32768 || big == 16384 || big == 8192) && !getenv("SDB_NO_L2_PIN")) {   // the set-aside is device-wide: only the big plans claim it
+      if ((big == 32768 || big == 16384 || big == 8192) && !getenv("SDB_NO_L2_PIN")) {   // the set-aside is device-wide: only the big plans claim it
         int max_persist = 0, max_window = 0;
         cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, e->prm.device);
         cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, e->prm.device);
@@ -711,7 +711,12 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
     e->d_lo_phase = e->dalloc<float>((size_t) S * K);
     if (!e->d_chans || !e->d_chanb[0] || !e->d_chanb[1] || !e->d_tails || !e->d_lo_phase)
       return fail("out of device memory (channels)");
-    CK(cudaStreamCreateWithFlags(&e->insp_stream, cudaStreamNonBlocking));
+    // The inspector kernel of feed i runs beside the transforms of feed i + 1.  Its CTAs are few and long-lived; the
+    // highest priority places them as soon as SM space frees up instead of after every CTA of a transform grid
+    // queued before them (65536 points: one grid per feed) has been dispatched.
+    int prio_least = 0, prio_greatest = 0;
+    CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
+    CK(cudaStreamCreateWithPriority(&e->insp_stream, cudaStreamNonBlocking, prio_greatest));
     for (int i = 0; i < 2; ++i) {
       CK(cudaEventCreateWithFlags(&e->ev_chan[i], cudaEventDisableTiming));
       CK(cudaEventCreateWithFlags(&e->ev_insp[i], cudaEventDisableTiming));
@@ -883,11 +888,10 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     a.x = x; a.fmt = fmt; a.stream_stride = stride; a.hist = nullptr; a.hist_len = 0;
     a.windows_per_stream = frames; a.first_window = 0; a.hop = (int) Np; a.base_off = 0;
     a.window = e->d_window; a.scratch = scr;
-    const bool fast = e->fs_psd.N2 == 256 && e->fs_psd.N1 >= 32 && e->fs_psd.N1 <= 256;        // SPEC F.4 / F.5
+    const bool fast = e->fs_psd.N2 == 256 && e->fs_psd.N1 >= 32 && e->fs_psd.N1 <= 128;        // SPEC F.5
     e->span_begin(FAM_COLS, lc.stream);
-    if (fast && e->fs_psd.N1 == 256) CK(sdb_launch_cols256(lc, e->fs_psd, a, e->fs_psd.twN, w0, cw));
-    else if (fast)                   CK(sdb_launch_cols128(lc, e->fs_psd, a, w0, cw));
-    else                             CK(sdb_launch_pass_a_range(lc, e->fs_psd, a, w0, cw));
+    if (fast) CK(sdb_launch_cols128(lc, e->fs_psd, a, w0, cw));
+    else      CK(sdb_launch_pass_a_range(lc, e->fs_psd, a, w0, cw));
     e->span_end(lc.stream);
     SdbPassBArgs b{};
     b.scratch = scr; b.n_windows = cw; b.psd = e->d_psd + (size_t) w0 * Np;
@@ -903,11 +907,10 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     a.x = x; a.fmt = fmt; a.stream_stride = stride; a.hist = e->d_hist; a.hist_len = (int) (W / 2);
     a.windows_per_stream = wps; a.first_window = first; a.hop = (int) (W / 2); a.base_off = 0;
     a.window = nullptr; a.scratch = scr;
-    const bool fast = e->fs_st.N2 == 256 && e->fs_st.N1 >= 32 && e->fs_st.N1 <= 256;
+    const bool fast = e->fs_st.N2 == 256 && e->fs_st.N1 >= 32 && e->fs_st.N1 <= 128;
     e->span_begin(FAM_COLS, lc.stream);
-    if (fast && e->fs_st.N1 == 256) CK(sdb_launch_cols256(lc, e->fs_st, a, e->fs_st.twN, w0, cw));
-    else if (fast)                  CK(sdb_launch_cols128(lc, e->fs_st, a, w0, cw));
-    else                            CK(sdb_launch_pass_a_range(lc, e->fs_st, a, w0, cw));
+    if (fast) CK(sdb_launch_cols128(lc, e->fs_st, a, w0, cw));
+    else      CK(sdb_launch_pass_a_range(lc, e->fs_st, a, w0, cw));
     e->span_end(lc.stream);
     SdbPassBArgs b{};
     b.scratch = scr; b.n_windows = cw; b.binmap = e->d_binmap;
@@ -958,15 +961,27 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     CK(cudaEventRecord(e->ev_psd_ready[ob], e->psd_stream));
     CK(cudaStreamWaitEvent(e->stream, e->ev_psd_ready[ob], 0));   // the main stream stays the engine's timeline
   } else {
+    if (Np && e->psd_read_valid[ob]) CK(cudaStreamWaitEvent(e->stream, e->ev_psd_read[ob], 0));   // async read of feed i-2
+    // ---- 65536-point PSD frames and channeliser windows: one launch, both passes fused, ordered by stream
+    const bool fused_psd = Np == 65536, fused_chan = K && W == 65536;
+    if ((fused_psd && frames > 0) || (fused_chan && wps > 0)) {
+      SdbFft65536Args f{};
+      f.x = x; f.fmt = fmt; f.stream_stride = stride; f.n_streams = (int) S;
+      f.n_psd = fused_psd ? frames : 0; f.n_chan = fused_chan ? wps : 0; f.first_chan = first;
+      f.window = e->d_window; f.psd = e->d_psd; f.inv_n = 1.0f / 65536.0f; f.shift_db = shift_db;
+      f.hist = e->d_hist; f.binmap = e->d_binmap; f.cspec = e->d_cspec; f.n_bins = e->n_bins; f.ka_mask = e->ka_mask;
+      e->span_begin(FAM_COLS);
+      CK(sdb_launch_fft65536(ctx, fused_psd ? e->fs_psd : e->fs_st, f));
+      e->span_end();
+    }
     // ---- main PSD
     if (Np) {
-      if (e->psd_read_valid[ob]) CK(cudaStreamWaitEvent(e->stream, e->ev_psd_read[ob], 0));   // async read of feed i-2
       if (e->psd_small) {
         e->span_begin(FAM_ROWS_PSD);
         CK(sdb_launch_small_psd(ctx, (int) Np, e->twiddle(Np), x, fmt, stride, frames, (int) S, e->d_window,
                                 e->d_psd, shift_db));
         e->span_end();
-      } else {
+      } else if (!fused_psd) {
         const int total = frames * (int) S;
         for (int w0 = 0; w0 < total; w0 += e->chunk_windows)
           if (psd_chunk(ctx, frames, w0, std::min(e->chunk_windows, total - w0), e->d_scratch)) return -1;
@@ -976,7 +991,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
       CK(cudaEventRecord(e->ev_psd_ready[ob], e->stream));
     }
     // ---- channeliser forward transforms
-    if (K && wps > 0) {
+    if (K && wps > 0 && !fused_chan) {
       const int total = wps * (int) S;
       for (int w0 = 0; w0 < total; w0 += e->chunk_windows)
         if (chan_chunk(ctx, wps, first, w0, std::min(e->chunk_windows, total - w0), e->d_scratch)) return -1;

@@ -2,21 +2,26 @@
 // 65536 = 256 x 256, each 256-point transform = 16 x 16 with BOTH radix-16 butterflies held in
 // registers (16 complex values per thread) and ONE shared-memory exchange between them.
 //
-//   pass A (k_cols256): a CTA owns 16 adjacent columns of a window: every thread issues 16 independent
-//       coalesced float2 loads (128 B per thread in flight), optional window multiply, radix-16 over the
-//       high row digit, twiddle W_256^(t ka), exchange, radix-16 over the low row digit, inter-pass twiddle
-//       W_65536^(n2 k1) = coarse x fine (SPEC F.4) read from a [k1][n2] table tabulated once with the same
-//       arithmetic, transposed coalesced store into the L2-pinned scratch.
-//   pass B (k_rows256): a CTA owns 32 rows of the scratch; same two butterflies; the second one is mapped
-//       so that a warp holds 32 consecutive output bins -> 128-byte PSD / compacted-spectrum stores.
+//   k_fft65536: one thread-block cluster of 16 CTAs per window.
+//     pass A: a CTA owns 16 adjacent columns: every thread issues 16 independent coalesced float2 loads
+//       (128 B per thread in flight), optional window multiply, radix-16 over the high row digit, twiddle
+//       W_256^(t ka), exchange, radix-16 over the low row digit, inter-pass twiddle W_65536^(n2 k1) =
+//       coarse x fine (SPEC F.4) read from a [k1][n2] table tabulated once with the same arithmetic, and a
+//       store of each row k1 into the shared memory of the CTA that transforms it in pass B.
+//     pass B: a CTA owns 16 rows; same two butterflies; the second one is mapped so that a half-warp holds
+//       16 consecutive output bins -> 64-byte PSD / compacted-spectrum stores.
+//   k_cols16T + k_rows256: the same decomposition for N = 32768 / 16384 / 8192 (SPEC F.5), two kernels with a
+//     scratch buffer between them.
 //
 // Same mathematics as the generic path in fft_kernels.cu (which remains for every other size); results
-// are bit-identical to oracle/fft_spec.c (SPEC.md F.4).
+// are bit-identical to oracle/fft_spec.c (SPEC.md F.4, F.5).
 // Replaces the forward FFTs of su_specttuner
 // (Tasks/LPFTask.cpp:83-87) and of the PSD (Suscan/Messages/PSDMessage.cpp:26-39).
 #include "sdb_internal.h"
 #include "sdb_math.h"
 #include "sdb_cpx.h"
+#include <cooperative_groups.h>
+namespace cg = cooperative_groups;
 
 #define C1 0.92387953251128675613f   // cos(pi/8)
 #define S1 0.38268343236508977173f   // sin(pi/8)
@@ -45,48 +50,76 @@ static __device__ __forceinline__ void fft16(float2 (&v)[16])
 // position p = 4 m + q of fft16's output holds X[m + 4 q]
 #define REV16(p) ((((p) >> 2)) | (((p) & 3) << 2))
 
-struct Cols256K {
-  const void *x; int fmt; size_t stream_stride;
-  const float2 *hist; int hist_len;
-  int windows_per_stream, first_window, hop, base_off, win_base;
-  const float *window;
-  float2 *scratch;
+// ---------------------------------------------------------------------------------------------
+// N = 65536 = 256 x 256 (SPEC F.4): both passes in one kernel.  The 16 CTAs of a window form a thread-block
+// cluster; CTA b owns columns [16 b, 16 b + 16) in pass A and rows k1 in [16 b, 16 b + 16) in pass B.  Pass A's
+// output row k1 goes straight into the shared memory of CTA k1 >> 4 (distributed shared memory), so the
+// 512 KB intermediate of a window never leaves the SMs.  A window is a PSD frame (window taps, |X|^2 / N
+// epilogue) or a channeliser window (history, compacting bin scatter); the kind is uniform across a cluster.
+struct Fft65536K {
+  SdbFft65536Args a;
   const float2 *tw256;     // W_256^i
-  const float2 *twfine;    // W_65536^i, i < 256
   const float2 *twpq;      // tabulated inter-pass twiddle [k1][n2]
 };
 
-#define LDC 273    // pitch of one column's [ka][17] block (odd: conflict-free across columns)
+#define LDC 273    // pass A: pitch of one column's [ka][17] block (odd: conflict-free across columns)
+#define LDX 256    // received rows [k1 & 15][n2]
+#define LDR 273    // pass B: pitch of one row's [ka][17] block
 
-__global__ void __launch_bounds__(256, 4) k_cols256(const Cols256K p)   // 64 regs, 39 KB smem -> 4 CTAs / SM
+static __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+static __device__ __forceinline__ void cluster_wait()   { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+
+__global__ void __cluster_dims__(16, 1, 1) __launch_bounds__(256, 3) k_fft65536(const Fft65536K p)
 {
+  // one buffer, three uses: pass A's exchange, the 16 rows the cluster sends this CTA, pass B's exchange
   __shared__ float2 sm[16 * LDC];
   __shared__ float2 s_tw[256];
+  __shared__ int s_win[2];                          // output window, PSD frame (1) or channeliser window (0)
+  cg::cluster_group cluster = cg::this_cluster();
+  const SdbFft65536Args &a = p.a;
   const int tid = threadIdx.x;
   s_tw[tid] = __ldg(p.tw256 + tid);
-  const int c = tid & 15, t = tid >> 4;
-  const int w = p.win_base + blockIdx.y;
-  const int stream = w / p.windows_per_stream;
-  const int j0 = p.first_window + (w - stream * p.windows_per_stream);
-  const int col = blockIdx.x * 16 + c;
-  const long v0 = (long) p.base_off + (long) j0 * p.hop;
-  const int fmt = p.fmt;
-  const char *__restrict__ xs = reinterpret_cast<const char *>(p.x) + (size_t) stream * p.stream_stride * sdb_fmt_bytes(fmt);
-  const float2 *__restrict__ hs = p.hist ? p.hist + (size_t) stream * p.hist_len : nullptr;
+  const int rank = (int) cluster.block_rank();      // == blockIdx.x & 15
+  const int w = blockIdx.x >> 4;
+  // windows of one stream are adjacent; with both kinds, PSD frame f sits between channeliser windows 2f and 2f + 1,
+  // which read the same samples, so that the later reads hit L2 (the first feed has no channeliser window 0)
+  const int per = a.n_psd + a.n_chan;
+  const int stream = w / per;
+  int u = w - stream * per;
+  bool psd; int win;                                // PSD frame or channeliser window index within the stream
+  if (a.n_psd && a.n_chan) { u += a.first_chan; const int f = u / 3, r = u - 3 * f; psd = r == 1; win = psd ? f : 2 * f + (r >> 1); }
+  else if (a.n_psd)        { psd = true; win = u; }
+  else                     { psd = false; win = u + a.first_chan; }
+  // kept in shared memory rather than in registers across both passes
+  if (tid == 0) { s_win[0] = psd ? stream * a.n_psd + win : stream * a.n_chan + (win - a.first_chan); s_win[1] = psd; }
 
+  // ---- pass A: columns [16 rank, 16 rank + 16)
+  const int c = tid & 15, t = tid >> 4;
+  const int col = rank * 16 + c;
+  const int hist_len = psd ? 0 : 32768;             // channeliser: half a window of history precedes x
+  const long v0 = (long) win * (psd ? 65536 : 32768);
+  const int fmt = a.fmt;
+  const char *__restrict__ xs = reinterpret_cast<const char *>(a.x) + (size_t) stream * a.stream_stride * sdb_fmt_bytes(fmt);
+  const float2 *__restrict__ hs = psd ? nullptr : a.hist + (size_t) stream * hist_len;
+
+  const float *__restrict__ wp = psd && a.window ? a.window + t * 256 + col : nullptr;
   float2 v[16];
   if (fmt == SDB_FMT_F32) {
     const float2 *__restrict__ xf = reinterpret_cast<const float2 *>(xs);
-    if (v0 >= p.hist_len) {                         // CTA-uniform: the window lies wholly in the new samples
-      const float2 *__restrict__ src = xf + (v0 - p.hist_len) + t * 256 + col;
+    if (v0 >= hist_len) {                           // CTA-uniform: the window lies wholly in the new samples
+      const float2 *__restrict__ src = xf + (v0 - hist_len) + t * 256 + col;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) v[j] = __ldg(src + j * 4096);    // row n1 = t + 16 j
+      for (int j = 0; j < 16; ++j) {
+        v[j] = __ldg(src + j * 4096);    // row n1 = t + 16 j
+        if (wp) { const float wv = __ldg(wp + j * 4096); v[j] = sdb_mul2(v[j], make_float2(wv, wv)); }
+      }
     } else {
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int r = t + 16 * j;
         const long vi = v0 + (long) r * 256 + col;
-        v[j] = vi < p.hist_len ? __ldg(hs + vi) : __ldg(xf + (vi - p.hist_len));
+        v[j] = vi < hist_len ? __ldg(hs + vi) : __ldg(xf + (vi - hist_len));
+        if (wp) { const float wv = __ldg(wp + j * 4096); v[j] = sdb_mul2(v[j], make_float2(wv, wv)); }
       }
     }
   } else {                                          // 8 / 16-bit SDR samples: converted in the load
@@ -94,14 +127,8 @@ __global__ void __launch_bounds__(256, 4) k_cols256(const Cols256K p)   // 64 re
     for (int j = 0; j < 16; ++j) {
       const int r = t + 16 * j;
       const long vi = v0 + (long) r * 256 + col;
-      v[j] = vi < p.hist_len ? __ldg(hs + vi) : sdb_ld_iq(xs, vi - p.hist_len, fmt);
-    }
-  }
-  if (p.window) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const float wv = __ldg(p.window + (t + 16 * j) * 256 + col);
-      v[j] = sdb_mul2(v[j], make_float2(wv, wv));
+      v[j] = vi < hist_len ? __ldg(hs + vi) : sdb_ld_iq(xs, vi - hist_len, fmt);
+      if (wp) { const float wv = __ldg(wp + j * 4096); v[j] = sdb_mul2(v[j], make_float2(wv, wv)); }
     }
   }
   fft16(v);                                         // over j: Y[t][ka], ka = REV16(position)
@@ -114,35 +141,91 @@ __global__ void __launch_bounds__(256, 4) k_cols256(const Cols256K p)   // 64 re
     sm[c * LDC + ka * 17 + t] = y;
   }
   __syncthreads();
-  const int ka = t;                                 // second butterfly: thread (c, ka) gathers all t
+  {
+    const int ka = t;                               // second butterfly: thread (c, ka) gathers all t
 #pragma unroll
-  for (int tt = 0; tt < 16; ++tt) v[tt] = sm[c * LDC + ka * 17 + tt];
-  fft16(v);                                         // over t: X[ka + 16 kb], kb = REV16(position)
-  float2 *__restrict__ out = p.scratch + (size_t) blockIdx.y * 65536;
+    for (int tt = 0; tt < 16; ++tt) v[tt] = sm[c * LDC + ka * 17 + tt];
+    cluster_arrive();                               // this CTA's exchange buffer is free for the rows it receives
+    fft16(v);                                       // over t: X[ka + 16 kb], kb = REV16(position)
 #pragma unroll
-  for (int q = 0; q < 16; ++q) {
-    const int kb = REV16(q);
-    const int k1 = ka + 16 * kb;
-    out[(size_t) k1 * 256 + col] = cmulf(v[q], __ldg(p.twpq + k1 * 256 + col));   // SPEC F.4 inter-pass twiddle
+    for (int q = 0; q < 16; ++q) {
+      const int k1 = ka + 16 * REV16(q);
+      v[q] = cmulf(v[q], __ldg(p.twpq + k1 * 256 + col));      // SPEC F.4 inter-pass twiddle
+    }
+    cluster_wait();                                 // every CTA of the window has read its exchange buffer
+#pragma unroll
+    for (int q = 0; q < 16; ++q) {                  // row k1 = ka + 16 kb to CTA kb, its row ka
+      float2 *dst = cluster.map_shared_rank(sm, REV16(q));
+      dst[ka * LDX + col] = v[q];
+    }
+  }
+  cluster_arrive();
+  cluster_wait();                                   // all 16 rows of this CTA have arrived
+
+  // ---- pass B: rows k1 = 16 rank + r; output bin k = k1 + 256 (ka + 16 kb)
+  const int out_win = s_win[0];
+  const bool out_psd = s_win[1];
+  const unsigned ka_mask = out_psd ? 0xffffu : a.ka_mask;
+  {
+    const int t = tid & 15, r = tid >> 4;           // 16 rows x 16 t
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = sm[r * LDX + t + 16 * j];
+    fft16(v);
+    __syncthreads();                                // every row read before the exchange overwrites it
+#pragma unroll
+    for (int q = 0; q < 16; ++q) {
+      const int ka = REV16(q);
+      if (!((ka_mask >> ka) & 1)) continue;         // channeliser: digits ka no channel touches are never formed
+      float2 y = v[q];
+      if (ka) y = cmulf(y, s_tw[t * ka]);
+      sm[r * LDR + ka * 17 + t] = y;
+    }
+  }
+  __syncthreads();
+  const int r = tid & 15, ka = tid >> 4;            // a half-warp = 16 consecutive rows = 16 consecutive bins
+  if (!((ka_mask >> ka) & 1)) return;
+#pragma unroll
+  for (int tt = 0; tt < 16; ++tt) v[tt] = sm[r * LDR + ka * 17 + tt];
+  fft16(v);
+  const int k1 = rank * 16 + r;
+  if (out_psd) {
+    float *__restrict__ out = a.psd + (size_t) out_win * 65536;
+#pragma unroll
+    for (int q = 0; q < 16; ++q) {
+      const int k = k1 + 256 * (ka + 16 * REV16(q));
+      float pw = __fmaf_rn(v[q].x, v[q].x, v[q].y * v[q].y) * a.inv_n;
+      // one-shot outputs: streaming stores, so that they do not displace the input in L2
+      if (a.shift_db) { pw = 10.0f * d_log10f(pw + 1e-8f); __stcs(out + ((k + 32768) & 65535), pw); }
+      else __stcs(out + k, pw);
+    }
+  } else {
+    float2 *__restrict__ out = a.cspec + (size_t) out_win * a.n_bins;
+#pragma unroll
+    for (int q = 0; q < 16; ++q) {
+      const int k = k1 + 256 * (ka + 16 * REV16(q));
+      const int m = __ldg(a.binmap + k);
+      if (m >= 0) __stcs(out + m, v[q]);
+    }
   }
 }
 
-cudaError_t sdb_launch_cols256(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassAArgs &a,
-                               const float2 *twfine, int win_base, int n_win)
+cudaError_t sdb_launch_fft65536(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbFft65536Args &a)
 {
-  Cols256K p;
-  p.x = a.x; p.fmt = a.fmt; p.stream_stride = a.stream_stride; p.hist = a.hist; p.hist_len = a.hist_len;
-  p.windows_per_stream = a.windows_per_stream; p.first_window = a.first_window; p.hop = a.hop;
-  p.base_off = a.base_off; p.win_base = win_base; p.window = a.window; p.scratch = a.scratch;
-  p.tw256 = fs.twN1; p.twfine = twfine; p.twpq = fs.twPQ;
-  dim3 grid(16, n_win);
-  k_cols256<<<grid, 256, 0, c.stream>>>(p);
+  const long n_win = (long) a.n_streams * (a.n_psd + a.n_chan);
+  if (fs.N1 != 256 || fs.N2 != 256 || n_win <= 0 || n_win > (1l << 27)) return cudaErrorInvalidValue;
+  Fft65536K p;
+  p.a = a; p.tw256 = fs.twN1; p.twpq = fs.twPQ;
+  static std::atomic<unsigned long long> attr_done{ 0 };   // one bit per device: function attributes are per context
+  if (sdb_first_on_device(attr_done))               // a 16-CTA cluster is beyond the portable size of 8
+    cudaFuncSetAttribute(k_fft65536, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+  k_fft65536<<<(unsigned) (16 * n_win), 256, 0, c.stream>>>(p);
   if (c.launch_counter) ++*c.launch_counter;
   return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------
-// N = 32768 / 16384 / 8192 = N1 x 256 with N1 = 16 T, T = 8 / 4 / 2 (SPEC F.5; BASELINE configs[3] and [0]).  Pass A:
+// N = 32768 / 16384 / 8192 = N1 x 256 with N1 = 16 T, T = 8 / 4 / 2 (SPEC F.5; BASELINE configs[3] and [0]), through a
+// scratch buffer between the two passes (the engine pins it in L2).  Pass A:
 // columns of 16 T -- the same first butterfly (fft16 over the high row digit), twiddle W_N1^(t ka), exchange, then a
 // T-point butterfly over the low row digit (T = 8: one radix-2 stage + two DFT4); pass B is k_rows256 with N1 rows per
 // window.
@@ -164,6 +247,15 @@ static __device__ __forceinline__ void fft8(float2 (&v)[8])
 // Pass A for N1 = 16 T rows, T = 8 (N = 32768), 4 (16384), 2 (8192): 128-thread CTAs that own C = 128 / T adjacent columns
 // (thread = (column c, low row digit t)); the first butterfly is the 65536 kernel's fft16 over the high row digit, the
 // second a T-point butterfly over the low one, 16 / T of them per thread (ka = t + T h).
+struct Cols256K {
+  const void *x; int fmt; size_t stream_stride;
+  const float2 *hist; int hist_len;
+  int windows_per_stream, first_window, hop, base_off, win_base;
+  const float *window;
+  float2 *scratch;
+  const float2 *tw256;     // W_N1^i
+  const float2 *twpq;      // tabulated inter-pass twiddle [k1][n2]
+};
 template <int T>
 __global__ void __launch_bounds__(128, 8) k_cols16T(const Cols256K p)
 {
@@ -240,7 +332,7 @@ cudaError_t sdb_launch_cols128(const SdbLaunchCtx &c, const SdbFourStep &fs, con
   p.x = a.x; p.fmt = a.fmt; p.stream_stride = a.stream_stride; p.hist = a.hist; p.hist_len = a.hist_len;
   p.windows_per_stream = a.windows_per_stream; p.first_window = a.first_window; p.hop = a.hop;
   p.base_off = a.base_off; p.win_base = win_base; p.window = a.window; p.scratch = a.scratch;
-  p.tw256 = fs.twN1; p.twfine = nullptr; p.twpq = fs.twPQ;
+  p.tw256 = fs.twN1; p.twpq = fs.twPQ;
   const int T = fs.N1 / 16;                         // 8, 4 or 2: columns per CTA = 128 / T
   dim3 grid(256 / (128 / T), n_win);
   if (T == 8)      k_cols16T<8><<<grid, 128, 0, c.stream>>>(p);
@@ -260,11 +352,9 @@ struct Rows256K {
   unsigned ka_mask;
 };
 
-#define LDR 273
-
-// N1 = rows per window: 256 (N = 65536, SPEC F.4) or 128 / 64 / 32 (N = 32768 / 16384 / 8192, SPEC F.5); output bin
+// Pass B of the scratch-based sizes: N1 = rows per window, 128 / 64 / 32 (N = 32768 / 16384 / 8192, SPEC F.5); output bin
 // k = k1 + N1 (ka + 16 kb)
-template <int MODE, int N1 = 256>
+template <int MODE, int N1>
 __global__ void __launch_bounds__(512, 2) k_rows256(const Rows256K p)
 {
   constexpr int NN = N1 * 256;
@@ -284,7 +374,7 @@ __global__ void __launch_bounds__(512, 2) k_rows256(const Rows256K p)
 #pragma unroll
     for (int q = 0; q < 16; ++q) {
       const int ka = REV16(q);
-      // channeliser: output bin k = k1 + 256 (ka + 16 kb); digits ka no channel touches are never formed
+      // channeliser: digits ka no channel touches are never formed
       if (MODE == 1 && !((p.ka_mask >> ka) & 1)) continue;
       float2 y = v[q];
       if (ka) y = cmulf(y, s_tw[t * ka]);
@@ -326,8 +416,6 @@ cudaError_t sdb_launch_rows256(const SdbLaunchCtx &c, const SdbFourStep &fs, con
   const size_t smem = (size_t) 32 * LDR * sizeof(float2);
   static std::atomic<unsigned long long> attr_done{ 0 };   // one bit per device: function attributes are per context
   if (sdb_first_on_device(attr_done)) {
-    cudaFuncSetAttribute(k_rows256<0, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    cudaFuncSetAttribute(k_rows256<1, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
     cudaFuncSetAttribute(k_rows256<0, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
     cudaFuncSetAttribute(k_rows256<1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
     cudaFuncSetAttribute(k_rows256<0, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
@@ -339,7 +427,7 @@ cudaError_t sdb_launch_rows256(const SdbLaunchCtx &c, const SdbFourStep &fs, con
 #define ROWS_CASE(N1_) case N1_: if (mode == 0) k_rows256<0, N1_><<<grid, 512, smem, c.stream>>>(p); \
                                  else           k_rows256<1, N1_><<<grid, 512, smem, c.stream>>>(p); break
   switch (fs.N1) {
-    ROWS_CASE(256); ROWS_CASE(128); ROWS_CASE(64); ROWS_CASE(32);
+    ROWS_CASE(128); ROWS_CASE(64); ROWS_CASE(32);
     default: return cudaErrorInvalidValue;
   }
 #undef ROWS_CASE

@@ -59,7 +59,29 @@ struct SdbPassBArgs {
   const int    *binmap;             // N entries, compact index or -1
   float2       *cspec;              // [n_windows][n_bins]
   int           n_bins;
-  unsigned      ka_mask;            // 65536 path: bit (k >> 8) & 15 set for every needed bin k (0 = all)
+  unsigned      ka_mask;            // bit (k / N1) & 15 set for every needed bin k (0 = all)
+};
+
+// N = 65536 (fft256_kernels.cu): every PSD frame and channeliser window of a feed in one launch, both passes fused.
+// Per stream the launch holds n_psd PSD frames (hop 65536, no history) and n_chan channeliser windows
+// first_chan .. first_chan + n_chan - 1 (hop 32768 over the 32768-sample history followed by x); when both are
+// present, n_chan == 2 n_psd - first_chan.
+struct SdbFft65536Args {
+  const void   *x;                  // new samples, stream 0, in format `fmt` (sdb_iq.h)
+  int           fmt;
+  size_t        stream_stride;      // in samples
+  int           n_streams, n_psd, n_chan, first_chan;
+  // PSD frames: [S][n_psd][65536] output
+  const float  *window;             // 65536 taps or null
+  float        *psd;
+  float         inv_n;
+  int           shift_db;
+  // channeliser windows: [S][n_chan][n_bins] output
+  const float2 *hist;               // [S][32768]
+  const int    *binmap;             // 65536 entries, compact index or -1
+  float2       *cspec;
+  int           n_bins;
+  unsigned      ka_mask;            // bit (k >> 8) & 15 set for every needed bin k
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -241,10 +263,9 @@ struct SdbLaunchCtx {
 
 cudaError_t sdb_launch_pass_a_range(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassAArgs &a,
                                     int win_base, int n_win);
-// 65536 = 256 x 256 specialisation (fft256_kernels.cu)
+// 65536 / 32768 / 16384 / 8192 = N1 x 256 specialisations (fft256_kernels.cu)
+cudaError_t sdb_launch_fft65536(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbFft65536Args &a);
 cudaError_t sdb_launch_cols128(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassAArgs &a, int win_base, int n_win);
-cudaError_t sdb_launch_cols256(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassAArgs &a,
-                               const float2 *twfine, int win_base, int n_win);
 cudaError_t sdb_launch_rows256(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a, int mode);
 cudaError_t sdb_launch_pass_b_psd(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a);
 cudaError_t sdb_launch_pass_b_chan(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a);
