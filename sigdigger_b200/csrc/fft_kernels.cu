@@ -517,9 +517,13 @@ __global__ void __launch_bounds__(1024) k_chan_ifft(const SdbChannelDev *__restr
   const SdbChannelDev ch = chans[ci];
   const int s = blockIdx.y;
   const int size = ch.size, hs = ch.halfsz, hw = ch.halfw;
+  // With P = 1 (every size above 4096, and the default for the others) each prevb[i] is read and then rewritten by
+  // the one thread that owns i, so a single buffer serves both roles; with P > 1 group 0 reads the previous round's
+  // half while group P - 1 writes the next one, hence two.  The phase buffer sits behind it (precise groups only).
+  const int nprev = P > 1 ? 2 : 1;
   float2 *bufs = sm;                                   // [P][size]
-  float2 *prevb[2] = { sm + (size_t) P * size, sm + (size_t) P * size + hs };
-  float *phase = reinterpret_cast<float *>(sm + (size_t) P * size + 2 * hs);   // [P][hs]
+  float2 *prevb[2] = { sm + (size_t) P * size, sm + (size_t) P * size + (nprev - 1) * hs };
+  float *phase = reinterpret_cast<float *>(sm + (size_t) P * size + nprev * hs);   // [P][hs]
   const int tid = threadIdx.x;
   const int per = BPT == 1 ? (size >= 4 ? size >> 2 : 1) : (int) blockDim.x;   // threads per hop
   const int g = tid / per, l = tid - g * per;
@@ -815,10 +819,13 @@ cudaError_t sdb_launch_chan_ifft_group(const SdbLaunchCtx &c, const SdbChannelDe
     if (c.launch_counter) ++*c.launch_counter;
     return cudaGetLastError();
   }
+  // 16384-point precise channels need 128 KB of hop buffer + 64 KB of carried half + 32 KB of phases = 224 KB, within
+  // the H100's 227 KB per-block opt-in
+  const size_t smem_cap = 224 * 1024;
   if (sdb_first_on_device(attr_done)) {
-    cudaFuncSetAttribute(k_chan_ifft<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(k_chan_ifft<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(k_chan_ifft<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(k_chan_ifft<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem_cap);
+    cudaFuncSetAttribute(k_chan_ifft<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem_cap);
+    cudaFuncSetAttribute(k_chan_ifft<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem_cap);
   }
   int bpt = 1, threads = size / 4;
   while (threads > 1024) { threads >>= 1; bpt <<= 1; }
@@ -839,9 +846,9 @@ cudaError_t sdb_launch_chan_ifft_group(const SdbLaunchCtx &c, const SdbChannelDe
     threads = size / 4;
   }
   if (threads < 32) threads = 32;
-  const size_t smem = (size_t) P * size * sizeof(float2) + (size_t) size * sizeof(float2)
-                      + (size_t) P * (size / 2) * sizeof(float);
-  if (smem > 200 * 1024) return cudaErrorInvalidValue;
+  const size_t smem = (size_t) P * size * sizeof(float2) + (size_t) (P > 1 ? 2 : 1) * (size / 2) * sizeof(float2)
+                      + (any_precise ? (size_t) P * (size / 2) * sizeof(float) : 0);
+  if (smem > smem_cap) return cudaErrorInvalidValue;
   dim3 grid(group_len, n_streams);
   if (bpt == 1)
     k_chan_ifft<1><<<grid, threads, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps, P,
