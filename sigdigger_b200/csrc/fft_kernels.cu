@@ -704,9 +704,8 @@ static __device__ __forceinline__ void group_fft16(float2 *s, const int M, const
 }
 
 #define IFFT16_THREADS 256
-// MINB = resident CTAs per SM the register allocation aims at: 3 -> 80 registers, 4 -> 64 (72 bytes of spills)
-template <int MINB>
-__global__ void __launch_bounds__(IFFT16_THREADS, MINB)
+// 3 CTAs per SM (42 KB of shared memory at 1024 points): 80 registers, no spills
+__global__ void __launch_bounds__(IFFT16_THREADS, 3)
 k_chan_ifft16(const SdbChannelDev *__restrict__ chans, const int *__restrict__ group, int n_channels,
               const float2 *__restrict__ cspec, int n_bins, int wps, int any_precise,
               float2 *__restrict__ tails, size_t tail_stream_stride, float *__restrict__ lo_phase,
@@ -737,17 +736,27 @@ k_chan_ifft16(const SdbChannelDev *__restrict__ chans, const int *__restrict__ g
     const bool active = g < Pg;
     float2 *buf = bufs + (size_t) g * padsz;
     if (active) {
+      // The thread owns the 16 slots (i - hw) mod size, i = l + u per: bin i of the channel when i < 2 hw, the zero
+      // guard band between the sidebands otherwise.  Eight bins and their weights are loaded before the first is
+      // used (16 loads in flight per thread; all 16 slots at once spill at 80 registers).
       const float2 *__restrict__ cs = cspec + ((size_t) s * wps + j0 + g) * n_bins;
-      for (int i = hw + l; i < size - hw; i += per) buf[PADI(i)] = make_float2(0.0f, 0.0f);
-#pragma unroll 4
-      for (int i = l; i < 2 * hw; i += per) {
-        const int cidx = i < ch.L1 ? ch.c1 + i : i - ch.L1;
-        float2 X = __ldg(cs + cidx);
-        const float w = __ldg(ch.kh + i);
-        const int r = i - hw;
-        X.x *= w; X.y *= w;
-        const int o = r >= 0 ? r : size + r;
-        buf[PADI(o)] = X;
+#pragma unroll 1
+      for (int u0 = 0; u0 < 16; u0 += 8) {
+        float2 X[8];
+        float w[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          const int i = l + (u0 + u) * per;
+          const int cidx = i < ch.L1 ? ch.c1 + i : i - ch.L1;
+          X[u] = i < 2 * hw ? __ldg(cs + cidx) : make_float2(0.0f, 0.0f);
+          w[u] = i < 2 * hw ? __ldg(ch.kh + i) : 0.0f;
+        }
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          const int i = l + (u0 + u) * per, r = i - hw;
+          if (i < 2 * hw) { X[u].x *= w[u]; X[u].y *= w[u]; }
+          buf[PADI(r >= 0 ? r : size + r)] = X[u];
+        }
       }
     }
     if (any_precise && ch.precise && tid == IFFT16_THREADS - 1) {
@@ -796,26 +805,17 @@ cudaError_t sdb_launch_chan_ifft_group(const SdbLaunchCtx &c, const SdbChannelDe
                                        float2 *chan_out, size_t chan_stream_stride, int any_precise)
 {
   static std::atomic<unsigned long long> attr_done{ 0 };   // one bit per device: function attributes are per context
-  static const int use16 = getenv("SDB_IFFT16") ? atoi(getenv("SDB_IFFT16")) : 1;
-  if (use16 && size >= 512 && size <= 4096) {
+  if (size >= 512 && size <= 4096) {
     static std::atomic<unsigned long long> attr16_done{ 0 };
-    static const int occ = getenv("SDB_IFFT16_OCC") ? atoi(getenv("SDB_IFFT16_OCC")) : 3;
-    if (sdb_first_on_device(attr16_done)) {
-      cudaFuncSetAttribute(k_chan_ifft16<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-      cudaFuncSetAttribute(k_chan_ifft16<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    }
+    if (sdb_first_on_device(attr16_done))
+      cudaFuncSetAttribute(k_chan_ifft16, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     const int per = size / 16, P = IFFT16_THREADS / per;
     const size_t smem = (size_t) P * (size + size / 16) * sizeof(float2) + (size_t) size * sizeof(float2)
                         + (any_precise ? (size_t) P * (size / 2) * sizeof(float) : 0);
     dim3 grid(group_len, n_streams);
-    if (occ == 4)
-      k_chan_ifft16<4><<<grid, IFFT16_THREADS, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps,
-                                                                 any_precise, tails, tail_stream_stride, lo_phase,
-                                                                 chan_out, chan_stream_stride);
-    else
-      k_chan_ifft16<3><<<grid, IFFT16_THREADS, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps,
-                                                                 any_precise, tails, tail_stream_stride, lo_phase,
-                                                                 chan_out, chan_stream_stride);
+    k_chan_ifft16<<<grid, IFFT16_THREADS, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps,
+                                                            any_precise, tails, tail_stream_stride, lo_phase,
+                                                            chan_out, chan_stream_stride);
     if (c.launch_counter) ++*c.launch_counter;
     return cudaGetLastError();
   }
