@@ -65,11 +65,10 @@ struct sdb_engine {
   std::vector<void *> allocs;
 
   unsigned Np = 0, W = 0;               // PSD size, channeliser window
-  SdbFourStep fs_psd{}, fs_st{};
-  bool psd_small = false;
+  SdbFourStep fs_psd{}, fs_st{};       // transform plans (make_plan)
   float *d_window = nullptr;
-  // four-step scratch of the two-kernel transforms (every four-step size but 65536, which runs fused)
-  float2 *d_scratch = nullptr; int chunk_windows = 1; size_t l2_pinned_bytes = 0; int sm_count = 0;
+  // four-step scratch of the two-kernel transforms (the F.5 and Stockham paths)
+  float2 *d_scratch = nullptr; int chunk_windows = 1; size_t l2_pinned_bytes = 0;
   // Two-kernel sizes with Np == W: the PSD transforms run on their own stream, concurrently with the channeliser
   // transforms of the same group of streams (feed_device): the two kernel chains fill each other's launch gaps
   // and partial waves, and both read the same input region while it is still in L2.
@@ -181,55 +180,69 @@ struct sdb_engine {
   }
 };
 
-static bool make_four_step(sdb_engine *e, unsigned N, SdbFourStep *fs)
+// The transform plan of an N-point window for the main PSD (psd = true) or the channeliser: which kernels run
+// (SdbFftPath), the split N = N1 x N2 and the tables.  This is the one place that ties transform sizes to kernels.
+static bool make_plan(sdb_engine *e, unsigned N, bool psd, SdbFourStep *fs)
 {
-  int l = ilog2u(N), l1 = l / 2;
-  if (N == 32768 || N == 16384 || N == 8192) l1 = l - 8;        // SPEC F.5: N1 x 256 on the register-butterfly passes
-  fs->N = (int) N; fs->N1 = 1 << l1; fs->N2 = (int) N / fs->N1;
+  *fs = SdbFourStep{};
+  fs->N = (int) N;
+  if (psd && N <= 4096) {
+    fs->path = SDB_FFT_SMALL_PSD;
+    fs->twN = e->twiddle(N);
+    return fs->twN != nullptr;
+  }
+  fs->path = N == 65536 ? SDB_FFT_CLUSTER
+           : (N == 8192 || N == 16384 || N == 32768) ? SDB_FFT_F5 : SDB_FFT_STOCKHAM;
+  const int l = ilog2u(N);
+  fs->N1 = 1 << (fs->path == SDB_FFT_STOCKHAM ? l / 2 : l - 8);   // cluster and F.5: N1 x 256
+  fs->N2 = (int) N / fs->N1;
+  fs->ka_shift = ilog2u(fs->N1);
   fs->twN1 = e->twiddle(fs->N1); fs->twN2 = e->twiddle(fs->N2); fs->twN = e->twiddle(N);
-  fs->twPQ = nullptr;
   if (!(fs->twN1 && fs->twN2 && fs->twN)) return false;
-  if (N == 65536) {
-    // the product the kernels used to form per output (two table look-ups + one complex multiply), tabulated
-    // once with the same arithmetic (SPEC F.1: one rounded product + one fused multiply-add per component)
-    auto it = e->tw.find(0x10000u | 1u);
-    if (it != e->tw.end()) { fs->twPQ = it->second; return true; }
-    std::vector<float2> c, f, pq((size_t) 65536);
-    sdbh::twiddle_fill(256, c); sdbh::twiddle_fill(65536, f);
-    for (unsigned k1 = 0; k1 < 256; ++k1)
-      for (unsigned n2 = 0; n2 < 256; ++n2) {
-        const unsigned p = n2 * k1;
-        const float2 a = c[p >> 8], b = f[p & 255];
-        pq[(size_t) k1 * 256 + n2].x = fmaf(a.x, b.x, -(a.y * b.y));
-        pq[(size_t) k1 * 256 + n2].y = fmaf(a.x, b.y, a.y * b.x);
-      }
-    float2 *d = e->dalloc<float2>(65536);
-    if (!d) return false;
-    cudaMemcpy(d, pq.data(), 65536 * sizeof(float2), cudaMemcpyHostToDevice);
-    e->tw[0x10000u | 1u] = d;
-    fs->twPQ = d;
-  }
-  if (N == 32768 || N == 16384 || N == 8192) {
-    // SPEC F.5: N1 x 256, inter-pass twiddle [k1][n2] = W_N1^(p >> 8) x W_N^(p & 255), p = n2 k1
-    const unsigned N1 = N / 256;
-    auto it = e->tw.find(N | 1u);
-    if (it != e->tw.end()) { fs->twPQ = it->second; return true; }
-    std::vector<float2> c, f, pq((size_t) N);
-    sdbh::twiddle_fill(N1, c); sdbh::twiddle_fill(N, f);
-    for (unsigned k1 = 0; k1 < N1; ++k1)
-      for (unsigned n2 = 0; n2 < 256; ++n2) {
-        const unsigned p = n2 * k1;
-        const float2 a = c[p >> 8], b = f[p & 255];
-        pq[(size_t) k1 * 256 + n2].x = fmaf(a.x, b.x, -(a.y * b.y));
-        pq[(size_t) k1 * 256 + n2].y = fmaf(a.x, b.y, a.y * b.x);
-      }
-    float2 *d = e->dalloc<float2>(N);
-    if (!d) return false;
-    cudaMemcpy(d, pq.data(), (size_t) N * sizeof(float2), cudaMemcpyHostToDevice);
-    e->tw[N | 1u] = d;
-    fs->twPQ = d;
-  }
+  if (fs->path == SDB_FFT_STOCKHAM) return true;
+  // SPEC F.4 / F.5 inter-pass twiddle [k1][n2] = W_N1^(p >> 8) x W_N^(p & 255), p = n2 k1: the product of two table
+  // look-ups, tabulated once with the arithmetic of SPEC F.1 (one rounded product + one fused multiply-add per
+  // component)
+  auto it = e->tw.find(N | 1u);
+  if (it != e->tw.end()) { fs->twPQ = it->second; return true; }
+  const unsigned N1 = (unsigned) fs->N1;
+  std::vector<float2> c, f, pq((size_t) N);
+  sdbh::twiddle_fill(N1, c); sdbh::twiddle_fill(N, f);
+  for (unsigned k1 = 0; k1 < N1; ++k1)
+    for (unsigned n2 = 0; n2 < 256; ++n2) {
+      const unsigned p = n2 * k1;
+      const float2 a = c[p >> 8], b = f[p & 255];
+      pq[(size_t) k1 * 256 + n2].x = fmaf(a.x, b.x, -(a.y * b.y));
+      pq[(size_t) k1 * 256 + n2].y = fmaf(a.x, b.y, a.y * b.x);
+    }
+  float2 *d = e->dalloc<float2>(N);
+  if (!d) return false;
+  cudaMemcpy(d, pq.data(), (size_t) N * sizeof(float2), cudaMemcpyHostToDevice);
+  e->tw[N | 1u] = d;
+  fs->twPQ = d;
   return true;
+}
+
+static bool uses_scratch(const SdbFourStep &fs) { return fs.path == SDB_FFT_F5 || fs.path == SDB_FFT_STOCKHAM; }
+
+// Windows per chunk of the four-step scratch, for the largest scratch transform `big` of the engine
+static size_t scratch_chunk_windows(const SdbFourStep &big, int device)
+{
+  const size_t window_bytes = (size_t) big.N * sizeof(float2);
+  size_t cw = std::max<size_t>(1, ((size_t) 64 << 20) / window_bytes);
+  if (big.path != SDB_FFT_F5) return cw;
+  // SPEC F.5 path: 512 KB of windows per SM is whole waves of both passes (two 32768-point windows: 32 k_cols16T
+  // CTAs at 8 per SM, 8 k_rows256 CTAs at 2 per SM).  On an H100 that is 69 MB, more than its 50 MB L2 can set
+  // aside for persisting lines, so the chunk is halved (whole waves still) until it fits.
+  const size_t per_sm = (size_t) 512 << 10;
+  int sms = 0, max_persist = 0;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && sms > 0 &&
+      (size_t) sms * per_sm <= ((size_t) 100 << 20)) {
+    cw = (size_t) sms * (per_sm / window_bytes);
+    cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, device);
+    while (max_persist > 0 && cw % 2 == 0 && cw * window_bytes > (size_t) max_persist) cw /= 2;
+  }
+  return cw;
 }
 
 extern "C" sdb_engine_t *sdb_engine_new(const sdb_engine_params *p, double samp_rate)
@@ -577,9 +590,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       if (!e->d_window) return fail("out of device memory");
       CK(cudaMemcpy(e->d_window, w.data(), Np * sizeof(float), cudaMemcpyHostToDevice));
     }
-    e->psd_small = Np <= 4096;
-    if (e->psd_small) { if (!e->twiddle(Np)) return fail("out of device memory"); }
-    else if (!make_four_step(e, Np, &e->fs_psd)) return fail("out of device memory");
+    if (!make_plan(e, Np, true, &e->fs_psd)) return fail("out of device memory");
     e->max_frames = max_feed / Np;
     for (int i = 0; i < 2; ++i) {
       e->d_psdb[i] = e->dalloc<float>((size_t) S * e->max_frames * Np);
@@ -591,33 +602,18 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       if (!e->chdet) return fail("out of device memory (channel detector)");
     }
   }
-  // ---- four-step scratch of the two-kernel sizes: whole waves of both passes, pinned in L2.  65536-point windows
-  // keep their intermediate in the shared memory of a thread-block cluster and need none.
+  if (K > 0 && !make_plan(e, W, false, &e->fs_st)) return fail("out of device memory");
+  // ---- four-step scratch of the two-kernel paths: whole waves of both passes, pinned in L2.  The cluster path keeps
+  // its intermediate in the shared memory of a thread-block cluster and needs none.
   {
-    unsigned big = std::max(Np > 4096 && Np != 65536 ? Np : 0u, K > 0 && W != 65536 ? W : 0u);
+    const SdbFourStep *big = nullptr;
+    if (Np && uses_scratch(e->fs_psd)) big = &e->fs_psd;
+    if (K > 0 && uses_scratch(e->fs_st) && (!big || e->fs_st.N > big->N)) big = &e->fs_st;
     if (big) {
-      size_t scratch_mb = 64;
-      if (const char *env = getenv("SDB_SCRATCH_MB")) { long v = atol(env); if (v >= 1 && v <= 4096) scratch_mb = (size_t) v; }
-      size_t cw = (scratch_mb << 20) / ((size_t) big * sizeof(float2));
-      if (cw < 1) cw = 1;
-      if ((big == 32768 || big == 16384 || big == 8192) && !getenv("SDB_SCRATCH_MB")) {
-        // SPEC F.5 path: 512 KB of windows per SM is whole waves of both passes (two 32768-point windows: 32
-        // k_cols16T CTAs at 8 per SM, 8 k_rows256 CTAs at 2 per SM).  On an H100 that is 69 MB, more than its
-        // 50 MB L2 can set aside for persisting lines, so the chunk is halved (whole waves still) until it fits.
-        int sms = 0, max_persist = 0;
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->prm.device) == cudaSuccess && sms > 0 &&
-            (size_t) sms * 65536 * sizeof(float2) <= (100u << 20)) {
-          cw = (size_t) sms * (65536 / big);          // the same bytes: two 32768-point windows per SM, ...
-          cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, e->prm.device);
-          while (max_persist > 0 && cw % 2 == 0 && cw * big * sizeof(float2) > (size_t) max_persist) cw /= 2;
-        }
-        e->sm_count = sms;
-      }
-      if (const char *env = getenv("SDB_CHUNK_WINDOWS")) { long v = atol(env); if (v >= 1 && v <= 65536) cw = (size_t) v; }
-      e->chunk_windows = (int) cw;
-      e->d_scratch = e->dalloc<float2>((size_t) e->chunk_windows * big);
+      e->chunk_windows = (int) scratch_chunk_windows(*big, e->prm.device);
+      e->d_scratch = e->dalloc<float2>((size_t) e->chunk_windows * big->N);
       if (!e->d_scratch) return fail("out of device memory (scratch)");
-      if (Np > 4096 && Np != 65536 && K > 0 && Np == W && !getenv("SDB_NO_PSD_STREAM")) {
+      if (Np && K > 0 && Np == W && uses_scratch(e->fs_psd)) {
         CK(cudaStreamCreateWithFlags(&e->psd_stream, cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&e->ev_feed, cudaEventDisableTiming));
       }
@@ -625,11 +621,11 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       // and every window costs two extra HBM round trips.  Accesses of the transform streams inside the window
       // are "persisting" (a set-aside part of L2 that normal traffic cannot evict); the kernels additionally
       // mark their one-shot outputs as streaming (st.global.cs).
-      if ((big == 32768 || big == 16384 || big == 8192) && !getenv("SDB_NO_L2_PIN")) {   // the set-aside is device-wide: only the big plans claim it
+      if (big->path == SDB_FFT_F5) {   // the set-aside is device-wide: only the F.5 plans claim it
         int max_persist = 0, max_window = 0;
         cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, e->prm.device);
         cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, e->prm.device);
-        const size_t bytes = (size_t) e->chunk_windows * big * sizeof(float2);
+        const size_t bytes = (size_t) e->chunk_windows * big->N * sizeof(float2);
         if (max_persist > 0 && max_window > 0) {
           const size_t set_aside = std::min(bytes, (size_t) max_persist);
           if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, set_aside) == cudaSuccess) {
@@ -651,15 +647,14 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
   // ---- channeliser plan
   e->max_hops = max_feed / (W / 2);
   if (K > 0) {
-    if (!make_four_step(e, W, &e->fs_st)) return fail("out of device memory");
     std::vector<int> binmap(W, -1);
     std::vector<char> need(W, 0);
     for (auto &c : e->channels)
       for (unsigned i = 0; i < 2 * c.halfw; ++i) need[(c.center + W - c.halfw + i) % W] = 1;
     int nb = 0;
     e->ka_mask = 0;
-    // bin k = k1 + N1 (ka + 16 kb): N1 = 256 (F.4) or W / 256 (F.5); the generic passes ignore the mask
-    const unsigned ka_shift = W == 32768 ? 7u : (W == 16384 ? 6u : (W == 8192 ? 5u : 8u));
+    // bin k = k1 + N1 (ka + 16 kb) on the cluster and F.5 paths; the Stockham passes ignore the mask
+    const int ka_shift = e->fs_st.ka_shift;
     for (unsigned b = 0; b < W; ++b) if (need[b]) { binmap[b] = nb++; e->ka_mask |= 1u << ((b >> ka_shift) & 15u); }
     e->n_bins = nb;
     e->d_binmap = e->dalloc<int>(W);
@@ -713,7 +708,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       return fail("out of device memory (channels)");
     // The inspector kernel of feed i runs beside the transforms of feed i + 1.  Its CTAs are few and long-lived; the
     // highest priority places them as soon as SM space frees up instead of after every CTA of a transform grid
-    // queued before them (65536 points: one grid per feed) has been dispatched.
+    // queued before them (the cluster path: one grid per feed) has been dispatched.
     int prio_least = 0, prio_greatest = 0;
     CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
     CK(cudaStreamCreateWithPriority(&e->insp_stream, cudaStreamNonBlocking, prio_greatest));
@@ -882,67 +877,52 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
   const int shift_db = (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) ? 1 : 0;
   const int ob = (int) (e->feed_index & 1u);     // result buffers of this feed
 
-  // transform launchers: windows [w0, w0 + cw) of the flattened [stream][window] order, scratch region `scr`
-  auto psd_chunk = [&](const SdbLaunchCtx &lc, int frames, int w0, int cw, float2 *scr) -> int {
-    SdbPassAArgs a{};
-    a.x = x; a.fmt = fmt; a.stream_stride = stride; a.hist = nullptr; a.hist_len = 0;
-    a.windows_per_stream = frames; a.first_window = 0; a.hop = (int) Np; a.base_off = 0;
-    a.window = e->d_window; a.scratch = scr;
-    const bool fast = e->fs_psd.N2 == 256 && e->fs_psd.N1 >= 32 && e->fs_psd.N1 <= 128;        // SPEC F.5
-    e->span_begin(FAM_COLS, lc.stream);
-    if (fast) CK(sdb_launch_cols128(lc, e->fs_psd, a, w0, cw));
-    else      CK(sdb_launch_pass_a_range(lc, e->fs_psd, a, w0, cw));
-    e->span_end(lc.stream);
-    SdbPassBArgs b{};
-    b.scratch = scr; b.n_windows = cw; b.psd = e->d_psd + (size_t) w0 * Np;
-    b.inv_n = 1.0f / (float) Np; b.shift_db = shift_db;
-    e->span_begin(FAM_ROWS_PSD, lc.stream);
-    if (fast) CK(sdb_launch_rows256(lc, e->fs_psd, b, 0));
-    else      CK(sdb_launch_pass_b_psd(lc, e->fs_psd, b));
-    e->span_end(lc.stream);
-    return 0;
-  };
-  auto chan_chunk = [&](const SdbLaunchCtx &lc, int wps, int first, int w0, int cw, float2 *scr) -> int {
-    SdbPassAArgs a{};
-    a.x = x; a.fmt = fmt; a.stream_stride = stride; a.hist = e->d_hist; a.hist_len = (int) (W / 2);
-    a.windows_per_stream = wps; a.first_window = first; a.hop = (int) (W / 2); a.base_off = 0;
-    a.window = nullptr; a.scratch = scr;
-    const bool fast = e->fs_st.N2 == 256 && e->fs_st.N1 >= 32 && e->fs_st.N1 <= 128;
-    e->span_begin(FAM_COLS, lc.stream);
-    if (fast) CK(sdb_launch_cols128(lc, e->fs_st, a, w0, cw));
-    else      CK(sdb_launch_pass_a_range(lc, e->fs_st, a, w0, cw));
-    e->span_end(lc.stream);
-    SdbPassBArgs b{};
-    b.scratch = scr; b.n_windows = cw; b.binmap = e->d_binmap;
-    b.cspec = e->d_cspec + (size_t) w0 * e->n_bins; b.n_bins = e->n_bins; b.ka_mask = e->ka_mask;
-    e->span_begin(FAM_ROWS_CHAN, lc.stream);
-    if (fast) CK(sdb_launch_rows256(lc, e->fs_st, b, 1));
-    else      CK(sdb_launch_pass_b_chan(lc, e->fs_st, b));
-    e->span_end(lc.stream);
-    return 0;
-  };
-
   const int frames = Np ? (int) (n / Np) : 0;
   const int H = K ? (int) (n / (W / 2)) : 0;
   const int first = (K && e->first_feed) ? 1 : 0;
   const int wps = K ? H - first : 0;
-  // Stream groups: G whole streams per step, PSD frames on psd_stream and channeliser windows on the main stream,
-  // each with its own part of the pinned scratch (G * (frames + wps) windows <= chunk_windows).
-  int G = 0;
-  if (e->psd_stream && Np && !e->psd_small && wps > 0) {
-    G = e->chunk_windows / (frames + wps);
-    // the largest group that fits the pinned scratch is the fastest (cfg2, 2048 streams: 12 streams 64.7 GS/s,
-    // 9 streams -- whole waves for either kernel alone -- 63.1, 8: 60.2, 6: 54.2; the two chains overlap, so
-    // wave quantisation of a single launch does not matter)
-    if (const char *env = getenv("SDB_GROUP_STREAMS")) { const long v = atol(env); if (v >= 1 && v <= G * 4) G = (int) v; }
-    if ((size_t) G * (frames + wps) > (size_t) e->chunk_windows) G = e->chunk_windows / (frames + wps);
-  }
-  if (G > (int) S) G = (int) S;
-
+  // arguments of the two-kernel transforms: PSD frames (hop Np, no history) and channeliser windows (hop W / 2 over
+  // the W / 2-sample history followed by x)
+  SdbPassAArgs psd_a{}, chan_a{};
+  psd_a.x = chan_a.x = x; psd_a.fmt = chan_a.fmt = fmt; psd_a.stream_stride = chan_a.stream_stride = stride;
+  psd_a.windows_per_stream = frames; psd_a.hop = (int) Np; psd_a.window = e->d_window;
+  chan_a.hist = e->d_hist; chan_a.hist_len = (int) (W / 2);
+  chan_a.windows_per_stream = wps; chan_a.first_window = first; chan_a.hop = (int) (W / 2);
+  SdbPassBArgs psd_b{}, chan_b{};
+  psd_b.shift_db = shift_db;
+  chan_b.binmap = e->d_binmap; chan_b.cspec = e->d_cspec; chan_b.n_bins = e->n_bins; chan_b.ka_mask = e->ka_mask;
   if (Np) {
     e->last_frames = frames;
     e->d_psd = e->d_psdb[ob];
+    psd_b.psd = e->d_psd; psd_b.inv_n = 1.0f / (float) Np;
   }
+  // windows [w0, w0 + cw) of the flattened [stream][window] order through scratch region `scr`; pass B is timed as
+  // family `fam_b` (FAM_ROWS_PSD: PSD epilogue, FAM_ROWS_CHAN: channeliser scatter)
+  auto chunk = [&](const SdbLaunchCtx &lc, const SdbFourStep &fs, SdbPassAArgs a, SdbPassBArgs b, int fam_b, int w0,
+                   int cw, float2 *scr) -> int {
+    const int mode = fam_b == FAM_ROWS_CHAN ? 1 : 0;
+    const bool f5 = fs.path == SDB_FFT_F5;
+    a.scratch = scr;
+    b.scratch = scr; b.n_windows = cw;
+    if (mode) b.cspec += (size_t) w0 * b.n_bins;
+    else      b.psd += (size_t) w0 * fs.N;
+    e->span_begin(FAM_COLS, lc.stream);
+    if (f5) CK(sdb_launch_cols128(lc, fs, a, w0, cw));
+    else    CK(sdb_launch_pass_a_range(lc, fs, a, w0, cw));
+    e->span_end(lc.stream);
+    e->span_begin(fam_b, lc.stream);
+    if (f5) CK(sdb_launch_rows256(lc, fs, b, mode));
+    else    CK(sdb_launch_pass_b(lc, fs, b, mode));
+    e->span_end(lc.stream);
+    return 0;
+  };
+
+  // Stream groups: G whole streams per step, PSD frames on psd_stream and channeliser windows on the main stream,
+  // each with its own part of the pinned scratch (G * (frames + wps) windows <= chunk_windows).  The largest group
+  // that fits the pinned scratch is the fastest (cfg2, 2048 streams: 12 streams 64.7 GS/s, 9 streams -- whole waves
+  // for either kernel alone -- 63.1, 8: 60.2, 6: 54.2; the two chains overlap, so wave quantisation of a single
+  // launch does not matter).
+  const int G = e->psd_stream && wps > 0 ? std::min(e->chunk_windows / (frames + wps), (int) S) : 0;
   if (G >= 1) {
     // timing mode (sdb_engine_timing): every kernel on the main stream, so that the CUDA-event spans are the
     // kernels' own durations and not those of two chains sharing the SMs
@@ -953,8 +933,8 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     float2 *scr_psd = e->d_scratch, *scr_ch = e->d_scratch + (size_t) G * frames * Np;
     for (int s0 = 0; s0 < (int) S; s0 += G) {
       const int g = std::min(G, (int) S - s0);
-      if (psd_chunk(pctx, frames, s0 * frames, g * frames, scr_psd)) return -1;
-      if (chan_chunk(ctx, wps, first, s0 * wps, g * wps, scr_ch)) return -1;
+      if (chunk(pctx, e->fs_psd, psd_a, psd_b, FAM_ROWS_PSD, s0 * frames, g * frames, scr_psd)) return -1;
+      if (chunk(ctx, e->fs_st, chan_a, chan_b, FAM_ROWS_CHAN, s0 * wps, g * wps, scr_ch)) return -1;
     }
     if (e->chdet) CK(sdb_chdet_feed_stream(e->chdet, e->d_psd, (uint32_t) frames, (size_t) frames * Np, e->psd_stream,
                                            &e->launches));
@@ -962,29 +942,31 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     CK(cudaStreamWaitEvent(e->stream, e->ev_psd_ready[ob], 0));   // the main stream stays the engine's timeline
   } else {
     if (Np && e->psd_read_valid[ob]) CK(cudaStreamWaitEvent(e->stream, e->ev_psd_read[ob], 0));   // async read of feed i-2
-    // ---- 65536-point PSD frames and channeliser windows: one launch, both passes fused, ordered by stream
-    const bool fused_psd = Np == 65536, fused_chan = K && W == 65536;
+    // ---- cluster-path PSD frames and channeliser windows: one launch, both passes fused, ordered by stream
+    const bool fused_psd = Np && e->fs_psd.path == SDB_FFT_CLUSTER, fused_chan = K && e->fs_st.path == SDB_FFT_CLUSTER;
     if ((fused_psd && frames > 0) || (fused_chan && wps > 0)) {
+      const SdbFourStep &fs = fused_psd ? e->fs_psd : e->fs_st;
       SdbFft65536Args f{};
       f.x = x; f.fmt = fmt; f.stream_stride = stride; f.n_streams = (int) S;
       f.n_psd = fused_psd ? frames : 0; f.n_chan = fused_chan ? wps : 0; f.first_chan = first;
-      f.window = e->d_window; f.psd = e->d_psd; f.inv_n = 1.0f / 65536.0f; f.shift_db = shift_db;
+      f.window = e->d_window; f.psd = e->d_psd; f.inv_n = 1.0f / (float) fs.N; f.shift_db = shift_db;
       f.hist = e->d_hist; f.binmap = e->d_binmap; f.cspec = e->d_cspec; f.n_bins = e->n_bins; f.ka_mask = e->ka_mask;
       e->span_begin(FAM_COLS);
-      CK(sdb_launch_fft65536(ctx, fused_psd ? e->fs_psd : e->fs_st, f));
+      CK(sdb_launch_fft65536(ctx, fs, f));
       e->span_end();
     }
     // ---- main PSD
     if (Np) {
-      if (e->psd_small) {
+      if (e->fs_psd.path == SDB_FFT_SMALL_PSD) {
         e->span_begin(FAM_ROWS_PSD);
-        CK(sdb_launch_small_psd(ctx, (int) Np, e->twiddle(Np), x, fmt, stride, frames, (int) S, e->d_window,
+        CK(sdb_launch_small_psd(ctx, (int) Np, e->fs_psd.twN, x, fmt, stride, frames, (int) S, e->d_window,
                                 e->d_psd, shift_db));
         e->span_end();
       } else if (!fused_psd) {
         const int total = frames * (int) S;
         for (int w0 = 0; w0 < total; w0 += e->chunk_windows)
-          if (psd_chunk(ctx, frames, w0, std::min(e->chunk_windows, total - w0), e->d_scratch)) return -1;
+          if (chunk(ctx, e->fs_psd, psd_a, psd_b, FAM_ROWS_PSD, w0, std::min(e->chunk_windows, total - w0),
+                    e->d_scratch)) return -1;
       }
       if (e->chdet) CK(sdb_chdet_feed_stream(e->chdet, e->d_psd, (uint32_t) frames, (size_t) frames * Np, e->stream,
                                              &e->launches));
@@ -994,7 +976,8 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     if (K && wps > 0 && !fused_chan) {
       const int total = wps * (int) S;
       for (int w0 = 0; w0 < total; w0 += e->chunk_windows)
-        if (chan_chunk(ctx, wps, first, w0, std::min(e->chunk_windows, total - w0), e->d_scratch)) return -1;
+        if (chunk(ctx, e->fs_st, chan_a, chan_b, FAM_ROWS_CHAN, w0, std::min(e->chunk_windows, total - w0),
+                  e->d_scratch)) return -1;
     }
   }
   // ---- per-channel inverse transforms + inspectors

@@ -250,7 +250,7 @@ static __device__ __forceinline__ void fft8(float2 (&v)[8])
 struct Cols256K {
   const void *x; int fmt; size_t stream_stride;
   const float2 *hist; int hist_len;
-  int windows_per_stream, first_window, hop, base_off, win_base;
+  int windows_per_stream, first_window, hop, win_base;
   const float *window;
   float2 *scratch;
   const float2 *tw256;     // W_N1^i
@@ -271,7 +271,7 @@ __global__ void __launch_bounds__(128, 8) k_cols16T(const Cols256K p)
   const int stream = w / p.windows_per_stream;
   const int j0 = p.first_window + (w - stream * p.windows_per_stream);
   const int col = blockIdx.x * C + c;
-  const long v0 = (long) p.base_off + (long) j0 * p.hop;
+  const long v0 = (long) j0 * p.hop;
   const int fmt = p.fmt;
   const char *__restrict__ xs = reinterpret_cast<const char *>(p.x) + (size_t) stream * p.stream_stride * sdb_fmt_bytes(fmt);
   const float2 *__restrict__ hs = p.hist ? p.hist + (size_t) stream * p.hist_len : nullptr;
@@ -331,7 +331,7 @@ cudaError_t sdb_launch_cols128(const SdbLaunchCtx &c, const SdbFourStep &fs, con
   Cols256K p;
   p.x = a.x; p.fmt = a.fmt; p.stream_stride = a.stream_stride; p.hist = a.hist; p.hist_len = a.hist_len;
   p.windows_per_stream = a.windows_per_stream; p.first_window = a.first_window; p.hop = a.hop;
-  p.base_off = a.base_off; p.win_base = win_base; p.window = a.window; p.scratch = a.scratch;
+  p.win_base = win_base; p.window = a.window; p.scratch = a.scratch;
   p.tw256 = fs.twN1; p.twpq = fs.twPQ;
   const int T = fs.N1 / 16;                         // 8, 4 or 2: columns per CTA = 128 / T
   dim3 grid(256 / (128 / T), n_win);

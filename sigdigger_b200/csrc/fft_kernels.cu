@@ -128,7 +128,7 @@ __global__ void __launch_bounds__(1024) k_pass_a(const PassAK p)
   const int stream = w / p.a.windows_per_stream;
   const int j = p.a.first_window + (w - stream * p.a.windows_per_stream);
   const int col0 = blockIdx.x * CW;
-  const long v0 = (long) p.a.base_off + (long) j * p.a.hop;
+  const long v0 = (long) j * p.a.hop;
   const int fmt = p.a.fmt;
   const char *__restrict__ xs = reinterpret_cast<const char *>(p.a.x) + (size_t) stream * p.a.stream_stride * sdb_fmt_bytes(fmt);
   const float2 *__restrict__ hs = p.a.hist ? p.a.hist + (size_t) stream * p.a.hist_len : nullptr;
@@ -237,8 +237,7 @@ __global__ void __launch_bounds__(1024) k_pass_b(const PassBK p)
   }
 }
 
-static cudaError_t launch_pass_b(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a,
-                                 int mode)
+cudaError_t sdb_launch_pass_b(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a, int mode)
 {
   PassBK p;
   p.fs = fs; p.a = a;
@@ -257,15 +256,6 @@ static cudaError_t launch_pass_b(const SdbLaunchCtx &c, const SdbFourStep &fs, c
   else           k_pass_b<1><<<grid, threads, smem, c.stream>>>(p);
   if (c.launch_counter) ++*c.launch_counter;
   return cudaGetLastError();
-}
-
-cudaError_t sdb_launch_pass_b_psd(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a)
-{
-  return launch_pass_b(c, fs, a, 0);
-}
-cudaError_t sdb_launch_pass_b_chan(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a)
-{
-  return launch_pass_b(c, fs, a, 1);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -498,17 +488,17 @@ cudaError_t sdb_launch_spectsrc(const SdbLaunchCtx &c, const SdbSpectCfg *cfg_de
 }
 
 // ---------------------------------------------------------------------------------------------
-// channeliser inverse side.  One CTA per (channel, stream).  Only the cross-fade couples consecutive hops (it needs
-// the second half of the previous hop's IFFT), so the CTA transforms P hops at a time -- P x size/4 threads, every
-// barrier of the shared-memory transform paid once per P hops, P gathers in flight -- and cross-fades them from the
-// buffers of their left neighbours; the last hop's second half is carried in shared memory (and between feeds in
-// `tails`).  Round 1 ran one hop at a time with size/4 threads: 22 us per 2048-point hop against < 1 us of work.
+// channeliser inverse side.  One CTA per (channel, stream) transforms the channel's hops one after the other.  Only
+// the cross-fade couples consecutive hops (it needs the second half of the previous hop's IFFT), which is carried in
+// shared memory (and between feeds in `tails`).  One hop per pass: measured on cfg3 (1024-point channels, 8 hops),
+// four hops per pass (1024-thread CTAs, 2 per SM) took 1.21 ms against 0.85 ms for one (256-thread CTAs, 8 per SM);
+// the barriers of a big CTA cost more than the hops it overlaps.
 // ---------------------------------------------------------------------------------------------
 template <int BPT>
 __global__ void __launch_bounds__(1024) k_chan_ifft(const SdbChannelDev *__restrict__ chans,
                                                      const int *__restrict__ group, int n_channels,
                                                      const float2 *__restrict__ cspec, int n_bins,
-                                                     int wps, int P, float2 *__restrict__ tails,
+                                                     int wps, float2 *__restrict__ tails,
                                                      size_t tail_stream_stride, float *__restrict__ lo_phase,
                                                      float2 *__restrict__ chan_out, size_t chan_stream_stride)
 {
@@ -517,30 +507,25 @@ __global__ void __launch_bounds__(1024) k_chan_ifft(const SdbChannelDev *__restr
   const SdbChannelDev ch = chans[ci];
   const int s = blockIdx.y;
   const int size = ch.size, hs = ch.halfsz, hw = ch.halfw;
-  // With P = 1 (every size above 4096, and the default for the others) each prevb[i] is read and then rewritten by
-  // the one thread that owns i, so a single buffer serves both roles; with P > 1 group 0 reads the previous round's
-  // half while group P - 1 writes the next one, hence two.  The phase buffer sits behind it (precise groups only).
-  const int nprev = P > 1 ? 2 : 1;
-  float2 *bufs = sm;                                   // [P][size]
-  float2 *prevb[2] = { sm + (size_t) P * size, sm + (size_t) P * size + (nprev - 1) * hs };
-  float *phase = reinterpret_cast<float *>(sm + (size_t) P * size + nprev * hs);   // [P][hs]
+  // Each prev[i] is read and then rewritten by the one thread that owns i, so a single buffer carries the previous
+  // hop's second half.  The phase buffer sits behind it (precise groups only).
+  float2 *buf = sm;                                    // [size]
+  float2 *prev = sm + size;                            // [hs]
+  float *phase = reinterpret_cast<float *>(sm + size + hs);   // [hs]
   const int tid = threadIdx.x;
   const int per = BPT == 1 ? (size >= 4 ? size >> 2 : 1) : (int) blockDim.x;   // threads per hop
-  const int g = tid / per, l = tid - g * per;
+  const bool active = tid < per;                       // channels below 128 points run in a CTA padded to 32 threads
+  const int l = tid;
   float2 *__restrict__ tail = tails + (size_t) s * tail_stream_stride + ch.tail_off;
   float2 *__restrict__ out = chan_out + (size_t) s * chan_stream_stride + ch.out_off;
 
-  for (int i = tid; i < hs; i += blockDim.x) prevb[0][i] = tail[i];
+  for (int i = tid; i < hs; i += blockDim.x) prev[i] = tail[i];
   float lo_phi = ch.precise ? lo_phase[(size_t) s * n_channels + ci] : 0.0f;
-  int pb = 0;
   __syncthreads();
 
-  for (int j0 = 0; j0 < wps; j0 += P) {
-    const int Pg = wps - j0 < P ? wps - j0 : P;        // hops in this group
-    const bool active = g < Pg;
-    float2 *buf = bufs + (size_t) (active ? g : 0) * size;
+  for (int j = 0; j < wps; ++j) {
     if (active) {
-      const float2 *__restrict__ cs = cspec + ((size_t) s * wps + j0 + g) * n_bins;
+      const float2 *__restrict__ cs = cspec + ((size_t) s * wps + j) * n_bins;
       // zero the guard region between the two sidebands, then gather + shape the channel's bins
       for (int i = hw + l; i < size - hw; i += per) buf[i] = make_float2(0.0f, 0.0f);
       for (int i = l; i < 2 * hw; i += per) {
@@ -555,7 +540,7 @@ __global__ void __launch_bounds__(1024) k_chan_ifft(const SdbChannelDev *__restr
     if (ch.precise && tid == 0) {
       // sequential phase accumulation, exactly as the per-sample NCQO would do it
       float phi = lo_phi;
-      for (int i = 0; i < Pg * hs; ++i) {
+      for (int i = 0; i < hs; ++i) {
         phase[i] = phi;
         phi += ch.lo_omega;
         if (phi >= 6.28318530717958647692f) phi -= 6.28318530717958647692f;
@@ -566,24 +551,22 @@ __global__ void __launch_bounds__(1024) k_chan_ifft(const SdbChannelDev *__restr
     __syncthreads();
     block_fft_inplace<+1, BPT>(buf, size, ch.log2size, active ? l : size, per, ch.tw);
     if (active) {
-      const float2 *pvb = g > 0 ? buf - size + hs : prevb[pb];
       for (int i = l; i < hs; i += per) {
         const float al = __ldg(ch.xfade + i), be = __ldg(ch.xfade + i + hs);
-        const float2 cu = buf[i], pv = pvb[i];
+        const float2 cu = buf[i], pv = prev[i];
         float2 o = make_float2(al * cu.x + be * pv.x, al * cu.y + be * pv.y);
         if (ch.precise) {
           float sn, cs_;
-          d_sincosf(phase[g * hs + i], &sn, &cs_);            // SPEC M.1, as the per-sample NCQO read does
+          d_sincosf(phase[i], &sn, &cs_);                   // SPEC M.1, as the per-sample NCQO read does
           o = cmulc(o, make_float2(cs_, sn));
         }
-        out[(size_t) (j0 + g) * hs + i] = o;
-        if (g == Pg - 1) prevb[pb ^ 1][i] = buf[i + hs];
+        out[(size_t) j * hs + i] = o;
+        prev[i] = buf[i + hs];
       }
     }
-    pb ^= 1;
     __syncthreads();
   }
-  for (int i = tid; i < hs; i += blockDim.x) tail[i] = prevb[pb][i];
+  for (int i = tid; i < hs; i += blockDim.x) tail[i] = prev[i];
   if (ch.precise && tid == 0) lo_phase[(size_t) s * n_channels + ci] = lo_phi;
 }
 
@@ -829,37 +812,21 @@ cudaError_t sdb_launch_chan_ifft_group(const SdbLaunchCtx &c, const SdbChannelDe
   }
   int bpt = 1, threads = size / 4;
   while (threads > 1024) { threads >>= 1; bpt <<= 1; }
-  // hops per pass.  Measured on cfg3 (1024-point channels, 8 hops): P = 4 (1024-thread CTAs, 2 per SM) 1.21 ms
-  // against 0.85 ms for P = 1 (256-thread CTAs, 8 per SM): the barriers of a big CTA cost more than the hops it
-  // overlaps, so one hop per pass stays the default (SDB_IFFT_HOPS overrides for experiments).
-  int P = 1;
-  static const int env_hops = getenv("SDB_IFFT_HOPS") ? atoi(getenv("SDB_IFFT_HOPS")) : 1;
-  if (bpt == 1 && env_hops > 1) {
-    const int per = size >= 4 ? size / 4 : 1;
-    P = 1024 / per;
-    if (P > env_hops) P = env_hops;
-    if (P > wps) P = wps;
-    if ((size_t) P * size > 8192) P = (int) (8192 / size);
-    if (P < 1) P = 1;
-    threads = ((P * per + 31) / 32) * 32;
-  } else if (bpt == 1) {
-    threads = size / 4;
-  }
   if (threads < 32) threads = 32;
-  const size_t smem = (size_t) P * size * sizeof(float2) + (size_t) (P > 1 ? 2 : 1) * (size / 2) * sizeof(float2)
-                      + (any_precise ? (size_t) P * (size / 2) * sizeof(float) : 0);
+  const size_t smem = (size_t) size * sizeof(float2) + (size_t) (size / 2) * sizeof(float2)
+                      + (any_precise ? (size_t) (size / 2) * sizeof(float) : 0);
   if (smem > smem_cap) return cudaErrorInvalidValue;
   dim3 grid(group_len, n_streams);
   if (bpt == 1)
-    k_chan_ifft<1><<<grid, threads, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps, P,
+    k_chan_ifft<1><<<grid, threads, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps,
                                                       tails, tail_stream_stride, lo_phase, chan_out,
                                                       chan_stream_stride);
   else if (bpt == 2)
-    k_chan_ifft<2><<<grid, threads, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps, P,
+    k_chan_ifft<2><<<grid, threads, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps,
                                                       tails, tail_stream_stride, lo_phase, chan_out,
                                                       chan_stream_stride);
   else if (bpt == 4)
-    k_chan_ifft<4><<<grid, threads, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps, P,
+    k_chan_ifft<4><<<grid, threads, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps,
                                                       tails, tail_stream_stride, lo_phase, chan_out,
                                                       chan_stream_stride);
   else

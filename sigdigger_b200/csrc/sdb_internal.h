@@ -26,12 +26,22 @@ static inline bool sdb_first_on_device(std::atomic<unsigned long long> &mask)
 // ---------------------------------------------------------------------------------------------
 // FFT plan pieces (fft_kernels.cu)
 // ---------------------------------------------------------------------------------------------
+// The kernels that transform one window (the engine's transform plan picks the path from the size and the role)
+enum SdbFftPath {
+  SDB_FFT_SMALL_PSD,        // PSD, N <= 4096: k_small_psd, one CTA per frame
+  SDB_FFT_CLUSTER,          // N = 65536: k_fft65536, both passes in one thread-block cluster
+  SDB_FFT_F5,               // N = 8192 / 16384 / 32768 = N1 x 256 (SPEC F.5): k_cols16T + k_rows256 through the scratch
+  SDB_FFT_STOCKHAM,         // every other size: k_pass_a + k_pass_b through the scratch
+};
+
 struct SdbFourStep {
+  int path;                 // SdbFftPath
   int N, N1, N2;            // N = N1 * N2; pass A does N1-point column FFTs, pass B N2-point row FFTs
+  int ka_shift;             // log2(N1): bin k = k1 + N1 (ka + 16 kb) on the cluster and F.5 paths
   const float2 *twN1;       // W_N1^i, i < N1 (forward sign)
   const float2 *twN2;
   const float2 *twN;        // W_N^i, i < N
-  const float2 *twPQ;       // N = 65536 / 32768: SPEC F.4 / F.5 inter-pass twiddle [k1][n2] = W_N1^(p>>8) x W_N^(p&255), p = n2 k1
+  const float2 *twPQ;       // cluster / F.5: SPEC F.4 / F.5 inter-pass twiddle [k1][n2] = W_N1^(p>>8) x W_N^(p&255), p = n2 k1
 };
 
 struct SdbPassAArgs {
@@ -42,8 +52,7 @@ struct SdbPassAArgs {
   int           hist_len;
   int           windows_per_stream; // windows handled per stream in this launch
   int           first_window;       // index of the first window (per stream) in this launch
-  int           hop;                // samples between consecutive windows
-  int           base_off;           // offset of window 0 in the virtual buffer hist ++ x
+  int           hop;                // samples between consecutive windows; window 0 starts the virtual buffer hist ++ x
   const float  *window;             // N taps or null
   float2       *scratch;            // [launch windows][N1][N2] as [k1][n2]
 };
@@ -267,8 +276,8 @@ cudaError_t sdb_launch_pass_a_range(const SdbLaunchCtx &c, const SdbFourStep &fs
 cudaError_t sdb_launch_fft65536(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbFft65536Args &a);
 cudaError_t sdb_launch_cols128(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassAArgs &a, int win_base, int n_win);
 cudaError_t sdb_launch_rows256(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a, int mode);
-cudaError_t sdb_launch_pass_b_psd(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a);
-cudaError_t sdb_launch_pass_b_chan(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a);
+// mode 0: PSD epilogue, 1: channeliser scatter
+cudaError_t sdb_launch_pass_b(const SdbLaunchCtx &c, const SdbFourStep &fs, const SdbPassBArgs &a, int mode);
 cudaError_t sdb_launch_hist_convert(cudaStream_t s, const void *x, int fmt, size_t stream_stride, size_t offset,
                                     float2 *hist, int hist_len, int n_streams);
 cudaError_t sdb_launch_small_psd(const SdbLaunchCtx &c, int N, const float2 *tw, const void *x, int fmt,

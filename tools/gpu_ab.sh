@@ -1,6 +1,6 @@
 #!/bin/bash
 # A/B of this tree's library against one built from the parent commit, parent and new alternating (cfg3 three runs
-# each, cfg2 / cfg5 / cfg4 two), then bench.py --dump-outputs of both on cfg3, cfg2 and cfg5 for an output comparison.
+# each, cfg2 / cfg5 / cfg4 two), then bench.py --dump-outputs of both on cfg3, cfg2, cfg5 and cfg4 for an output comparison.
 # Usage: bash tools/gpu_ab.sh <parent library .so> [output directory, default: a new temporary directory]
 # The new arm also loads its library through SDB_LIB, so that both arms run the same bench.py legs.
 PARENT=${1:?parent library}
@@ -23,7 +23,7 @@ PY
 for w in cfg3:3 cfg2:2 cfg5:2 cfg4:2; do
   for i in $(seq 1 ${w#*:}); do run parent ${w%:*} $i; run new ${w%:*} $i; done
 done
-for w in cfg3 cfg2 cfg5; do
+for w in cfg3 cfg2 cfg5 cfg4; do
   for arm in parent new; do
     lib=$PARENT; [ $arm = new ] && lib=$NEW
     SDB_LIB=$lib timeout 300 python bench.py --workload $w --steps 2 --warmup 1 --no-cpu --no-formats --no-single \
