@@ -1,4 +1,4 @@
-// chain_kernels.cu -- per-channel inspector chains and Tasks/ primitives as serial recurrences, one
+// chain_kernels.cu -- per-channel inspector chains as serial recurrences, one
 // GPU thread per (stream, channel) chain with the loop state carried in registers for the whole
 // batch of channel samples (persistent across feeds through SdbChainState).
 //
@@ -66,7 +66,7 @@ __device__ unsigned long long g_role_cls[5][8];      // the same, by inspector c
 #ifdef SDB_STAGE_CYCLES
 __device__ unsigned long long g_cta_cycles[24];
 #endif
-cudaError_t sdb_stage_cta_cycles(unsigned long long out[64], int reset)
+static cudaError_t sdb_stage_cta_cycles(unsigned long long out[64], int reset)
 {
 #ifdef SDB_STAGE_CYCLES
   cudaError_t e = cudaMemcpyFromSymbol(out, g_cta_cycles, sizeof(unsigned long long) * 24);
@@ -84,7 +84,7 @@ cudaError_t sdb_stage_cta_cycles(unsigned long long out[64], int reset)
   return cudaSuccess;
 #endif
 }
-cudaError_t sdb_stage_cycles(unsigned long long out[8], int reset)
+static cudaError_t sdb_stage_cycles(unsigned long long out[8], int reset)
 {
 #ifdef SDB_STAGE_CYCLES
   cudaError_t e = cudaMemcpyFromSymbol(out, g_stage_cycles, sizeof(unsigned long long) * 8);
@@ -99,6 +99,25 @@ cudaError_t sdb_stage_cycles(unsigned long long out[8], int reset)
   return cudaSuccess;
 #endif
 }
+
+extern "C" int sdb_debug_stage_cycles(uint64_t out[8], int reset)
+{
+  unsigned long long tmp[8];
+  CK(cudaDeviceSynchronize());
+  CK(sdb_stage_cycles(tmp, reset));
+  for (int i = 0; i < 8; ++i) out[i] = tmp[i];
+  return 0;
+}
+
+extern "C" int sdb_debug_cta_cycles(uint64_t out[64], int reset)
+{
+  unsigned long long tmp[64];
+  CK(cudaDeviceSynchronize());
+  CK(sdb_stage_cta_cycles(tmp, reset));
+  for (int i = 0; i < 64; ++i) out[i] = tmp[i];
+  return 0;
+}
+
 static __device__ __forceinline__ void cp_async8(void *smem_dst, const void *gsrc)
 {
   const unsigned sa = (unsigned) __cvta_generic_to_shared(smem_dst);
@@ -973,116 +992,5 @@ cudaError_t sdb_launch_inspectors_n(const SdbLaunchCtx &c, const SdbChainCfg *cf
       cfg_dev, n_channels, n_streams, chain_map, state, pool, pool_stride, taps_pool, chans_dev, chan_in,
       chan_stream_stride, n_hops, soft, hard, sym_counts, sym_cap, fresh, d2);
   if (c.launch_counter) ++*c.launch_counter;
-  return cudaGetLastError();
-}
-
-// ------------------------------------------------------------------ Tasks/ primitives -----------
-// One thread per buffer of the batch; same recurrences, state in registers.
-__global__ void k_task_xlate(const float2 *__restrict__ src, float2 *__restrict__ dst, size_t n, size_t batch,
-                             float omega, float phi0)
-{
-  size_t b = blockIdx.x * (size_t) blockDim.x + threadIdx.x;
-  if (b >= batch) return;
-  float phi = phi0;
-  const float2 *x = src + b * n;
-  float2 *y = dst + b * n;
-  for (size_t i = 0; i < n; ++i) {
-    float2 ph = ncqo_read(phi, omega);
-    float2 v = x[i];
-    y[i] = make_float2(v.x * ph.x - v.y * ph.y, v.x * ph.y + v.y * ph.x);
-  }
-}
-
-// quadrature demod has no loop-carried state beyond x[p-1]: fully parallel over samples
-__global__ void k_task_quad(const float2 *__restrict__ src, float2 *__restrict__ dst, size_t n, size_t batch)
-{
-  size_t i = blockIdx.x * (size_t) blockDim.x + threadIdx.x;
-  if (i >= n * batch) return;
-  size_t p = i % n;
-  if (p == 0) { dst[i] = make_float2(0.0f, 0.0f); return; }
-  float2 x = src[i], pv = src[i - 1];
-  float dr = x.x * pv.x + x.y * pv.y;
-  float di = x.y * pv.x - x.x * pv.y;
-  dst[i] = make_float2(0.0f, 0.318309886183790671538f * d_atan2f(di, dr));
-}
-
-// mode 0 Costas, 1 PLL, 2 AGC.  pool: per-buffer AGC arrays, interleaved by 32 buffers ([slot][lane]).
-__global__ void k_task_chain(const float2 *__restrict__ src, float2 *__restrict__ dst, size_t n, size_t batch,
-                             const SdbChainCfg *__restrict__ cp, int mode, float *pool, size_t pool_stride)
-{
-  size_t b = blockIdx.x * (size_t) blockDim.x + threadIdx.x;
-  if (b >= batch) return;
-  const float2 *x = src + b * n;
-  float2 *y = dst + b * n;
-  if (mode == 0) {
-    CostasK ck; CostasS cs;
-    ck.kind = cp->costas_kind; ck.af_n = cp->af_n; ck.a = cp->c_a; ck.b = cp->c_b;
-#pragma unroll
-    for (int i = 0; i < SDB_MAX_IIR; ++i) {
-      ck.af_b[i] = cp->af_b[i]; ck.af_a[i] = cp->af_a[i];
-      cs.xr[i] = cs.xi[i] = cs.yr[i] = cs.yi[i] = 0.0f;
-    }
-    cs.phi = cs.omega = cs.lock = cs.yre = cs.yim = 0.0f;
-    for (size_t i = 0; i < n; ++i) y[i] = costas_step(ck, cs, x[i]);
-  } else if (mode == 1) {
-    float phi = 0.0f, omega = 0.0f;
-    const float a = cp->pll_alpha, be = cp->pll_beta;
-    for (size_t i = 0; i < n; ++i) y[i] = pll_step(a, be, phi, omega, x[i]);
-  } else {
-    AgcK ak; AgcS as;
-    ak.knee = cp->knee; ak.slope_m1 = cp->gain_slope - 1.0f; ak.fixed_gain = cp->fixed_gain;
-    ak.far_ = cp->far_; ak.faf = cp->faf; ak.sar = cp->sar; ak.saf = cp->saf;
-    ak.hang_max = cp->hang_max; ak.dl_size = cp->dl_size; ak.mh_size = cp->mh_size;
-    as.fast = as.slow = as.peak = -160.0f; as.hang_n = as.dl_ptr = as.mh_ptr = 0;
-    float *bp = pool + (b / 32) * 32 * pool_stride + (b % 32);
-    float *dl = bp + (size_t) cp->st_dl_off * 32, *mh = bp + (size_t) cp->st_mh_off * 32;
-    for (unsigned i = 0; i < 2 * ak.dl_size; ++i) dl[i * 32] = 0.0f;
-    for (unsigned i = 0; i < ak.mh_size; ++i) mh[i * 32] = -160.0f;
-    for (size_t i = 0; i < n; ++i) y[i] = agc_step(ak, as, dl, mh, x[i]);
-  }
-}
-
-// One buffer, loop state handed in and out (the bulk twins of su_costas_feed / su_pll_track: a Tasks/ work()
-// block continues where the previous one stopped).  mode 0: st = CostasK ++ CostasS, 1: st = {alpha, beta, phi, omega}
-__global__ void k_task_chain_state(const float2 *__restrict__ x, float2 *__restrict__ y, size_t n, int mode,
-                                   float *__restrict__ st)
-{
-  if (blockIdx.x != 0 || threadIdx.x != 0) return;
-  if (mode == 0) {
-    CostasK ck = *reinterpret_cast<const CostasK *>(st);
-    CostasS cs = *reinterpret_cast<const CostasS *>(reinterpret_cast<const unsigned char *>(st) + sizeof(CostasK));
-    for (size_t i = 0; i < n; ++i) y[i] = costas_step(ck, cs, x[i]);
-    *reinterpret_cast<CostasS *>(reinterpret_cast<unsigned char *>(st) + sizeof(CostasK)) = cs;
-  } else {
-    const float a = st[0], be = st[1];
-    float phi = st[2], omega = st[3];
-    for (size_t i = 0; i < n; ++i) y[i] = pll_step(a, be, phi, omega, x[i]);
-    st[2] = phi; st[3] = omega;
-  }
-}
-cudaError_t sdb_launch_task_chain_state(cudaStream_t s, const float2 *src, float2 *dst, size_t n, int mode, float *st)
-{
-  k_task_chain_state<<<1, 32, 0, s>>>(src, dst, n, mode, st);
-  return cudaGetLastError();
-}
-size_t sdb_costas_k_bytes(void) { return sizeof(CostasK); }
-size_t sdb_costas_s_bytes(void) { return sizeof(CostasS); }
-
-cudaError_t sdb_launch_task_xlate(cudaStream_t s, const float2 *src, float2 *dst, size_t n, size_t batch,
-                                  float omega, float phi0)
-{
-  k_task_xlate<<<(unsigned) ((batch + 31) / 32), 32, 0, s>>>(src, dst, n, batch, omega, phi0);
-  return cudaGetLastError();
-}
-cudaError_t sdb_launch_task_quad(cudaStream_t s, const float2 *src, float2 *dst, size_t n, size_t batch)
-{
-  size_t tot = n * batch;
-  k_task_quad<<<(unsigned) ((tot + 255) / 256), 256, 0, s>>>(src, dst, n, batch);
-  return cudaGetLastError();
-}
-cudaError_t sdb_launch_task_chain(cudaStream_t s, const float2 *src, float2 *dst, size_t n, size_t batch,
-                                  const SdbChainCfg *cfg_dev, int mode, float *pool, size_t pool_stride)
-{
-  k_task_chain<<<(unsigned) ((batch + 31) / 32), 32, 0, s>>>(src, dst, n, batch, cfg_dev, mode, pool, pool_stride);
   return cudaGetLastError();
 }

@@ -341,14 +341,11 @@ __global__ void __launch_bounds__(1024) k_chdet_fused(const ChdetFusedK q)
 // ---------------------------------------------------------------------------------------------
 // host object + C-ABI
 // ---------------------------------------------------------------------------------------------
-static thread_local std::string g_chdet_err;
-extern "C" const char *sdb_last_error(void);
-
 struct sdb_chdet {
   int device = 0; unsigned N = 0, S = 0, min_bins = 1;
   float alpha = 0, gamma = 0, snr = 0;
-  float *d_avg = nullptr, *d_n0 = nullptr; int *d_n0_primed = nullptr;
-  SdbDetectedDev *d_out = nullptr; unsigned *d_count = nullptr, *d_total = nullptr;
+  DevBuf<float> d_avg, d_n0; DevBuf<int> d_n0_primed;
+  DevBuf<SdbDetectedDev> d_out; DevBuf<unsigned> d_count, d_total;
   bool primed = false;
 };
 
@@ -356,8 +353,6 @@ extern "C" void sdb_chdet_destroy(sdb_chdet_t *d)
 {
   if (!d) return;
   cudaSetDevice(d->device);
-  cudaFree(d->d_avg); cudaFree(d->d_n0); cudaFree(d->d_n0_primed); cudaFree(d->d_out); cudaFree(d->d_count);
-  cudaFree(d->d_total);
   delete d;
 }
 
@@ -372,12 +367,9 @@ extern "C" sdb_chdet_t *sdb_chdet_new(int device, uint32_t n_bins, uint32_t n_st
   d->device = device; d->N = n_bins; d->S = n_streams; d->alpha = alpha; d->gamma = gamma; d->snr = snr;
   d->min_bins = min_bins < 1 ? 1 : min_bins;
   const size_t S = n_streams;
-  bool ok = cudaMalloc(&d->d_avg, S * n_bins * sizeof(float)) == cudaSuccess &&
-            cudaMalloc(&d->d_n0, S * sizeof(float)) == cudaSuccess &&
-            cudaMalloc(&d->d_n0_primed, S * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&d->d_out, S * CHDET_CAP * sizeof(SdbDetectedDev)) == cudaSuccess &&
-            cudaMalloc(&d->d_count, S * sizeof(unsigned)) == cudaSuccess &&
-            cudaMalloc(&d->d_total, S * sizeof(unsigned)) == cudaSuccess;
+  bool ok = d->d_avg.alloc(S * n_bins) == cudaSuccess && d->d_n0.alloc(S) == cudaSuccess &&
+            d->d_n0_primed.alloc(S) == cudaSuccess && d->d_out.alloc(S * CHDET_CAP) == cudaSuccess &&
+            d->d_count.alloc(S) == cudaSuccess && d->d_total.alloc(S) == cudaSuccess;
   if (ok) {
     cudaMemset(d->d_avg, 0, S * n_bins * sizeof(float));
     cudaMemset(d->d_n0, 0, S * sizeof(float));

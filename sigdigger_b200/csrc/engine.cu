@@ -21,15 +21,8 @@
 #include <cstdio>
 #include <cstring>
 
-static thread_local std::string g_err;
-static int fail(const std::string &m) { g_err = m; return -1; }
-#define CK(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { \
-  g_err = std::string(#expr) + ": " + cudaGetErrorString(e__); return -1; } } while (0)
-#define CKP(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { \
-  g_err = std::string(#expr) + ": " + cudaGetErrorString(e__); return nullptr; } } while (0)
-
+thread_local std::string g_err;
 extern "C" const char *sdb_last_error(void) { return g_err.c_str(); }
-int sdb_set_error(const char *m) { g_err = m ? m : ""; return -1; }     // other units of the library (tv_kernels.cu)
 
 extern "C" int sdb_device_count(void)
 {
@@ -62,7 +55,7 @@ struct sdb_engine {
   bool committed = false, first_feed = true, timing = false, chains_fresh = true;
   std::vector<Channel> channels;
   std::map<unsigned, float2 *> tw;     // twiddle tables by size
-  std::vector<void *> allocs;
+  std::vector<DevBuf<unsigned char>> allocs;   // every device buffer of the engine (dalloc), freed with it
 
   unsigned Np = 0, W = 0;               // PSD size, channeliser window
   SdbFourStep fs_psd{}, fs_st{};       // transform plans (make_plan)
@@ -130,11 +123,10 @@ struct sdb_engine {
 
   template <typename T> T *dalloc(size_t n)
   {
-    void *p = nullptr;
-    if (n == 0) n = 1;
-    if (cudaMalloc(&p, n * sizeof(T)) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-    allocs.push_back(p);
-    return (T *) p;
+    DevBuf<unsigned char> b;
+    if (b.alloc(std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return nullptr;
+    allocs.push_back(std::move(b));
+    return (T *) allocs.back().get();
   }
   const float2 *twiddle(unsigned n)
   {
@@ -276,7 +268,6 @@ extern "C" void sdb_engine_destroy(sdb_engine_t *e)
   e->collect_spans();
   if (e->l2_pinned_bytes) { cudaCtxResetPersistingL2Cache(); cudaGetLastError(); }
   if (e->chdet) sdb_chdet_destroy(e->chdet);
-  for (void *p : e->allocs) cudaFree(p);
   for (int i = 0; i < 2; ++i) {
     if (e->ev_chan[i]) cudaEventDestroy(e->ev_chan[i]);
     if (e->ev_insp[i]) cudaEventDestroy(e->ev_insp[i]);
@@ -356,10 +347,6 @@ extern "C" int sdb_engine_set_inspector(sdb_engine_t *e, int handle, const sdb_i
   return 0;
 }
 
-struct sdb_chdet;
-cudaError_t sdb_chdet_feed_stream(sdb_chdet *d, const float *psd_dev, uint32_t frames, size_t stream_stride,
-                                  cudaStream_t stream, uint64_t *launch_counter);
-
 extern "C" int sdb_engine_set_channel_detector(sdb_engine_t *e, float alpha, float beta, float gamma, float snr,
                                                uint32_t min_bins)
 {
@@ -388,8 +375,6 @@ extern "C" long sdb_engine_read_channels(sdb_engine_t *e, uint32_t stream, doubl
   return n;
 }
 
-extern "C" int sdb_chdet_read_all(struct sdb_chdet *d, double samp_rate, const double *centers, sdb_detected_channel *out,
-                                  size_t cap, uint32_t *counts);
 // all streams at once: centers[S] (host), out[S][cap], counts[S]
 extern "C" int sdb_engine_read_all_channels(sdb_engine_t *e, const double *centers, sdb_detected_channel *out, size_t cap,
                                             uint32_t *counts)
@@ -567,6 +552,19 @@ static bool build_chain_cfg(const Channel &ch, SdbChainCfg &c, std::vector<float
   c.eq_type = (int) g.eq_type; c.eq_locked = g.eq_locked; c.eq_mu = g.eq_rate;
   if (g.eq_type > 1) return false;
   return true;
+}
+
+// Lays out the chain's state lines in its float pool (AGC delay line, magnitude history, matched-filter line) and
+// returns its initial loop state: AGC levels at the -160 dB floor, Gardner phase 1/4, CMA equaliser at identity.
+static SdbChainState chain_layout(SdbChainCfg &c)
+{
+  c.st_dl_off = 0; c.st_mh_off = 2 * (int) c.dl_size; c.st_mf_off = c.st_mh_off + (int) c.mh_size;
+  c.st_pool = c.st_mf_off + 2 * c.mf_n;
+  SdbChainState s;
+  memset(&s, 0, sizeof(s));
+  s.fast_level = s.slow_level = s.peak = -160.0f;
+  s.k_phi = 0.25f; s.k_bnor = c.bnor; s.eq_wr[0] = 1.0f;
+  return s;
 }
 
 extern "C" int sdb_engine_commit(sdb_engine_t *e)
@@ -772,12 +770,12 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
     // ---- chains
     e->h_cfg.resize(K);
     std::vector<float> taps_pool;
+    std::vector<SdbChainState> st0(K);
     size_t pool = 1, cap = 1;
     for (int k = 0; k < K; ++k) {
       if (!build_chain_cfg(e->channels[k], e->h_cfg[k], taps_pool)) return fail("invalid inspector configuration");
       SdbChainCfg &c = e->h_cfg[k];
-      c.st_dl_off = 0; c.st_mh_off = 2 * (int) c.dl_size; c.st_mf_off = c.st_mh_off + (int) c.mh_size;
-      c.st_pool = c.st_mf_off + 2 * c.mf_n;
+      st0[k] = chain_layout(c);
       pool = std::max<size_t>(pool, (size_t) c.st_pool);
       cap = std::max<size_t>(cap, e->max_hops * e->channels[k].halfsz);
     }
@@ -806,13 +804,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
     if (!taps_pool.empty())
       CK(cudaMemcpy(e->d_taps, taps_pool.data(), taps_pool.size() * sizeof(float), cudaMemcpyHostToDevice));
     std::vector<SdbChainState> st(chains);
-    for (size_t ci = 0; ci < chains; ++ci) {
-      const SdbChainCfg &c = e->h_cfg[ci % K];
-      SdbChainState &s = st[ci];
-      memset(&s, 0, sizeof(s));
-      s.fast_level = s.slow_level = s.peak = -160.0f;
-      s.k_phi = 0.25f; s.k_bnor = c.bnor; s.eq_wr[0] = 1.0f;
-    }
+    for (size_t ci = 0; ci < chains; ++ci) st[ci] = st0[ci % K];
     CK(cudaMemcpy(e->d_state, st.data(), chains * sizeof(SdbChainState), cudaMemcpyHostToDevice));
     {
       // lines start empty: delay line and filter line 0, magnitude history at the -160 dB floor (SPEC A); the engine
@@ -1246,25 +1238,6 @@ extern "C" void sdb_engine_timing(sdb_engine_t *e, int enable)
   e->timing = enable != 0;
   for (int i = 0; i < FAM_COUNT; ++i) { e->fam_ms[i] = 0; e->fam_n[i] = 0; }
 }
-cudaError_t sdb_stage_cycles(unsigned long long out[8], int reset);
-extern "C" int sdb_debug_stage_cycles(uint64_t out[8], int reset)
-{
-  unsigned long long tmp[8];
-  CK(cudaDeviceSynchronize());
-  CK(sdb_stage_cycles(tmp, reset));
-  for (int i = 0; i < 8; ++i) out[i] = tmp[i];
-  return 0;
-}
-
-cudaError_t sdb_stage_cta_cycles(unsigned long long out[64], int reset);
-extern "C" int sdb_debug_cta_cycles(uint64_t out[64], int reset)
-{
-  unsigned long long tmp[64];
-  CK(cudaDeviceSynchronize());
-  CK(sdb_stage_cta_cycles(tmp, reset));
-  for (int i = 0; i < 64; ++i) out[i] = tmp[i];
-  return 0;
-}
 
 extern "C" int sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches)
 {
@@ -1276,145 +1249,6 @@ extern "C" int sdb_engine_kernel_time(sdb_engine_t *e, const char *family, doubl
       return 0;
     }
   return fail("unknown kernel family");
-}
-
-// ---------------------------------------------------------------------------------------------
-// Tasks/ primitives on host buffers
-// ---------------------------------------------------------------------------------------------
-struct TaskBufs {
-  float2 *src = nullptr, *dst = nullptr; float *pool = nullptr; SdbChainCfg *cfg = nullptr;
-  ~TaskBufs() { cudaFree(src); cudaFree(dst); cudaFree(pool); cudaFree(cfg); }
-  int put_cfg(const SdbChainCfg &c)
-  {
-    CK(cudaMalloc(&cfg, sizeof(c)));
-    CK(cudaMemcpy(cfg, &c, sizeof(c), cudaMemcpyHostToDevice));
-    return 0;
-  }
-};
-
-static int task_io_begin(TaskBufs &b, const sdb_complex *src, size_t n, size_t batch)
-{
-  if (!src || n == 0 || batch == 0) return fail("invalid task buffer");
-  if (sdb_device_count() <= 0) return fail("no CUDA device: sigdigger_b200 has no CPU fallback");
-  CK(cudaMalloc(&b.src, n * batch * sizeof(float2)));
-  CK(cudaMalloc(&b.dst, n * batch * sizeof(float2)));
-  CK(cudaMemcpy(b.src, src, n * batch * sizeof(float2), cudaMemcpyHostToDevice));
-  return 0;
-}
-static int task_io_end(TaskBufs &b, sdb_complex *dst, size_t n, size_t batch)
-{
-  CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(dst, b.dst, n * batch * sizeof(float2), cudaMemcpyDeviceToHost));
-  return 0;
-}
-
-extern "C" int sdb_task_carrier_xlate(const sdb_complex *src, sdb_complex *dst, size_t n, size_t batch,
-                                      float rel_freq, float phase)
-{
-  TaskBufs b;
-  if (task_io_begin(b, src, n, batch)) return -1;
-  // su_ncqo_init(-relFreq); su_ncqo_set_phase(-phase)   (Tasks/CarrierXlator.cpp:36-37)
-  float omega = 3.14159265358979323846f * (-rel_freq);
-  float phi = -phase;
-  phi = phi - 6.28318530717958647692f * floorf(phi / 6.28318530717958647692f);
-  if (phi >= 6.28318530717958647692f) phi = 0.0f;
-  CK(sdb_launch_task_xlate(0, b.src, b.dst, n, batch, omega, phi));
-  return task_io_end(b, dst, n, batch);
-}
-
-extern "C" int sdb_task_quad_demod(const sdb_complex *src, sdb_complex *dst, size_t n, size_t batch)
-{
-  TaskBufs b;
-  if (task_io_begin(b, src, n, batch)) return -1;
-  CK(sdb_launch_task_quad(0, b.src, b.dst, n, batch));
-  return task_io_end(b, dst, n, batch);
-}
-
-extern "C" int sdb_task_costas(const sdb_complex *src, sdb_complex *dst, size_t n, size_t batch, int kind,
-                               float tau, float loop_bw)
-{
-  if (kind < 1 || kind > 3) return fail("invalid Costas kind");
-  TaskBufs b;
-  if (task_io_begin(b, src, n, batch)) return -1;
-  SdbChainCfg c; memset(&c, 0, sizeof(c));
-  // su_costas_init(&costas, kind, 0, 1/tau, 3, loopbw)   (Tasks/CostasRecoveryTask.cpp:36-41)
-  c.costas_kind = kind;
-  c.c_a = 3.14159265358979323846f * loop_bw;
-  c.c_b = 0.5f * c.c_a * c.c_a;
-  if (!sdbh::butter_lp(2, 1.0f / tau, c.af_b, c.af_a)) return fail("invalid arm bandwidth");
-  c.af_n = 3;
-  if (b.put_cfg(c)) return -1;
-  CK(sdb_launch_task_chain(0, b.src, b.dst, n, batch, b.cfg, 0, nullptr, 0));
-  return task_io_end(b, dst, n, batch);
-}
-
-extern "C" int sdb_task_pll(const sdb_complex *src, sdb_complex *dst, size_t n, size_t batch, float bw)
-{
-  TaskBufs b;
-  if (task_io_begin(b, src, n, batch)) return -1;
-  SdbChainCfg c; memset(&c, 0, sizeof(c));
-  float fc = 3.14159265358979323846f * bw;
-  float dinv = 1.0f / (1.0f + 2.0f * 0.707f * fc + fc * fc);
-  c.pll_alpha = 4.0f * fc * fc * dinv;
-  c.pll_beta = 4.0f * 0.707f * fc * dinv;
-  if (b.put_cfg(c)) return -1;
-  CK(sdb_launch_task_chain(0, b.src, b.dst, n, batch, b.cfg, 1, nullptr, 0));
-  return task_io_end(b, dst, n, batch);
-}
-
-extern "C" int sdb_task_agc(const sdb_complex *src, sdb_complex *dst, size_t n, size_t batch, float tau)
-{
-  TaskBufs b;
-  if (task_io_begin(b, src, n, batch)) return -1;
-  SdbChainCfg c; memset(&c, 0, sizeof(c));
-  // AGCTask sets only the five time constants; delay line / history keep the defaults (20)
-  // (Tasks/AGCTask.cpp:43-47 and the comment in SURVEY.md 8a row a6)
-  sdbh::AgcDesign d = sdbh::agc_from_tau(tau, 2.0f);
-  c.knee = d.knee; c.gain_slope = d.gain_slope; c.fixed_gain = d.fixed_gain;
-  c.hang_max = d.hang_max; c.dl_size = 20; c.mh_size = 20;
-  c.far_ = d.far_; c.faf = d.faf; c.sar = d.sar; c.saf = d.saf;
-  c.st_dl_off = 0; c.st_mh_off = 40; c.st_pool = 60;
-  CK(cudaMalloc(&b.pool, ((batch + 31) / 32) * 32 * 60 * sizeof(float)));
-  if (b.put_cfg(c)) return -1;
-  CK(sdb_launch_task_chain(0, b.src, b.dst, n, batch, b.cfg, 2, b.pool, 60));
-  return task_io_end(b, dst, n, batch);
-}
-
-// ---- bulk twins of the per-sample sigutils calls, continuing from (and returning) the caller's loop state
-static int task_state_run(const sdb_complex *src, sdb_complex *dst, size_t n, int mode, void *st, size_t st_bytes)
-{
-  if (!src || !dst || !st) return fail("null argument");
-  if (sdb_device_count() <= 0) return fail("no CUDA device: sigdigger_b200 has no CPU fallback");
-  if (n == 0) return 0;
-  float2 *d_x = nullptr, *d_y = nullptr; float *d_st = nullptr;
-  int rc = 0;
-  if (cudaMalloc(&d_x, n * sizeof(float2)) != cudaSuccess || cudaMalloc(&d_y, n * sizeof(float2)) != cudaSuccess ||
-      cudaMalloc(&d_st, st_bytes) != cudaSuccess) rc = fail("out of device memory");
-  if (!rc && (cudaMemcpy(d_x, src, n * sizeof(float2), cudaMemcpyHostToDevice) != cudaSuccess ||
-              cudaMemcpy(d_st, st, st_bytes, cudaMemcpyHostToDevice) != cudaSuccess)) rc = fail("copy failed");
-  if (!rc && sdb_launch_task_chain_state(0, d_x, d_y, n, mode, d_st) != cudaSuccess) rc = fail("launch failed");
-  if (!rc && (cudaMemcpy(dst, d_y, n * sizeof(float2), cudaMemcpyDeviceToHost) != cudaSuccess ||
-              cudaMemcpy(st, d_st, st_bytes, cudaMemcpyDeviceToHost) != cudaSuccess)) rc = fail(cudaGetErrorString(cudaGetLastError()));
-  cudaFree(d_x); cudaFree(d_y); cudaFree(d_st);
-  return rc;
-}
-extern "C" int sdb_task_costas_state(const sdb_complex *src, sdb_complex *dst, size_t n, const void *k, size_t k_bytes,
-                                     void *s, size_t s_bytes)
-{
-  if (k_bytes != sdb_costas_k_bytes() || s_bytes != sdb_costas_s_bytes()) return fail("costas state size mismatch");
-  std::vector<unsigned char> st(k_bytes + s_bytes);
-  memcpy(st.data(), k, k_bytes); memcpy(st.data() + k_bytes, s, s_bytes);
-  if (task_state_run(src, dst, n, 0, st.data(), st.size())) return -1;
-  memcpy(s, st.data() + k_bytes, s_bytes);
-  return 0;
-}
-extern "C" int sdb_task_pll_state(const sdb_complex *src, sdb_complex *dst, size_t n, float alpha, float beta,
-                                  float state[2])
-{
-  float st[4] = { alpha, beta, state[0], state[1] };
-  if (task_state_run(src, dst, n, 1, st, sizeof(st))) return -1;
-  state[0] = st[2]; state[1] = st[3];
-  return 0;
 }
 
 // ---- take over the running state of another engine (live re-plan: suscan keeps every inspector that stays open
@@ -1523,151 +1357,6 @@ extern "C" int sdb_engine_migrate_map(sdb_engine_t *dst, sdb_engine_t *src, cons
   return migrate_impl(dst, src, map);
 }
 
-// ---- TimeWindow tasks that are fully specified in-repo (SPEC Y; kernels in tasks_kernels.cu)
-struct DevMem {
-  void *p = nullptr;
-  ~DevMem() { cudaFree(p); }
-  template <typename T> T *as() { return (T *) p; }
-};
-
-static int task_src_begin(DevMem &src, const sdb_complex *host, size_t n, size_t batch)
-{
-  if (!host || n == 0 || batch == 0) return fail("invalid task buffer");
-  if (sdb_device_count() <= 0) return fail("no CUDA device: sigdigger_b200 has no CPU fallback");
-  CK(cudaMalloc(&src.p, n * batch * sizeof(float2)));
-  CK(cudaMemcpy(src.p, host, n * batch * sizeof(float2), cudaMemcpyHostToDevice));
-  return 0;
-}
-
-extern "C" int sdb_task_delayed_conj(const sdb_complex *src, sdb_complex *dst, size_t n, size_t batch, size_t delay)
-{
-  if (delay == 0) return fail("Delay is zero samples");   // DelayedConjTask.cpp:36-37
-  if (!dst) return fail("null argument");
-  TaskBufs b;
-  if (task_io_begin(b, src, n, batch)) return -1;
-  CK(sdb_launch_task_delayed_conj(0, b.src, b.dst, n, batch, delay));
-  return task_io_end(b, dst, n, batch);
-}
-
-extern "C" long sdb_task_histogram_feed(const sdb_complex *src, float *out, size_t n, size_t batch, int space)
-{
-  if (!out) return fail("null argument");
-  if (space < SDB_SPACE_AMPLITUDE || space > SDB_SPACE_FREQUENCY) return fail("unknown decision space");
-  DevMem s, o;
-  if (task_src_begin(s, src, n, batch)) return -1;
-  const size_t count = space == SDB_SPACE_FREQUENCY ? n - 1 : n;
-  if (count == 0) return 0;
-  CK(cudaMalloc(&o.p, count * batch * sizeof(float)));
-  CK(sdb_launch_task_hist(0, s.as<float2>(), o.as<float>(), n, batch, space));
-  CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(out, o.p, count * batch * sizeof(float), cudaMemcpyDeviceToHost));
-  return (long) count;
-}
-
-extern "C" long sdb_task_sample_manual(const sdb_complex *src, size_t n, size_t batch, int space, size_t symbol_sync,
-                                       double symbol_count, sdb_complex *out)
-{
-  if (!out) return fail("null argument");
-  if (space < SDB_SPACE_AMPLITUDE || space > SDB_SPACE_FREQUENCY) return fail("unknown decision space");
-  if (!(symbol_count >= 1.0) || symbol_count > (double) n) return fail("symbol_count must be in [1, n]");
-  DevMem s, o;
-  if (task_src_begin(s, src, n, batch)) return -1;
-  // WaveSampler.cpp:44-45: delta = length / symbolCount; sampOffset = symbolSync / delta
-  const double delta = (double) n / symbol_count;
-  const double samp_offset = (double) symbol_sync / delta;
-  const float delta_inv = 1.f / (float) delta;
-  const long long count = (long long) symbol_count;
-  CK(cudaMalloc(&o.p, (size_t) count * batch * sizeof(float2)));
-  CK(sdb_launch_task_sample_manual(0, s.as<float2>(), n, batch, space, (double) symbol_sync, delta, samp_offset,
-                                   delta_inv, count, o.as<float2>()));
-  CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(out, o.p, (size_t) count * batch * sizeof(float2), cudaMemcpyDeviceToHost));
-  return (long) count;
-}
-
-extern "C" int sdb_task_sample_zero_crossing(const sdb_complex *src, size_t n, size_t batch, int space, int amplitude,
-                                             float threshold_re, float threshold_im, float zc_angle_re,
-                                             float zc_angle_im, float bnor, uint8_t *sym, uint32_t *counts, size_t cap)
-{
-  if (!sym || !counts || cap == 0) return fail("null argument");
-  if (space < SDB_SPACE_AMPLITUDE || space > SDB_SPACE_FREQUENCY) return fail("unknown decision space");
-  if (!(bnor > 0.0f)) return fail("bnor must be positive");
-  if (bnor > 1.0f) bnor = 1.0f;                            // WaveSampler.cpp:50-51
-  DevMem s, ev, o, c;
-  if (task_src_begin(s, src, n, batch)) return -1;
-  const size_t pitch = (n + 15) & ~(size_t) 15;
-  CK(cudaMalloc(&ev.p, pitch * batch));
-  CK(cudaMalloc(&o.p, cap * batch));
-  CK(cudaMalloc(&c.p, batch * sizeof(unsigned)));
-  CK(cudaMemset(o.p, 0, cap * batch));
-  // WaveSampler.cpp:236-241
-  const float thres = amplitude ? threshold_re * threshold_re + threshold_im * threshold_im
-                                : threshold_re * zc_angle_re - threshold_im * zc_angle_im;
-  CK(sdb_launch_task_zero_crossing(0, s.as<float2>(), n, batch, space, amplitude ? 1 : 0, thres,
-                                   make_float2(zc_angle_re, zc_angle_im), bnor, ev.as<unsigned char>(), pitch,
-                                   o.as<unsigned char>(), c.as<unsigned>(), cap));
-  CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(sym, o.p, cap * batch, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(counts, c.p, batch * sizeof(unsigned), cudaMemcpyDeviceToHost));
-  return 0;
-}
-
-extern "C" int sdb_task_carrier_detect(const sdb_complex *src, size_t n, size_t batch, double avg_rel_bw,
-                                       double dc_notch_rel_bw, float *peak)
-{
-  if (!peak) return fail("null argument");
-  if (n > ((size_t) 1 << 20)) return fail("carrier detector: at most 2^20 samples");
-  if (!(avg_rel_bw >= 0.0 && avg_rel_bw <= 1.0)) return fail("avg_rel_bw must be in [0, 1]");
-  if (!(dc_notch_rel_bw >= 0.0)) dc_notch_rel_bw = 0.0;   // qBound(0., x, 1.), CarrierDetector.cpp:35
-  if (dc_notch_rel_bw > 1.0) dc_notch_rel_bw = 1.0;
-  DevMem s, w, buf, pk;
-  if (task_src_begin(s, src, n, batch)) return -1;
-  size_t alloc = 64;                                        // SPEC Y.5: transform size >= 64
-  while (alloc < n) alloc <<= 1;
-  std::vector<float> win;
-  sdbh::window_fill(win, (unsigned) n, SDB_WINDOW_BLACKMANN_HARRIS);
-  CK(cudaMalloc(&w.p, n * sizeof(float)));
-  CK(cudaMemcpy(w.p, win.data(), n * sizeof(float), cudaMemcpyHostToDevice));
-  CK(cudaMalloc(&buf.p, alloc * batch * sizeof(float2)));
-  CK(cudaMalloc(&pk.p, batch * sizeof(float)));
-  CK(sdb_launch_task_carrier_prep(0, s.as<float2>(), w.as<float>(), n, alloc, batch, buf.as<float2>()));
-  CK(cudaDeviceSynchronize());
-  // the transform is the engine's own PSD (rectangular window: the taps are already applied)
-  sdb_engine_params prm; memset(&prm, 0, sizeof(prm));
-  prm.n_streams = (uint32_t) batch; prm.psd_size = (uint32_t) alloc; prm.psd_window = SDB_WINDOW_NONE;
-  prm.max_feed = (uint32_t) alloc;
-  sdb_engine_t *e = sdb_engine_new(&prm, 1.0);
-  if (!e) return -1;
-  int rc = sdb_engine_commit(e);
-  if (!rc) rc = sdb_engine_feed_device(e, (const sdb_complex *) buf.p, alloc, alloc);
-  if (!rc) rc = sdb_engine_sync(e);
-  if (!rc) {
-    const int bins = (int) ((double) alloc * avg_rel_bw) + 1;
-    const int skip = (int) (.5 * dc_notch_rel_bw * (double) alloc);
-    cudaError_t ce = sdb_launch_task_carrier_find(0, sdb_engine_psd_device(e), alloc, batch, bins, (bins - 1) / 2, skip,
-                                                  pk.as<float>());
-    if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
-    if (ce == cudaSuccess) ce = cudaMemcpy(peak, pk.p, batch * sizeof(float), cudaMemcpyDeviceToHost);
-    if (ce != cudaSuccess) { g_err = std::string("carrier detector: ") + cudaGetErrorString(ce); rc = -1; }
-  }
-  sdb_engine_destroy(e);
-  return rc;
-}
-
-extern "C" int sdb_task_decide(const sdb_complex *soft, uint8_t *sym, size_t n, int mode, unsigned bps, float min,
-                               float max)
-{
-  if (!sym) return fail("null argument");
-  if (mode < 0 || mode > 1 || bps < 1 || bps > 8 || !(max > min)) return fail("invalid decider");
-  DevMem s, o;
-  if (task_src_begin(s, soft, n, 1)) return -1;
-  CK(cudaMalloc(&o.p, n));
-  CK(sdb_launch_task_decide(0, s.as<float2>(), o.as<unsigned char>(), n, mode, min, max - min, 1 << bps));
-  CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(sym, o.p, n, cudaMemcpyDeviceToHost));
-  return 0;
-}
-
 // Offline inspector over `batch` captured channel-rate buffers (what the GUI's TimeWindow / SamplerDialog
 // do block-wise on the CPU, Components/TimeWindow.cpp:1571-2183): one GPU chain per buffer.
 extern "C" long sdb_task_inspector(const sdb_inspector_config *cfg, const sdb_complex *src, size_t n,
@@ -1679,29 +1368,15 @@ extern "C" long sdb_task_inspector(const sdb_inspector_config *cfg, const sdb_co
   ch.center = 0; ch.size = 2; ch.width = 2; ch.halfw = 1; ch.halfsz = 1; ch.has_insp = true; ch.cfg = *cfg;
   SdbChainCfg c; std::vector<float> taps;
   if (!build_chain_cfg(ch, c, taps)) return fail("invalid inspector configuration");
-  c.st_dl_off = 0; c.st_mh_off = 2 * (int) c.dl_size; c.st_mf_off = c.st_mh_off + (int) c.mh_size;
-  c.st_pool = c.st_mf_off + 2 * c.mf_n;
+  const std::vector<SdbChainState> st(batch, chain_layout(c));
   const size_t pool = (size_t) std::max(1, c.st_pool);
   SdbChannelDev cd; memset(&cd, 0, sizeof(cd)); cd.halfsz = 1; cd.out_off = 0;
-  std::vector<SdbChainState> st(batch);
   const size_t pool_floats = ((batch + 31) / 32) * 32 * pool;
-  for (size_t i = 0; i < batch; ++i) {
-    memset(&st[i], 0, sizeof(SdbChainState));
-    st[i].fast_level = st[i].slow_level = st[i].peak = -160.0f;
-    st[i].k_phi = 0.25f; st[i].k_bnor = c.bnor; st[i].eq_wr[0] = 1.0f;
-  }
-  struct Bufs { void *p[9] = {0}; ~Bufs() { for (auto q : p) cudaFree(q); } } b;
-  float2 *d_src, *d_soft; uint8_t *d_hard; uint32_t *d_cnt; SdbChainCfg *d_cfg; SdbChainState *d_st;
-  float *d_pool, *d_taps; SdbChannelDev *d_cd;
-  CK(cudaMalloc(&b.p[0], n * batch * sizeof(float2))); d_src = (float2 *) b.p[0];
-  CK(cudaMalloc(&b.p[1], cap * batch * sizeof(float2))); d_soft = (float2 *) b.p[1];
-  CK(cudaMalloc(&b.p[2], cap * batch)); d_hard = (uint8_t *) b.p[2];
-  CK(cudaMalloc(&b.p[3], batch * sizeof(uint32_t))); d_cnt = (uint32_t *) b.p[3];
-  CK(cudaMalloc(&b.p[4], sizeof(SdbChainCfg))); d_cfg = (SdbChainCfg *) b.p[4];
-  CK(cudaMalloc(&b.p[5], batch * sizeof(SdbChainState))); d_st = (SdbChainState *) b.p[5];
-  CK(cudaMalloc(&b.p[6], pool_floats * sizeof(float))); d_pool = (float *) b.p[6];
-  CK(cudaMalloc(&b.p[7], std::max<size_t>(1, taps.size()) * sizeof(float))); d_taps = (float *) b.p[7];
-  CK(cudaMalloc(&b.p[8], sizeof(SdbChannelDev))); d_cd = (SdbChannelDev *) b.p[8];
+  DevBuf<float2> d_src, d_soft; DevBuf<uint8_t> d_hard; DevBuf<uint32_t> d_cnt; DevBuf<SdbChainCfg> d_cfg;
+  DevBuf<SdbChainState> d_st; DevBuf<float> d_pool, d_taps; DevBuf<SdbChannelDev> d_cd;
+  CK(d_src.alloc(n * batch)); CK(d_soft.alloc(cap * batch)); CK(d_hard.alloc(cap * batch)); CK(d_cnt.alloc(batch));
+  CK(d_cfg.alloc(1)); CK(d_st.alloc(batch)); CK(d_pool.alloc(pool_floats));
+  CK(d_taps.alloc(std::max<size_t>(1, taps.size()))); CK(d_cd.alloc(1));
   CK(cudaMemcpy(d_src, src, n * batch * sizeof(float2), cudaMemcpyHostToDevice));
   CK(cudaMemcpy(d_cfg, &c, sizeof(c), cudaMemcpyHostToDevice));
   CK(cudaMemcpy(d_st, st.data(), batch * sizeof(SdbChainState), cudaMemcpyHostToDevice));
@@ -1719,477 +1394,11 @@ extern "C" long sdb_task_inspector(const sdb_inspector_config *cfg, const sdb_co
   return 0;
 }
 
-extern "C" int sdb_task_lpf(const sdb_complex *src, sdb_complex *dst, size_t n, size_t batch, float bw)
-{
-  // LPFTask: specttuner with the default 4096-sample window, one channel at f0 = 0 with
-  // guard = 2 pi / bw (no decimation), input flushed with zeros until n outputs exist
-  // (Tasks/LPFTask.cpp:52-69,104-107).
-  if (!src || !dst || n == 0 || batch == 0) return fail("invalid task buffer");
-  const unsigned W = 4096;   // sigutils_specttuner_params_INITIALIZER default window (SURVEY.md A.2)
-  sdb_engine_params p; memset(&p, 0, sizeof(p));
-  size_t padded = ((n + W / 2 + W / 2 - 1) / (W / 2)) * (W / 2);   // + half-window latency, rounded up
-  p.n_streams = (uint32_t) batch; p.psd_size = 0; p.st_window_size = W; p.max_feed = (uint32_t) padded; p.device = 0;
-  int dev = 0; cudaGetDevice(&dev); p.device = dev;
-  sdb_engine_t *e = sdb_engine_new(&p, 1.0);
-  if (!e) return -1;
-  sdb_channel_params cp; cp.f0 = 0.0f; cp.bw = 3.14159265358979323846f * bw; cp.guard = 6.28318530717958647692f / cp.bw;
-  cp.precise = 0;
-  int rc = -1;
-  std::vector<float2> in(batch * padded, make_float2(0.f, 0.f)), out(padded);
-  for (size_t b = 0; b < batch; ++b) memcpy(&in[b * padded], src + b * n, n * sizeof(float2));
-  do {
-    int h = sdb_engine_open_channel(e, &cp, nullptr);
-    if (h < 0) break;
-    if (sdb_engine_commit(e)) break;
-    if (sdb_engine_feed_host(e, reinterpret_cast<const sdb_complex *>(in.data()), padded, padded)) break;
-    bool ok = true;
-    for (size_t b = 0; b < batch && ok; ++b) {
-      long got = sdb_engine_read_channel(e, (uint32_t) b, h, reinterpret_cast<sdb_complex *>(out.data()), padded);
-      if (got < (long) n) { g_err = "lpf produced too few samples"; ok = false; break; }
-      memcpy(dst + b * n, out.data(), n * sizeof(float2));
-    }
-    if (ok) rc = 0;
-  } while (0);
-  sdb_engine_destroy(e);
-  return rc;
-}
-
-// ---------------------------------------------------------------------------------------------
-// SpectrumView (Panoramic/Scanner.cpp:36-293): panoramic stitcher
-// ---------------------------------------------------------------------------------------------
-cudaError_t sdb_launch_sview_project(cudaStream_t s, double freq_min, double freq_range, double fft_bandwidth,
-                                     float rel_bw, unsigned spectrum_size, const float *psd, size_t psd_size,
-                                     const double *centers_dev, int n_hops, int adjust_sides, int *j0, int *nb,
-                                     float *va, float *vc, int max_bins);
-cudaError_t sdb_launch_sview_accumulate(cudaStream_t s, unsigned spectrum_size, const int *j0, const int *nb,
-                                        const float *va, const float *vc, int n_hops, int max_bins, float *psd,
-                                        float *accum, float *count, float *count_snapshot);
-
-struct sdb_sview {
-  int device = 0;
-  double freq_min = 0, freq_max = 0, freq_range = 0, fft_bandwidth = 0;
-  float rel_bw = 0.5f;                     // include/Scanner.h:70
-  unsigned spectrum_size = 65536;          // SIGDIGGER_SCANNER_SPECTRUM_SIZE
-  int max_bins = 0;
-  float *d_psd = nullptr, *d_accum = nullptr, *d_count = nullptr, *d_count_snap = nullptr;
-  size_t hop_cap = 0;
-  double *d_centers = nullptr; int *d_j0 = nullptr, *d_nb = nullptr; float *d_va = nullptr, *d_vc = nullptr;
-};
-
-extern "C" sdb_sview_t *sdb_sview_new(int device)
-{
-  if (sdb_device_count() <= 0) { g_err = "no CUDA device: sigdigger_b200 has no CPU fallback"; return nullptr; }
-  CKP(cudaSetDevice(device));
-  sdb_sview *v = new sdb_sview();
-  v->device = device;
-  const size_t n = 65536 * sizeof(float);
-  if (cudaMalloc(&v->d_psd, n) != cudaSuccess || cudaMalloc(&v->d_accum, n) != cudaSuccess ||
-      cudaMalloc(&v->d_count, n) != cudaSuccess || cudaMalloc(&v->d_count_snap, n) != cudaSuccess) { g_err = "out of device memory"; delete v; return nullptr; }
-  cudaMemset(v->d_psd, 0, n); cudaMemset(v->d_accum, 0, n); cudaMemset(v->d_count, 0, n);
-  return v;
-}
-
-extern "C" void sdb_sview_destroy(sdb_sview_t *v)
-{
-  if (!v) return;
-  cudaSetDevice(v->device);
-  cudaFree(v->d_psd); cudaFree(v->d_accum); cudaFree(v->d_count); cudaFree(v->d_count_snap); cudaFree(v->d_centers);
-  cudaFree(v->d_j0); cudaFree(v->d_nb); cudaFree(v->d_va); cudaFree(v->d_vc);
-  delete v;
-}
-
-extern "C" int sdb_sview_reset(sdb_sview_t *v)
-{
-  if (!v) return fail("null view");
-  CK(cudaSetDevice(v->device));
-  const size_t n = 65536 * sizeof(float);          // SpectrumView::reset, Scanner.cpp:287-293
-  CK(cudaMemset(v->d_psd, 0, n)); CK(cudaMemset(v->d_accum, 0, n)); CK(cudaMemset(v->d_count, 0, n));
-  return 0;
-}
-
-int sdb_sview_reset_async(sdb_sview_t *v, cudaStream_t st)     // the same, ordered on the caller's stream
-{
-  if (!v) return fail("null view");
-  const size_t n = 65536 * sizeof(float);
-  CK(cudaMemsetAsync(v->d_psd, 0, n, st)); CK(cudaMemsetAsync(v->d_accum, 0, n, st));
-  CK(cudaMemsetAsync(v->d_count, 0, n, st));
-  return 0;
-}
-
-extern "C" int sdb_sview_set_range(sdb_sview_t *v, double fmin, double fmax, double fft_bandwidth, float rel_bw)
-{
-  if (!v) return fail("null view");
-  if (!(fmax > fmin) || !(fft_bandwidth > 0)) return fail("invalid frequency range");
-  v->freq_min = fmin; v->freq_max = fmax; v->freq_range = fmax - fmin;   // setRange, Scanner.cpp:41-54
-  unsigned n = (unsigned) (v->freq_range / 1000.0), sz = 1;               // SIGDIGGER_SCANNER_FREQ_RESOLUTION
-  while (sz < n) sz <<= 1;
-  if (sz > 65536) sz = 65536;
-  v->spectrum_size = sz;
-  v->fft_bandwidth = fft_bandwidth; v->rel_bw = rel_bw;
-  // a hop contributes at most sz * (fft_bandwidth - 2 skip) / freq_range + 1 bins, and every projection uses THIS
-  // fft_bandwidth (the kernels take the geometry from the view, not from the call): the `nb > max_bins` clamp in the
-  // projection kernels is a guard that cannot bind
-  double mb = (double) sz * fft_bandwidth / v->freq_range + 4.0;
-  v->max_bins = mb > (double) sz ? (int) sz : (int) mb;
-  if (v->max_bins < 2) v->max_bins = 2;
-  v->hop_cap = 0;   // contribution buffers depend on max_bins: reallocate lazily
-  return sdb_sview_reset(v);
-}
-
-extern "C" uint32_t sdb_sview_size(const sdb_sview_t *v) { return v ? v->spectrum_size : 0; }
-extern "C" uint32_t sdb_sview_max_bins(const sdb_sview_t *v) { return v ? (uint32_t) v->max_bins : 0; }
-
-extern "C" int sdb_sview_project(sdb_sview_t *v, const float *psd_dev, size_t psd_size, const double *centers,
-                                 size_t n_hops, int adjust_sides)
-{
-  if (!v || !psd_dev || !centers) return fail("null argument");
-  if (v->max_bins <= 0) return fail("set_range first");
-  CK(cudaSetDevice(v->device));
-  if (n_hops > v->hop_cap) {
-    cudaFree(v->d_centers); cudaFree(v->d_j0); cudaFree(v->d_nb); cudaFree(v->d_va); cudaFree(v->d_vc);
-    v->d_centers = nullptr; v->d_j0 = v->d_nb = nullptr; v->d_va = v->d_vc = nullptr;
-    CK(cudaMalloc(&v->d_centers, n_hops * sizeof(double)));
-    CK(cudaMalloc(&v->d_j0, n_hops * sizeof(int)));
-    CK(cudaMalloc(&v->d_nb, n_hops * sizeof(int)));
-    CK(cudaMalloc(&v->d_va, n_hops * (size_t) v->max_bins * sizeof(float)));
-    CK(cudaMalloc(&v->d_vc, n_hops * (size_t) v->max_bins * sizeof(float)));
-    v->hop_cap = n_hops;
-  }
-  CK(cudaMemcpy(v->d_centers, centers, n_hops * sizeof(double), cudaMemcpyHostToDevice));
-  CK(cudaMemset(v->d_va, 0, n_hops * (size_t) v->max_bins * sizeof(float)));
-  CK(cudaMemset(v->d_vc, 0, n_hops * (size_t) v->max_bins * sizeof(float)));
-  CK(sdb_launch_sview_project(0, v->freq_min, v->freq_range, v->fft_bandwidth, v->rel_bw, v->spectrum_size, psd_dev,
-                              psd_size, v->d_centers, (int) n_hops, adjust_sides, v->d_j0, v->d_nb, v->d_va, v->d_vc,
-                              v->max_bins));
-  return 0;
-}
-
-// ---- stream-ordered variants for the panoramic sweep (panoramic.cu): caller-owned device buffers, no host copies,
-// ---- no default-stream work.  `centers_dev` holds the hop centres on the device.
-cudaError_t sdb_launch_sview_project_tiled(cudaStream_t s, double freq_min, double freq_range, double fft_bandwidth,
-                                           float rel_bw, unsigned spectrum_size, const float *psd, size_t psd_size,
-                                           size_t hop_stride, int psd_is_linear, const double *centers_dev, int n_hops,
-                                           int adjust_sides, int *j0, int *nb, float *va, float *vc, int max_bins);
-// psd_dev: hop h's frame at psd_dev + h * hop_stride; psd_is_linear: the engine's linear natural-order PSD (the
-// PSDMessage conversion happens inside the projection) instead of shifted dB.  Returns 1 when the geometry needs the
-// general kernel (histogram mode or a very wide hop): the caller then converts and calls with psd_is_linear = 0.
-int sdb_sview_project_async(sdb_sview_t *v, cudaStream_t st, const float *psd_dev, size_t psd_size, size_t hop_stride,
-                            int psd_is_linear, const double *centers_dev, size_t n_hops, int adjust_sides, int32_t *j0,
-                            int32_t *nb, float *va, float *vc)
-{
-  if (!v || !psd_dev || !centers_dev || !j0 || !nb || !va || !vc) return fail("null argument");
-  if (v->max_bins <= 0) return fail("set_range first");
-  const bool linear_mode = v->fft_bandwidth / v->freq_range * v->spectrum_size >= 2.001;  // every hop, with margin
-                                                                                              // for the kernel's own test
-  if (linear_mode && v->max_bins <= 384) {
-    CK(sdb_launch_sview_project_tiled(st, v->freq_min, v->freq_range, v->fft_bandwidth, v->rel_bw, v->spectrum_size,
-                                      psd_dev, psd_size, hop_stride, psd_is_linear, centers_dev, (int) n_hops,
-                                      adjust_sides, j0, nb, va, vc, v->max_bins));
-    return 0;
-  }
-  if (psd_is_linear || hop_stride != psd_size) return 1;
-  CK(sdb_launch_sview_project(st, v->freq_min, v->freq_range, v->fft_bandwidth, v->rel_bw, v->spectrum_size, psd_dev,
-                              psd_size, centers_dev, (int) n_hops, adjust_sides, j0, nb, va, vc, v->max_bins));
-  return 0;
-}
-
-int sdb_sview_accumulate_async(sdb_sview_t *v, cudaStream_t st, const int32_t *j0, const int32_t *nb, const float *va,
-                               const float *vc, size_t n_hops)
-{
-  if (!v) return fail("null view");
-  CK(sdb_launch_sview_accumulate(st, v->spectrum_size, j0, nb, va, vc, (int) n_hops, v->max_bins, v->d_psd, v->d_accum,
-                                 v->d_count, v->d_count_snap));
-  return 0;
-}
-
-cudaError_t sdb_chdet_pack_device(sdb_chdet_t *d, double samp_rate, const double *centers_dev, sdb_detected_channel *out_dev,
-                                  size_t cap, int *counts_dev, cudaStream_t stream);
 // channel lists of the last feed, converted to Hz on the device (sdb_engine_read_all_channels without the host)
 int sdb_engine_pack_channels_device(sdb_engine_t *e, const double *centers_dev, sdb_detected_channel *out_dev, size_t cap,
                                     int *counts_dev, cudaStream_t st)
 {
   if (!e || !e->committed || !e->chdet) return fail("channel detector not enabled");
   CK(sdb_chdet_pack_device(e->chdet, e->samp_rate, centers_dev, out_dev, cap, counts_dev, st));
-  return 0;
-}
-
-cudaError_t sdb_launch_psd_shift_db(cudaStream_t s, const float *lin, float *db, size_t n_frames, unsigned n);
-int sdb_psd_shift_db_async(cudaStream_t st, const float *lin_dev, float *db_dev, size_t n_frames, uint32_t psd_size)
-{
-  if (!lin_dev || !db_dev || lin_dev == db_dev) return fail("invalid argument");
-  CK(sdb_launch_psd_shift_db(st, lin_dev, db_dev, n_frames, psd_size));
-  return 0;
-}
-
-
-extern "C" int sdb_psd_shift_db_device(const float *lin_dev, float *db_dev, size_t n_frames, uint32_t psd_size)
-{
-  if (!lin_dev || !db_dev) return fail("null argument");
-  if (lin_dev == db_dev) return fail("in-place conversion is not supported (the halves swap)");
-  if (psd_size < 2 || (psd_size & (psd_size - 1))) return fail("psd_size must be a power of two");
-  CK(sdb_launch_psd_shift_db(0, lin_dev, db_dev, n_frames, psd_size));
-  return 0;
-}
-
-// ---- SpectrumView::feed(SpectrumView const &) (Panoramic/Scanner.cpp:276-286; used by the zoom path of
-// ---- Scanner::setViewRange, :471-479): project the other view's accumulators / counts, then the same accumulate
-// ---- + interpolate pass a hop gets.
-cudaError_t sdb_launch_sview_project_view(cudaStream_t s, double freq_min, double freq_range, unsigned spectrum_size,
-                                          const float *src_acc, const float *src_cnt, unsigned src_size, double fmin,
-                                          double fmax, int *j0, int *nb, float *va, float *vc);
-
-extern "C" int sdb_sview_feed_view(sdb_sview_t *v, const sdb_sview_t *detail)
-{
-  if (!v || !detail) return fail("null view");
-  if (v == detail) return fail("a view cannot be fed into itself");
-  if (v->max_bins <= 0 || detail->max_bins <= 0) return fail("set_range first");
-  if (v->device != detail->device) return fail("both views must live on the same device");
-  CK(cudaSetDevice(v->device));
-  int *j0 = nullptr, *nb = nullptr; float *va = nullptr, *vc = nullptr;
-  const size_t row = 65536 * sizeof(float);
-  cudaError_t e = cudaMalloc(&j0, sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&nb, sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&va, row);
-  if (e == cudaSuccess) e = cudaMalloc(&vc, row);
-  if (e == cudaSuccess) e = cudaMemset(j0, 0, sizeof(int));
-  if (e == cudaSuccess) e = cudaMemset(nb, 0, sizeof(int));
-  if (e == cudaSuccess) e = cudaMemset(va, 0, row);
-  if (e == cudaSuccess) e = cudaMemset(vc, 0, row);
-  if (e == cudaSuccess)
-    e = sdb_launch_sview_project_view(0, v->freq_min, v->freq_range, v->spectrum_size, detail->d_accum, detail->d_count,
-                                      detail->spectrum_size, detail->freq_min, detail->freq_max, j0, nb, va, vc);
-  if (e == cudaSuccess)
-    e = sdb_launch_sview_accumulate(0, v->spectrum_size, j0, nb, va, vc, 1, 65536, v->d_psd, v->d_accum, v->d_count,
-                                    v->d_count_snap);
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  cudaFree(j0); cudaFree(nb); cudaFree(va); cudaFree(vc);
-  if (e != cudaSuccess) return fail(std::string("sdb_sview_feed_view: ") + cudaGetErrorString(e));
-  return 0;
-}
-
-// ---- SNR estimator on the inspectors' decision-space histograms (Misc/SNREstimator.cpp; SPEC Y.7)
-cudaError_t sdb_launch_snr_feed(cudaStream_t s, const unsigned *history, unsigned length, unsigned n, void *states,
-                                float *gaussian, float *hi, float *htilde, float *term);
-struct SnrHostState { float sigma, alpha, delta; unsigned intervals; };
-struct sdb_snr_estimator {
-  int device = 0; unsigned n = 0, length = 0;
-  std::vector<SnrHostState> st; std::vector<unsigned> bps;
-  bool dirty = true;                       // host copy of the states newer than the device copy
-  unsigned *d_hist = nullptr; void *d_states = nullptr; float *d_work = nullptr;   // gaussian | hi | htilde | term
-};
-
-extern "C" sdb_snr_estimator_t *sdb_snr_estimator_new(uint32_t n_estimators, uint32_t length, int device)
-{
-  if (sdb_device_count() <= 0) { g_err = "no CUDA device: sigdigger_b200 has no CPU fallback"; return nullptr; }
-  if (n_estimators == 0 || length == 0) { g_err = "snr estimator: empty geometry"; return nullptr; }
-  CKP(cudaSetDevice(device));
-  sdb_snr_estimator *e = new sdb_snr_estimator();
-  e->device = device; e->n = n_estimators; e->length = length;
-  e->st.assign(n_estimators, SnrHostState{ 1.f / 8.f, 1.f, 0.f, 0u });   // SNR_ESTIMATOR_DEFAULT_SIGMA / _ALPHA
-  e->bps.assign(n_estimators, 0u);
-  const size_t tot = (size_t) n_estimators * length;
-  if (cudaMalloc(&e->d_hist, tot * sizeof(unsigned)) != cudaSuccess ||
-      cudaMalloc(&e->d_states, n_estimators * sizeof(SnrHostState)) != cudaSuccess ||
-      cudaMalloc(&e->d_work, 4 * tot * sizeof(float)) != cudaSuccess) {
-    cudaFree(e->d_hist); cudaFree(e->d_states); cudaFree(e->d_work);
-    g_err = "out of device memory"; delete e; return nullptr;
-  }
-  cudaMemset(e->d_work, 0, 4 * tot * sizeof(float));
-  return e;
-}
-
-extern "C" void sdb_snr_estimator_destroy(sdb_snr_estimator_t *e)
-{
-  if (!e) return;
-  cudaSetDevice(e->device);
-  cudaFree(e->d_hist); cudaFree(e->d_states); cudaFree(e->d_work);
-  delete e;
-}
-
-static int snr_pull(sdb_snr_estimator *e)
-{
-  if (e->dirty) return 0;
-  CK(cudaSetDevice(e->device));
-  CK(cudaMemcpy(e->st.data(), e->d_states, e->n * sizeof(SnrHostState), cudaMemcpyDeviceToHost));
-  return 0;
-}
-
-// setBps (SNREstimator.cpp:122-131): a change of bps restarts sigma
-extern "C" int sdb_snr_estimator_set_bps(sdb_snr_estimator_t *e, uint32_t index, uint32_t bps)
-{
-  if (!e || index >= e->n) return fail("wrong estimator index");
-  if (bps > 8) return fail("bps out of range");
-  if (snr_pull(e)) return -1;
-  if (e->bps[index] != bps) {                  // as the reference: setBps(0) on a fresh estimator leaves it idle
-    e->bps[index] = bps; e->st[index].sigma = 1.f / 8.f; e->st[index].intervals = 1u << bps;
-  }
-  e->dirty = true;
-  return 0;
-}
-
-extern "C" int sdb_snr_estimator_set_alpha(sdb_snr_estimator_t *e, uint32_t index, float alpha)
-{
-  if (!e || index >= e->n) return fail("wrong estimator index");
-  if (snr_pull(e)) return -1;
-  e->st[index].alpha = alpha; e->dirty = true;
-  return 0;
-}
-
-extern "C" int sdb_snr_estimator_set_sigma(sdb_snr_estimator_t *e, uint32_t index, float sigma)
-{
-  if (!e || index >= e->n) return fail("wrong estimator index");
-  if (snr_pull(e)) return -1;
-  e->st[index].sigma = sigma; e->dirty = true;
-  return 0;
-}
-
-// feed (SNREstimator.cpp:133-158) for every estimator: histories [n][length] counts, host memory
-extern "C" int sdb_snr_estimator_feed(sdb_snr_estimator_t *e, const uint32_t *histories)
-{
-  if (!e || !histories) return fail("null argument");
-  CK(cudaSetDevice(e->device));
-  const size_t tot = (size_t) e->n * e->length;
-  if (e->dirty) {
-    CK(cudaMemcpy(e->d_states, e->st.data(), e->n * sizeof(SnrHostState), cudaMemcpyHostToDevice));
-    e->dirty = false;
-  }
-  CK(cudaMemcpy(e->d_hist, histories, tot * sizeof(unsigned), cudaMemcpyHostToDevice));
-  CK(sdb_launch_snr_feed(0, e->d_hist, e->length, e->n, e->d_states, e->d_work, e->d_work + tot, e->d_work + 2 * tot,
-                         e->d_work + 3 * tot));
-  CK(cudaDeviceSynchronize());
-  return 0;
-}
-
-// getSigma / getSNR (include/SNREstimator.h:74-84) and getModel (:61-65); any pointer may be NULL
-extern "C" int sdb_snr_estimator_read(sdb_snr_estimator_t *e, float *sigma, float *snr, float *model)
-{
-  if (!e) return fail("null argument");
-  if (snr_pull(e)) return -1;
-  for (unsigned i = 0; i < e->n; ++i) {
-    if (sigma) sigma[i] = e->st[i].sigma;
-    if (snr) snr[i] = 1.f / (e->st[i].intervals * e->st[i].sigma);
-  }
-  if (model) {
-    const size_t tot = (size_t) e->n * e->length;
-    CK(cudaSetDevice(e->device));
-    CK(cudaMemcpy(model, e->d_work + tot, tot * sizeof(float), cudaMemcpyDeviceToHost));
-  }
-  return 0;
-}
-
-// ---- spectrum averager (Misc/Averager.cpp:25-60)
-cudaError_t sdb_launch_psd_average(cudaStream_t s, const float *psd, size_t stream_stride, unsigned frames, unsigned n,
-                                   size_t n_streams, float alpha, int primed, float *last);
-struct sdb_averager {
-  int device = 0; unsigned n = 0; size_t n_streams = 0; float alpha = 1.0f; bool primed = false;
-  float *d_last = nullptr;
-};
-
-extern "C" sdb_averager_t *sdb_averager_new(uint32_t psd_size, uint32_t n_streams, float alpha, int device)
-{
-  if (sdb_device_count() <= 0) { g_err = "no CUDA device: sigdigger_b200 has no CPU fallback"; return nullptr; }
-  if (psd_size == 0 || n_streams == 0) { g_err = "averager: empty geometry"; return nullptr; }
-  CKP(cudaSetDevice(device));
-  sdb_averager *a = new sdb_averager();
-  a->device = device; a->n = psd_size; a->n_streams = n_streams; a->alpha = alpha;
-  if (cudaMalloc(&a->d_last, (size_t) psd_size * n_streams * sizeof(float)) != cudaSuccess) {
-    g_err = "out of device memory"; delete a; return nullptr;
-  }
-  cudaMemset(a->d_last, 0, (size_t) psd_size * n_streams * sizeof(float));
-  return a;
-}
-
-extern "C" void sdb_averager_destroy(sdb_averager_t *a)
-{
-  if (!a) return;
-  cudaSetDevice(a->device);
-  cudaFree(a->d_last);
-  delete a;
-}
-
-extern "C" int sdb_averager_set_alpha(sdb_averager_t *a, float alpha)
-{
-  if (!a) return fail("null averager");
-  a->alpha = alpha;
-  return 0;
-}
-
-extern "C" int sdb_averager_reset(sdb_averager_t *a)
-{
-  if (!a) return fail("null averager");
-  a->primed = false;
-  return 0;
-}
-
-extern "C" int sdb_averager_feed_device(sdb_averager_t *a, const float *psd_dev, size_t frames, size_t stream_stride)
-{
-  if (!a || !psd_dev) return fail("null argument");
-  if (frames == 0) return 0;
-  if (stream_stride < frames * a->n && a->n_streams > 1) return fail("stream stride smaller than the frames");
-  CK(cudaSetDevice(a->device));
-  CK(sdb_launch_psd_average(0, psd_dev, stream_stride, (unsigned) frames, a->n, a->n_streams, a->alpha,
-                            a->primed ? 1 : 0, a->d_last));
-  a->primed = true;
-  return 0;
-}
-
-extern "C" const float *sdb_averager_device(const sdb_averager_t *a) { return a ? a->d_last : nullptr; }
-
-extern "C" int sdb_averager_read(sdb_averager_t *a, float *dst, size_t cap)
-{
-  if (!a || !dst) return fail("null argument");
-  const size_t tot = (size_t) a->n * a->n_streams;
-  if (cap < tot) return fail("destination too small");
-  CK(cudaSetDevice(a->device));
-  CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(dst, a->d_last, tot * sizeof(float), cudaMemcpyDeviceToHost));
-  return 0;
-}
-
-extern "C" int sdb_sview_contrib(sdb_sview_t *v, int32_t **j0, int32_t **nb, float **va, float **vc)
-{
-  if (!v) return fail("null view");
-  if (j0) *j0 = v->d_j0;
-  if (nb) *nb = v->d_nb;
-  if (va) *va = v->d_va;
-  if (vc) *vc = v->d_vc;
-  return 0;
-}
-
-// copy the last projection's contribution lists into caller-owned DEVICE buffers (the send buffers of the
-// NCCL gather): j0/nb [n_hops] int32, va/vc [n_hops][max_bins] float32
-extern "C" int sdb_sview_contrib_copy(sdb_sview_t *v, int32_t *j0, int32_t *nb, float *va, float *vc, size_t n_hops)
-{
-  if (!v || !j0 || !nb || !va || !vc) return fail("null argument");
-  if (n_hops > v->hop_cap) return fail("more hops than the last projection held");
-  CK(cudaSetDevice(v->device));
-  const size_t row = (size_t) v->max_bins * sizeof(float);
-  CK(cudaMemcpy(j0, v->d_j0, n_hops * sizeof(int), cudaMemcpyDeviceToDevice));
-  CK(cudaMemcpy(nb, v->d_nb, n_hops * sizeof(int), cudaMemcpyDeviceToDevice));
-  CK(cudaMemcpy(va, v->d_va, n_hops * row, cudaMemcpyDeviceToDevice));
-  CK(cudaMemcpy(vc, v->d_vc, n_hops * row, cudaMemcpyDeviceToDevice));
-  return 0;
-}
-
-extern "C" int sdb_sview_accumulate(sdb_sview_t *v, const int32_t *j0, const int32_t *nb, const float *va,
-                                    const float *vc, size_t n_hops)
-{
-  if (!v) return fail("null view");
-  CK(cudaSetDevice(v->device));
-  CK(sdb_launch_sview_accumulate(0, v->spectrum_size, j0, nb, va, vc, (int) n_hops, v->max_bins, v->d_psd, v->d_accum,
-                                 v->d_count, v->d_count_snap));
-  return 0;
-}
-
-extern "C" int sdb_sview_read(sdb_sview_t *v, float *psd, float *accum, float *count, size_t cap)
-{
-  if (!v) return fail("null view");
-  if (cap < v->spectrum_size) return fail("destination too small");
-  CK(cudaSetDevice(v->device));
-  CK(cudaDeviceSynchronize());
-  const size_t n = v->spectrum_size * sizeof(float);
-  if (psd) CK(cudaMemcpy(psd, v->d_psd, n, cudaMemcpyDeviceToHost));
-  if (accum) CK(cudaMemcpy(accum, v->d_accum, n, cudaMemcpyDeviceToHost));
-  if (count) CK(cudaMemcpy(count, v->d_count, n, cudaMemcpyDeviceToHost));
   return 0;
 }

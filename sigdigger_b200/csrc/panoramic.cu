@@ -14,8 +14,7 @@
 // {j0, nb, va, vc (, channel lists)} of its shard into one device buffer and rank 0 posts one ncclRecv per peer
 // inside a group (ncclSend on the peers).  NCCL is bound at run time (dlopen "libnccl.so.2": the process that
 // initialised torch.distributed has it loaded already); a single rank needs no NCCL at all.
-#include "../../include/sigdigger_b200.h"
-#include <cuda_runtime.h>
+#include "sdb_internal.h"
 #include <nccl.h>
 #include <dlfcn.h>
 
@@ -70,9 +69,8 @@ void shard(size_t n_hops, int world, int rank, size_t *lo, size_t *hi)
 // the peers own arrays of their shard's size and send them section by section to the rows [lo_r, hi_r) of rank 0
 // (one NCCL group of ncclSend / ncclRecv): nothing is unpacked or copied after the gather.
 struct HopLists {
-  int32_t *j0 = nullptr, *nb = nullptr; float *va = nullptr, *vc = nullptr;
-  int32_t *ccnt = nullptr; sdb_detected_channel *chan = nullptr;
-  size_t rows = 0;
+  DevBuf<int32_t> j0, nb; DevBuf<float> va, vc;
+  DevBuf<int32_t> ccnt; DevBuf<sdb_detected_channel> chan;
 };
 
 // Rank 0, after the gather: the per-hop channel lists ([hops][cap], mostly empty) packed hop after hop, so that the
@@ -128,11 +126,11 @@ struct sdb_panoramic {
   sdb_sview_t *view = nullptr;
   size_t mb = 0;
   HopLists lists;
-  double *d_centers = nullptr; size_t centers_cap = 0;
-  float *d_db = nullptr; size_t db_cap = 0;
+  DevBuf<double> d_centers;
+  DevBuf<float> d_db;
   // rank 0, detector: the gathered channel lists land in pinned host memory behind ev_chan
-  int32_t *h_off = nullptr; sdb_detected_channel *h_chan = nullptr; size_t h_rows = 0, n_hops_last = 0;
-  int32_t *d_off = nullptr; sdb_detected_channel *d_dense = nullptr; size_t dense_cap = 0;
+  PinnedBuf<int32_t> h_off; PinnedBuf<sdb_detected_channel> h_chan; size_t n_hops_last = 0;
+  DevBuf<int32_t> d_off; DevBuf<sdb_detected_channel> d_dense; size_t dense_cap = 0;
   std::vector<sdb_detected_channel> h_full; std::vector<int32_t> h_full_cnt; bool full_valid = false;   // overflow path
   std::vector<double> centers_last;            // hop centres of the last sweep (already on the device)
   cudaEvent_t ev_chan = nullptr, ev_eng = nullptr; bool chan_pending = false;
@@ -182,12 +180,6 @@ extern "C" sdb_panoramic_t *sdb_panoramic_new(const sdb_panoramic_params *p, int
   return s;
 }
 
-static void free_lists(HopLists &l)
-{
-  cudaFree(l.j0); cudaFree(l.nb); cudaFree(l.va); cudaFree(l.vc); cudaFree(l.ccnt); cudaFree(l.chan);
-  l = HopLists();
-}
-
 extern "C" void sdb_panoramic_destroy(sdb_panoramic_t *s)
 {
   if (!s) return;
@@ -196,9 +188,6 @@ extern "C" void sdb_panoramic_destroy(sdb_panoramic_t *s)
   if (s->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(s->comm);
   if (s->eng) sdb_engine_destroy(s->eng);
   if (s->view) sdb_sview_destroy(s->view);
-  free_lists(s->lists);
-  cudaFree(s->d_centers); cudaFree(s->d_db);
-  cudaFreeHost(s->h_off); cudaFreeHost(s->h_chan); cudaFree(s->d_off); cudaFree(s->d_dense);
   for (auto &e : s->ev) if (e) cudaEventDestroy(e);
   if (s->ev_chan) cudaEventDestroy(s->ev_chan);
   if (s->ev_eng) cudaEventDestroy(s->ev_eng);
@@ -206,41 +195,27 @@ extern "C" void sdb_panoramic_destroy(sdb_panoramic_t *s)
   delete s;
 }
 
-// stream-ordered pieces of engine.cu / chdet_kernels.cu (same library, not part of the C-ABI)
-int sdb_sview_project_async(sdb_sview_t *v, cudaStream_t st, const float *psd_dev, size_t psd_size, size_t hop_stride,
-                            int psd_is_linear, const double *centers_dev, size_t n_hops, int adjust_sides, int32_t *j0,
-                            int32_t *nb, float *va, float *vc);
-int sdb_sview_accumulate_async(sdb_sview_t *v, cudaStream_t st, const int32_t *j0, const int32_t *nb, const float *va,
-                               const float *vc, size_t n_hops);
-int sdb_engine_pack_channels_device(sdb_engine_t *e, const double *centers_dev, sdb_detected_channel *out_dev, size_t cap,
-                                    int *counts_dev, cudaStream_t st);
-int sdb_psd_shift_db_async(cudaStream_t st, const float *lin_dev, float *db_dev, size_t n_frames, uint32_t psd_size);
-
 static int ensure(sdb_panoramic *s, size_t n_hops, size_t n_local)
 {
   const size_t rows = s->rank == 0 ? n_hops : n_local, mb = s->mb, cap = s->prm.channel_cap;
-  if (s->lists.rows < rows) {
+  // The row count of each group of buffers is the size of one of them, released first and allocated last: after a
+  // failed allocation it is 0, so the next sweep allocates the whole group again.
+  HopLists &l = s->lists;
+  if (l.j0.size() < rows) {
     PCK(cudaStreamSynchronize(s->stream));
-    free_lists(s->lists);
-    HopLists &l = s->lists;
-    PCK(cudaMalloc(&l.j0, rows * sizeof(int32_t))); PCK(cudaMalloc(&l.nb, rows * sizeof(int32_t)));
-    PCK(cudaMalloc(&l.va, rows * mb * sizeof(float))); PCK(cudaMalloc(&l.vc, rows * mb * sizeof(float)));
-    if (s->prm.detect) {
-      PCK(cudaMalloc(&l.ccnt, rows * sizeof(int32_t)));
-      PCK(cudaMalloc(&l.chan, rows * cap * sizeof(sdb_detected_channel)));
-    }
-    l.rows = rows;
+    l.j0.release();
+    s->n_hops_last = 0;                    // the lists of the last sweep are gone
+    PCK(l.nb.alloc(rows)); PCK(l.va.alloc(rows * mb)); PCK(l.vc.alloc(rows * mb));
+    if (s->prm.detect) { PCK(l.ccnt.alloc(rows)); PCK(l.chan.alloc(rows * cap)); }
+    PCK(l.j0.alloc(rows));
   }
-  if (s->centers_cap < n_hops) {
+  if (s->d_centers.size() < n_hops) {
     PCK(cudaStreamSynchronize(s->stream));
-    cudaFree(s->d_centers); s->d_centers = nullptr;
-    PCK(cudaMalloc(&s->d_centers, n_hops * sizeof(double)));
-    s->centers_cap = n_hops;
+    PCK(s->d_centers.alloc(n_hops));
   }
-  if (s->rank == 0 && s->prm.detect && s->h_rows < n_hops) {
+  if (s->rank == 0 && s->prm.detect && s->h_off.size() < n_hops + 1) {
     PCK(cudaStreamSynchronize(s->stream));
-    cudaFreeHost(s->h_off); cudaFreeHost(s->h_chan); cudaFree(s->d_off); cudaFree(s->d_dense);
-    s->h_off = nullptr; s->h_chan = nullptr; s->d_off = nullptr; s->d_dense = nullptr;
+    s->h_off.release();                    // sdb_panoramic_read_channels reads nothing until the lists are complete
     // room for 8 channels per hop on average (the lists hold up to `cap` each); a sweep that finds more is read
     // back in full, on demand (sdb_panoramic_read_channels)
     s->dense_cap = std::min(n_hops * cap, 8 * n_hops + 256);
@@ -248,11 +223,8 @@ static int ensure(sdb_panoramic *s, size_t n_hops, size_t n_local)
       const long v = atol(env);
       if (v >= 1) s->dense_cap = std::min(s->dense_cap, (size_t) v);
     }
-    PCK(cudaMallocHost(&s->h_off, (n_hops + 1) * sizeof(int32_t)));
-    PCK(cudaMallocHost(&s->h_chan, s->dense_cap * sizeof(sdb_detected_channel)));
-    PCK(cudaMalloc(&s->d_off, (n_hops + 1) * sizeof(int32_t)));
-    PCK(cudaMalloc(&s->d_dense, s->dense_cap * sizeof(sdb_detected_channel)));
-    s->h_rows = n_hops;
+    PCK(s->h_chan.alloc(s->dense_cap)); PCK(s->d_off.alloc(n_hops + 1)); PCK(s->d_dense.alloc(s->dense_cap));
+    PCK(s->h_off.alloc(n_hops + 1));
   }
   if (n_local && (!s->eng || s->eng_hops != n_local)) {
     if (s->eng) sdb_engine_destroy(s->eng);
@@ -309,10 +281,9 @@ static int sweep_impl(sdb_panoramic *s, const sdb_complex *hops_local, int on_de
                                      l.j0 + row0, l.nb + row0, l.va + row0 * mb, l.vc + row0 * mb);
     if (rc == 1) {
       // geometry outside the tiled kernel (a hop narrower than two view bins, or very wide): dB frames, contiguous
-      if (s->db_cap < n_local * N) {
+      if (s->d_db.size() < n_local * N) {
         PCK(cudaStreamSynchronize(st));
-        cudaFree(s->d_db); s->d_db = nullptr;
-        PCK(cudaMalloc(&s->d_db, n_local * N * sizeof(float))); s->db_cap = n_local * N;
+        PCK(s->d_db.alloc(n_local * N));
       }
       if (s->prm.detect) {
         for (size_t h = 0; h < (F == 1 ? 1 : n_local); ++h)
@@ -388,7 +359,6 @@ extern "C" int sdb_panoramic_sweep_host(sdb_panoramic_t *s, const sdb_complex *h
                                         size_t n_hops)
 { return sweep_impl(s, hops_local, 0, centers_all, n_hops); }
 
-int sdb_sview_reset_async(sdb_sview_t *v, cudaStream_t st);
 extern "C" int sdb_panoramic_reset(sdb_panoramic_t *s)
 {
   if (!s) return pfail("null");
@@ -404,7 +374,7 @@ extern "C" int sdb_panoramic_read(sdb_panoramic_t *s, float *psd, float *accum, 
 extern "C" uint32_t sdb_panoramic_size(const sdb_panoramic_t *s) { return s ? sdb_sview_size(s->view) : 0; }
 extern "C" long sdb_panoramic_read_channels(sdb_panoramic_t *s, size_t hop, sdb_detected_channel *out, size_t cap)
 {
-  if (!s || s->rank != 0 || !s->prm.detect || hop >= s->n_hops_last || !s->h_off) return -1;
+  if (!s || s->rank != 0 || !s->prm.detect || hop >= s->n_hops_last || !s->h_off.size()) return -1;
   if (s->chan_pending) { cudaEventSynchronize(s->ev_chan); s->chan_pending = false; }
   const size_t n_hops = s->n_hops_last, pc = s->prm.channel_cap;
   if ((size_t) s->h_off[n_hops] <= s->dense_cap) {

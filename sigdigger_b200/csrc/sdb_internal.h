@@ -1,5 +1,5 @@
-// sdb_internal.h -- structures shared by the host runtime (engine.cu) and the kernels.
-// Product code: nothing here includes or links oracle/.
+// sdb_internal.h -- structures shared by the host runtime and the kernels, and the declarations the library's units
+// share with each other.  Product code: nothing here includes or links oracle/.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,6 +7,59 @@
 #include "sdb_iq.h"
 #ifdef __cplusplus
 #include <atomic>
+#include <string>
+
+// ---------------------------------------------------------------------------------------------
+// error sink: the message sdb_last_error() returns (defined in engine.cu).  fail() sets it and returns -1; CK / CKP
+// return -1 / nullptr from the calling function when a CUDA call fails.
+// ---------------------------------------------------------------------------------------------
+extern thread_local std::string g_err __attribute__((visibility("hidden")));
+static inline int fail(const std::string &m) { g_err = m; return -1; }
+#define CK(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { \
+  g_err = std::string(#expr) + ": " + cudaGetErrorString(e__); return -1; } } while (0)
+#define CKP(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { \
+  g_err = std::string(#expr) + ": " + cudaGetErrorString(e__); return nullptr; } } while (0)
+
+// ---------------------------------------------------------------------------------------------
+// Device memory (or, Pinned, page-locked host memory) with one owner.  The element count is part of the buffer:
+// alloc() frees the old allocation first and leaves size 0 when the new one fails, so a failed reallocation can never
+// leave a stale size beside a null pointer.  Move-only; the destructor frees.
+// ---------------------------------------------------------------------------------------------
+template <typename T, bool Pinned = false> class DevBuf {
+public:
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+  DevBuf &operator=(DevBuf &&o) noexcept
+  {
+    if (this != &o) { release(); p_ = o.p_; n_ = o.n_; o.p_ = nullptr; o.n_ = 0; }
+    return *this;
+  }
+  ~DevBuf() { release(); }
+  cudaError_t alloc(size_t n)
+  {
+    release();
+    void *p = nullptr;
+    const cudaError_t e = Pinned ? cudaMallocHost(&p, n * sizeof(T)) : cudaMalloc(&p, n * sizeof(T));
+    if (e != cudaSuccess) { cudaGetLastError(); return e; }
+    p_ = (T *) p; n_ = n;
+    return cudaSuccess;
+  }
+  void release()
+  {
+    if (p_) { if (Pinned) cudaFreeHost(p_); else cudaFree(p_); }
+    p_ = nullptr; n_ = 0;
+  }
+  size_t size() const { return n_; }
+  T *get() const { return p_; }
+  operator T *() const { return p_; }
+private:
+  T *p_ = nullptr;
+  size_t n_ = 0;
+};
+template <typename T> using PinnedBuf = DevBuf<T, true>;
+
 // cudaFuncSetAttribute applies to the CURRENT device: a process that drives several GPUs (one GUI process, two
 // analyzers) must set it once per device, not once per process.  Returns true the first time on each device.
 static inline bool sdb_first_on_device(std::atomic<unsigned long long> &mask)
@@ -305,29 +358,30 @@ cudaError_t sdb_launch_spectsrc(const SdbLaunchCtx &c, const SdbSpectCfg *cfg_de
                                 int n_channels, int n_streams, int max_ns, const float2 *chan_in,
                                 size_t chan_stream_stride, uint32_t n_hops, float *spect, size_t spect_stream_stride,
                                 uint32_t *spect_size, float *est, int *est_valid);
-cudaError_t sdb_launch_task_xlate(cudaStream_t s, const float2 *src, float2 *dst, size_t n, size_t batch,
-                                  float omega, float phi0);
-cudaError_t sdb_launch_task_chain_state(cudaStream_t s, const float2 *src, float2 *dst, size_t n, int mode, float *st);
-size_t sdb_costas_k_bytes(void);
-size_t sdb_costas_s_bytes(void);
-cudaError_t sdb_launch_task_quad(cudaStream_t s, const float2 *src, float2 *dst, size_t n, size_t batch);
-cudaError_t sdb_launch_task_chain(cudaStream_t s, const float2 *src, float2 *dst, size_t n, size_t batch,
-                                  const SdbChainCfg *cfg_dev, int mode, float *pool, size_t pool_stride);
-// tasks_kernels.cu (SPEC Y)
-cudaError_t sdb_launch_task_delayed_conj(cudaStream_t s, const float2 *src, float2 *dst, size_t n, size_t batch,
-                                         size_t delay);
-cudaError_t sdb_launch_task_hist(cudaStream_t s, const float2 *src, float *out, size_t n, size_t batch, int space);
-cudaError_t sdb_launch_task_sample_manual(cudaStream_t s, const float2 *src, size_t n, size_t batch, int space,
-                                          double sync, double delta, double samp_offset, float delta_inv,
-                                          long long count, float2 *out);
-cudaError_t sdb_launch_task_zero_crossing(cudaStream_t s, const float2 *src, size_t n, size_t batch, int space,
-                                          int amplitude, float thres, float2 zca, float bnor, unsigned char *ev,
-                                          size_t ev_pitch, unsigned char *sym, unsigned *counts, size_t cap);
-cudaError_t sdb_launch_task_carrier_prep(cudaStream_t s, const float2 *src, const float *w, size_t n, size_t alloc,
-                                         size_t batch, float2 *dst);
-cudaError_t sdb_launch_task_carrier_find(cudaStream_t s, const float *psd, size_t alloc, size_t batch, int bins,
-                                         int delta, int skip, float *peak);
+// tasks_kernels.cu
 cudaError_t sdb_launch_dc_remove(cudaStream_t st, const void *x, int fmt, size_t stream_stride, size_t n, int n_streams,
                                  float alpha, float2 *state, float2 *cur, double2 *part, float2 *out);
-cudaError_t sdb_launch_task_decide(cudaStream_t s, const float2 *x, unsigned char *sym, size_t n, int mode, float dmin,
-                                   float dh, int intervals);
+
+#ifdef __cplusplus
+#include "../../include/sigdigger_b200.h"
+// chdet_kernels.cu: the engine's detector pass, and the channel lists converted to Hz on the device
+cudaError_t sdb_chdet_feed_stream(sdb_chdet_t *d, const float *psd_dev, uint32_t frames, size_t stream_stride,
+                                  cudaStream_t stream, uint64_t *launch_counter);
+cudaError_t sdb_chdet_pack_device(sdb_chdet_t *d, double samp_rate, const double *centers_dev,
+                                  sdb_detected_channel *out_dev, size_t cap, int *counts_dev, cudaStream_t stream);
+// stream-ordered pieces of the panoramic sweep (panoramic.cu): caller-owned device buffers, no host copies, no
+// default-stream work.  engine.cu:
+int sdb_engine_pack_channels_device(sdb_engine_t *e, const double *centers_dev, sdb_detected_channel *out_dev, size_t cap,
+                                    int *counts_dev, cudaStream_t st);
+// sview_kernels.cu.  psd_dev: hop h's frame at psd_dev + h * hop_stride; psd_is_linear: the engine's linear
+// natural-order PSD (the PSDMessage conversion happens inside the projection) instead of shifted dB; centers_dev: the
+// hop centres on the device.  Returns 1 when the geometry needs the general kernel (histogram mode or a very wide hop):
+// the caller then converts and calls with psd_is_linear = 0.
+int sdb_sview_project_async(sdb_sview_t *v, cudaStream_t st, const float *psd_dev, size_t psd_size, size_t hop_stride,
+                            int psd_is_linear, const double *centers_dev, size_t n_hops, int adjust_sides, int32_t *j0,
+                            int32_t *nb, float *va, float *vc);
+int sdb_sview_accumulate_async(sdb_sview_t *v, cudaStream_t st, const int32_t *j0, const int32_t *nb, const float *va,
+                               const float *vc, size_t n_hops);
+int sdb_sview_reset_async(sdb_sview_t *v, cudaStream_t st);
+int sdb_psd_shift_db_async(cudaStream_t st, const float *lin_dev, float *db_dev, size_t n_frames, uint32_t psd_size);
+#endif

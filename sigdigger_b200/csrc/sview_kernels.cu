@@ -189,10 +189,10 @@ __global__ void k_sview_project_tiled(SviewGeom g, const float *__restrict__ psd
 }
 
 // linear mode for every hop <=> the hop covers at least two destination bins (Scanner.cpp:254-262)
-cudaError_t sdb_launch_sview_project_tiled(cudaStream_t s, double freq_min, double freq_range, double fft_bandwidth,
-                                           float rel_bw, unsigned spectrum_size, const float *psd, size_t psd_size,
-                                           size_t hop_stride, int psd_is_linear, const double *centers_dev, int n_hops,
-                                           int adjust_sides, int *j0, int *nb, float *va, float *vc, int max_bins)
+static cudaError_t sdb_launch_sview_project_tiled(cudaStream_t s, double freq_min, double freq_range, double fft_bandwidth,
+                                                  float rel_bw, unsigned spectrum_size, const float *psd, size_t psd_size,
+                                                  size_t hop_stride, int psd_is_linear, const double *centers_dev, int n_hops,
+                                                  int adjust_sides, int *j0, int *nb, float *va, float *vc, int max_bins)
 {
   SviewGeom g{ freq_min, freq_range, fft_bandwidth, rel_bw, spectrum_size };
   if (n_hops <= 0) return cudaSuccess;
@@ -274,9 +274,9 @@ __global__ void k_sview_project_view(SviewGeom g, const float *__restrict__ src_
   }
 }
 
-cudaError_t sdb_launch_sview_project_view(cudaStream_t s, double freq_min, double freq_range, unsigned spectrum_size,
-                                          const float *src_acc, const float *src_cnt, unsigned src_size, double fmin,
-                                          double fmax, int *j0, int *nb, float *va, float *vc)
+static cudaError_t sdb_launch_sview_project_view(cudaStream_t s, double freq_min, double freq_range, unsigned spectrum_size,
+                                                 const float *src_acc, const float *src_cnt, unsigned src_size, double fmin,
+                                                 double fmax, int *j0, int *nb, float *va, float *vc)
 {
   SviewGeom g{ freq_min, freq_range, 0.0, 0.0f, spectrum_size };
   k_sview_project_view<<<(spectrum_size + 255) / 256, 256, 0, s>>>(g, src_acc, src_cnt, src_size, fmin, fmax, j0, nb,
@@ -371,10 +371,10 @@ __global__ void k_sview_fill(unsigned spectrum_size, float *__restrict__ psd, co
   }
 }
 
-cudaError_t sdb_launch_sview_project(cudaStream_t s, double freq_min, double freq_range, double fft_bandwidth,
-                                     float rel_bw, unsigned spectrum_size, const float *psd, size_t psd_size,
-                                     const double *centers_dev, int n_hops, int adjust_sides, int *j0, int *nb,
-                                     float *va, float *vc, int max_bins)
+static cudaError_t sdb_launch_sview_project(cudaStream_t s, double freq_min, double freq_range, double fft_bandwidth,
+                                            float rel_bw, unsigned spectrum_size, const float *psd, size_t psd_size,
+                                            const double *centers_dev, int n_hops, int adjust_sides, int *j0, int *nb,
+                                            float *va, float *vc, int max_bins)
 {
   SviewGeom g{ freq_min, freq_range, fft_bandwidth, rel_bw, spectrum_size };
   if (n_hops <= 0) return cudaSuccess;
@@ -382,9 +382,9 @@ cudaError_t sdb_launch_sview_project(cudaStream_t s, double freq_min, double fre
   return cudaGetLastError();
 }
 
-cudaError_t sdb_launch_sview_accumulate(cudaStream_t s, unsigned spectrum_size, const int *j0, const int *nb,
-                                        const float *va, const float *vc, int n_hops, int max_bins, float *psd,
-                                        float *accum, float *count, float *count_snapshot)
+static cudaError_t sdb_launch_sview_accumulate(cudaStream_t s, unsigned spectrum_size, const int *j0, const int *nb,
+                                               const float *va, const float *vc, int n_hops, int max_bins, float *psd,
+                                               float *accum, float *count, float *count_snapshot)
 {
   if (n_hops > 0) {
     cudaError_t e = cudaMemcpyAsync(count_snapshot, count, (size_t) spectrum_size * sizeof(float),
@@ -431,8 +431,8 @@ __global__ void k_psd_average(const float *__restrict__ psd, size_t stream_strid
   last[t] = v;
 }
 
-cudaError_t sdb_launch_psd_average(cudaStream_t s, const float *psd, size_t stream_stride, unsigned frames, unsigned n,
-                                   size_t n_streams, float alpha, int primed, float *last)
+static cudaError_t sdb_launch_psd_average(cudaStream_t s, const float *psd, size_t stream_stride, unsigned frames, unsigned n,
+                                          size_t n_streams, float alpha, int primed, float *last)
 {
   if (frames == 0 || n_streams * n == 0) return cudaSuccess;
   k_psd_average<<<(unsigned) ((n_streams * n + 255) / 256), 256, 0, s>>>(psd, stream_stride, frames, n, n_streams,
@@ -440,7 +440,7 @@ cudaError_t sdb_launch_psd_average(cudaStream_t s, const float *psd, size_t stre
   return cudaGetLastError();
 }
 
-cudaError_t sdb_launch_psd_shift_db(cudaStream_t s, const float *lin, float *db, size_t n_frames, unsigned n)
+static cudaError_t sdb_launch_psd_shift_db(cudaStream_t s, const float *lin, float *db, size_t n_frames, unsigned n)
 {
   const size_t total = n_frames * n;
   if (total == 0) return cudaSuccess;
@@ -448,4 +448,297 @@ cudaError_t sdb_launch_psd_shift_db(cudaStream_t s, const float *lin, float *db,
   if (blocks > 132 * 16) blocks = 132 * 16;        // 16 CTAs on each of an H100's 132 SMs, grid-stride beyond
   k_psd_shift_db<<<(unsigned) blocks, 256, 0, s>>>(lin, db, total, n);
   return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------
+// SpectrumView (Panoramic/Scanner.cpp:36-293): panoramic stitcher
+// ---------------------------------------------------------------------------------------------
+
+struct sdb_sview {
+  int device = 0;
+  double freq_min = 0, freq_max = 0, freq_range = 0, fft_bandwidth = 0;
+  float rel_bw = 0.5f;                     // include/Scanner.h:70
+  unsigned spectrum_size = 65536;          // SIGDIGGER_SCANNER_SPECTRUM_SIZE
+  int max_bins = 0;
+  DevBuf<float> d_psd, d_accum, d_count, d_count_snap;
+  // contribution lists of the last sdb_sview_project: j0 / nb [hops], va / vc [hops][max_bins]
+  DevBuf<double> d_centers; DevBuf<int> d_j0, d_nb; DevBuf<float> d_va, d_vc;
+};
+
+extern "C" sdb_sview_t *sdb_sview_new(int device)
+{
+  if (sdb_device_count() <= 0) { g_err = "no CUDA device: sigdigger_b200 has no CPU fallback"; return nullptr; }
+  CKP(cudaSetDevice(device));
+  sdb_sview *v = new sdb_sview();
+  v->device = device;
+  const size_t n = 65536 * sizeof(float);
+  if (v->d_psd.alloc(65536) != cudaSuccess || v->d_accum.alloc(65536) != cudaSuccess ||
+      v->d_count.alloc(65536) != cudaSuccess || v->d_count_snap.alloc(65536) != cudaSuccess) {
+    g_err = "out of device memory"; delete v; return nullptr;
+  }
+  cudaMemset(v->d_psd, 0, n); cudaMemset(v->d_accum, 0, n); cudaMemset(v->d_count, 0, n);
+  return v;
+}
+
+extern "C" void sdb_sview_destroy(sdb_sview_t *v)
+{
+  if (!v) return;
+  cudaSetDevice(v->device);
+  delete v;
+}
+
+extern "C" int sdb_sview_reset(sdb_sview_t *v)
+{
+  if (!v) return fail("null view");
+  CK(cudaSetDevice(v->device));
+  const size_t n = 65536 * sizeof(float);          // SpectrumView::reset, Scanner.cpp:287-293
+  CK(cudaMemset(v->d_psd, 0, n)); CK(cudaMemset(v->d_accum, 0, n)); CK(cudaMemset(v->d_count, 0, n));
+  return 0;
+}
+
+int sdb_sview_reset_async(sdb_sview_t *v, cudaStream_t st)     // the same, ordered on the caller's stream
+{
+  if (!v) return fail("null view");
+  const size_t n = 65536 * sizeof(float);
+  CK(cudaMemsetAsync(v->d_psd, 0, n, st)); CK(cudaMemsetAsync(v->d_accum, 0, n, st));
+  CK(cudaMemsetAsync(v->d_count, 0, n, st));
+  return 0;
+}
+
+extern "C" int sdb_sview_set_range(sdb_sview_t *v, double fmin, double fmax, double fft_bandwidth, float rel_bw)
+{
+  if (!v) return fail("null view");
+  if (!(fmax > fmin) || !(fft_bandwidth > 0)) return fail("invalid frequency range");
+  v->freq_min = fmin; v->freq_max = fmax; v->freq_range = fmax - fmin;   // setRange, Scanner.cpp:41-54
+  unsigned n = (unsigned) (v->freq_range / 1000.0), sz = 1;               // SIGDIGGER_SCANNER_FREQ_RESOLUTION
+  while (sz < n) sz <<= 1;
+  if (sz > 65536) sz = 65536;
+  v->spectrum_size = sz;
+  v->fft_bandwidth = fft_bandwidth; v->rel_bw = rel_bw;
+  // a hop contributes at most sz * (fft_bandwidth - 2 skip) / freq_range + 1 bins, and every projection uses THIS
+  // fft_bandwidth (the kernels take the geometry from the view, not from the call): the `nb > max_bins` clamp in the
+  // projection kernels is a guard that cannot bind
+  double mb = (double) sz * fft_bandwidth / v->freq_range + 4.0;
+  v->max_bins = mb > (double) sz ? (int) sz : (int) mb;
+  if (v->max_bins < 2) v->max_bins = 2;
+  v->d_centers.release();   // the contribution lists depend on max_bins: sdb_sview_project reallocates them
+  return sdb_sview_reset(v);
+}
+
+extern "C" uint32_t sdb_sview_size(const sdb_sview_t *v) { return v ? v->spectrum_size : 0; }
+extern "C" uint32_t sdb_sview_max_bins(const sdb_sview_t *v) { return v ? (uint32_t) v->max_bins : 0; }
+
+extern "C" int sdb_sview_project(sdb_sview_t *v, const float *psd_dev, size_t psd_size, const double *centers,
+                                 size_t n_hops, int adjust_sides)
+{
+  if (!v || !psd_dev || !centers) return fail("null argument");
+  if (v->max_bins <= 0) return fail("set_range first");
+  CK(cudaSetDevice(v->device));
+  if (n_hops > v->d_centers.size()) {
+    // d_centers is released first and allocated last: its size is 0 until every list has been allocated
+    v->d_centers.release();
+    CK(v->d_j0.alloc(n_hops)); CK(v->d_nb.alloc(n_hops));
+    CK(v->d_va.alloc(n_hops * (size_t) v->max_bins)); CK(v->d_vc.alloc(n_hops * (size_t) v->max_bins));
+    CK(v->d_centers.alloc(n_hops));
+  }
+  CK(cudaMemcpy(v->d_centers, centers, n_hops * sizeof(double), cudaMemcpyHostToDevice));
+  CK(cudaMemset(v->d_va, 0, n_hops * (size_t) v->max_bins * sizeof(float)));
+  CK(cudaMemset(v->d_vc, 0, n_hops * (size_t) v->max_bins * sizeof(float)));
+  CK(sdb_launch_sview_project(0, v->freq_min, v->freq_range, v->fft_bandwidth, v->rel_bw, v->spectrum_size, psd_dev,
+                              psd_size, v->d_centers, (int) n_hops, adjust_sides, v->d_j0, v->d_nb, v->d_va, v->d_vc,
+                              v->max_bins));
+  return 0;
+}
+
+// ---- stream-ordered variants for the panoramic sweep (sdb_internal.h)
+int sdb_sview_project_async(sdb_sview_t *v, cudaStream_t st, const float *psd_dev, size_t psd_size, size_t hop_stride,
+                            int psd_is_linear, const double *centers_dev, size_t n_hops, int adjust_sides, int32_t *j0,
+                            int32_t *nb, float *va, float *vc)
+{
+  if (!v || !psd_dev || !centers_dev || !j0 || !nb || !va || !vc) return fail("null argument");
+  if (v->max_bins <= 0) return fail("set_range first");
+  const bool linear_mode = v->fft_bandwidth / v->freq_range * v->spectrum_size >= 2.001;  // every hop, with margin
+                                                                                              // for the kernel's own test
+  if (linear_mode && v->max_bins <= 384) {
+    CK(sdb_launch_sview_project_tiled(st, v->freq_min, v->freq_range, v->fft_bandwidth, v->rel_bw, v->spectrum_size,
+                                      psd_dev, psd_size, hop_stride, psd_is_linear, centers_dev, (int) n_hops,
+                                      adjust_sides, j0, nb, va, vc, v->max_bins));
+    return 0;
+  }
+  if (psd_is_linear || hop_stride != psd_size) return 1;
+  CK(sdb_launch_sview_project(st, v->freq_min, v->freq_range, v->fft_bandwidth, v->rel_bw, v->spectrum_size, psd_dev,
+                              psd_size, centers_dev, (int) n_hops, adjust_sides, j0, nb, va, vc, v->max_bins));
+  return 0;
+}
+
+int sdb_sview_accumulate_async(sdb_sview_t *v, cudaStream_t st, const int32_t *j0, const int32_t *nb, const float *va,
+                               const float *vc, size_t n_hops)
+{
+  if (!v) return fail("null view");
+  CK(sdb_launch_sview_accumulate(st, v->spectrum_size, j0, nb, va, vc, (int) n_hops, v->max_bins, v->d_psd, v->d_accum,
+                                 v->d_count, v->d_count_snap));
+  return 0;
+}
+
+int sdb_psd_shift_db_async(cudaStream_t st, const float *lin_dev, float *db_dev, size_t n_frames, uint32_t psd_size)
+{
+  if (!lin_dev || !db_dev || lin_dev == db_dev) return fail("invalid argument");
+  CK(sdb_launch_psd_shift_db(st, lin_dev, db_dev, n_frames, psd_size));
+  return 0;
+}
+
+
+extern "C" int sdb_psd_shift_db_device(const float *lin_dev, float *db_dev, size_t n_frames, uint32_t psd_size)
+{
+  if (!lin_dev || !db_dev) return fail("null argument");
+  if (lin_dev == db_dev) return fail("in-place conversion is not supported (the halves swap)");
+  if (psd_size < 2 || (psd_size & (psd_size - 1))) return fail("psd_size must be a power of two");
+  CK(sdb_launch_psd_shift_db(0, lin_dev, db_dev, n_frames, psd_size));
+  return 0;
+}
+
+// ---- SpectrumView::feed(SpectrumView const &) (Panoramic/Scanner.cpp:276-286; used by the zoom path of
+// ---- Scanner::setViewRange, :471-479): project the other view's accumulators / counts, then the same accumulate
+// ---- + interpolate pass a hop gets.
+
+extern "C" int sdb_sview_feed_view(sdb_sview_t *v, const sdb_sview_t *detail)
+{
+  if (!v || !detail) return fail("null view");
+  if (v == detail) return fail("a view cannot be fed into itself");
+  if (v->max_bins <= 0 || detail->max_bins <= 0) return fail("set_range first");
+  if (v->device != detail->device) return fail("both views must live on the same device");
+  CK(cudaSetDevice(v->device));
+  DevBuf<int> j0, nb; DevBuf<float> va, vc;
+  const size_t row = 65536 * sizeof(float);
+  cudaError_t e = j0.alloc(1);
+  if (e == cudaSuccess) e = nb.alloc(1);
+  if (e == cudaSuccess) e = va.alloc(65536);
+  if (e == cudaSuccess) e = vc.alloc(65536);
+  if (e == cudaSuccess) e = cudaMemset(j0, 0, sizeof(int));
+  if (e == cudaSuccess) e = cudaMemset(nb, 0, sizeof(int));
+  if (e == cudaSuccess) e = cudaMemset(va, 0, row);
+  if (e == cudaSuccess) e = cudaMemset(vc, 0, row);
+  if (e == cudaSuccess)
+    e = sdb_launch_sview_project_view(0, v->freq_min, v->freq_range, v->spectrum_size, detail->d_accum, detail->d_count,
+                                      detail->spectrum_size, detail->freq_min, detail->freq_max, j0, nb, va, vc);
+  if (e == cudaSuccess)
+    e = sdb_launch_sview_accumulate(0, v->spectrum_size, j0, nb, va, vc, 1, 65536, v->d_psd, v->d_accum, v->d_count,
+                                    v->d_count_snap);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) return fail(std::string("sdb_sview_feed_view: ") + cudaGetErrorString(e));
+  return 0;
+}
+
+// ---- spectrum averager (Misc/Averager.cpp:25-60)
+struct sdb_averager {
+  int device = 0; unsigned n = 0; size_t n_streams = 0; float alpha = 1.0f; bool primed = false;
+  DevBuf<float> d_last;
+};
+
+extern "C" sdb_averager_t *sdb_averager_new(uint32_t psd_size, uint32_t n_streams, float alpha, int device)
+{
+  if (sdb_device_count() <= 0) { g_err = "no CUDA device: sigdigger_b200 has no CPU fallback"; return nullptr; }
+  if (psd_size == 0 || n_streams == 0) { g_err = "averager: empty geometry"; return nullptr; }
+  CKP(cudaSetDevice(device));
+  sdb_averager *a = new sdb_averager();
+  a->device = device; a->n = psd_size; a->n_streams = n_streams; a->alpha = alpha;
+  if (a->d_last.alloc((size_t) psd_size * n_streams) != cudaSuccess) {
+    g_err = "out of device memory"; delete a; return nullptr;
+  }
+  cudaMemset(a->d_last, 0, (size_t) psd_size * n_streams * sizeof(float));
+  return a;
+}
+
+extern "C" void sdb_averager_destroy(sdb_averager_t *a)
+{
+  if (!a) return;
+  cudaSetDevice(a->device);
+  delete a;
+}
+
+extern "C" int sdb_averager_set_alpha(sdb_averager_t *a, float alpha)
+{
+  if (!a) return fail("null averager");
+  a->alpha = alpha;
+  return 0;
+}
+
+extern "C" int sdb_averager_reset(sdb_averager_t *a)
+{
+  if (!a) return fail("null averager");
+  a->primed = false;
+  return 0;
+}
+
+extern "C" int sdb_averager_feed_device(sdb_averager_t *a, const float *psd_dev, size_t frames, size_t stream_stride)
+{
+  if (!a || !psd_dev) return fail("null argument");
+  if (frames == 0) return 0;
+  if (stream_stride < frames * a->n && a->n_streams > 1) return fail("stream stride smaller than the frames");
+  CK(cudaSetDevice(a->device));
+  CK(sdb_launch_psd_average(0, psd_dev, stream_stride, (unsigned) frames, a->n, a->n_streams, a->alpha,
+                            a->primed ? 1 : 0, a->d_last));
+  a->primed = true;
+  return 0;
+}
+
+extern "C" const float *sdb_averager_device(const sdb_averager_t *a) { return a ? a->d_last.get() : nullptr; }
+
+extern "C" int sdb_averager_read(sdb_averager_t *a, float *dst, size_t cap)
+{
+  if (!a || !dst) return fail("null argument");
+  const size_t tot = (size_t) a->n * a->n_streams;
+  if (cap < tot) return fail("destination too small");
+  CK(cudaSetDevice(a->device));
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(dst, a->d_last, tot * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+extern "C" int sdb_sview_contrib(sdb_sview_t *v, int32_t **j0, int32_t **nb, float **va, float **vc)
+{
+  if (!v) return fail("null view");
+  if (j0) *j0 = v->d_j0;
+  if (nb) *nb = v->d_nb;
+  if (va) *va = v->d_va;
+  if (vc) *vc = v->d_vc;
+  return 0;
+}
+
+// copy the last projection's contribution lists into caller-owned DEVICE buffers (the send buffers of the
+// NCCL gather): j0/nb [n_hops] int32, va/vc [n_hops][max_bins] float32
+extern "C" int sdb_sview_contrib_copy(sdb_sview_t *v, int32_t *j0, int32_t *nb, float *va, float *vc, size_t n_hops)
+{
+  if (!v || !j0 || !nb || !va || !vc) return fail("null argument");
+  if (n_hops > v->d_centers.size()) return fail("more hops than the last projection held");
+  CK(cudaSetDevice(v->device));
+  const size_t row = (size_t) v->max_bins * sizeof(float);
+  CK(cudaMemcpy(j0, v->d_j0, n_hops * sizeof(int), cudaMemcpyDeviceToDevice));
+  CK(cudaMemcpy(nb, v->d_nb, n_hops * sizeof(int), cudaMemcpyDeviceToDevice));
+  CK(cudaMemcpy(va, v->d_va, n_hops * row, cudaMemcpyDeviceToDevice));
+  CK(cudaMemcpy(vc, v->d_vc, n_hops * row, cudaMemcpyDeviceToDevice));
+  return 0;
+}
+
+extern "C" int sdb_sview_accumulate(sdb_sview_t *v, const int32_t *j0, const int32_t *nb, const float *va,
+                                    const float *vc, size_t n_hops)
+{
+  if (!v) return fail("null view");
+  CK(cudaSetDevice(v->device));
+  CK(sdb_launch_sview_accumulate(0, v->spectrum_size, j0, nb, va, vc, (int) n_hops, v->max_bins, v->d_psd, v->d_accum,
+                                 v->d_count, v->d_count_snap));
+  return 0;
+}
+
+extern "C" int sdb_sview_read(sdb_sview_t *v, float *psd, float *accum, float *count, size_t cap)
+{
+  if (!v) return fail("null view");
+  if (cap < v->spectrum_size) return fail("destination too small");
+  CK(cudaSetDevice(v->device));
+  CK(cudaDeviceSynchronize());
+  const size_t n = v->spectrum_size * sizeof(float);
+  if (psd) CK(cudaMemcpy(psd, v->d_psd, n, cudaMemcpyDeviceToHost));
+  if (accum) CK(cudaMemcpy(accum, v->d_accum, n, cudaMemcpyDeviceToHost));
+  if (count) CK(cudaMemcpy(count, v->d_count, n, cudaMemcpyDeviceToHost));
+  return 0;
 }

@@ -12,13 +12,8 @@
 // Bound: serial latency of the step (one processor advances a few MS/s; a batch scales with the SM count).
 // Compiled with -fmad=false: bit-identical to oracle/tvproc.c and to the host step of <sigutils/tvproc.h>.
 #include "sdb_tv_steps.h"
-#include "../../include/sigdigger_b200.h"
-#include <string>
 #include <vector>
 #include <string.h>
-
-int sdb_set_error(const char *m);
-#define TCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return sdb_set_error((std::string(#x) + ": " + cudaGetErrorString(e_)).c_str()); } while (0)
 
 __global__ void __launch_bounds__(32) k_tv_feed(const SdbTvCfg c, SdbTvState *__restrict__ states,
                                                 float *__restrict__ delays, float *__restrict__ lines,
@@ -79,8 +74,7 @@ __global__ void k_tv_feed_transform(const float2 *__restrict__ x, size_t n, int 
 struct sdb_tv_processor {
   int device = 0; unsigned batch = 0;
   sdb_tv_params prm; SdbTvCfg cfg;
-  SdbTvState *d_state = nullptr; float *d_delay = nullptr, *d_line = nullptr, *d_ring = nullptr, *d_x = nullptr;
-  unsigned *d_done = nullptr; size_t x_cap = 0;
+  DevBuf<SdbTvState> d_state; DevBuf<float> d_delay, d_line, d_ring, d_x; DevBuf<unsigned> d_done;
   cudaStream_t stream = nullptr;
 };
 
@@ -92,8 +86,6 @@ extern "C" void sdb_tv_processor_destroy(sdb_tv_processor_t *t)
   if (!t) return;
   cudaSetDevice(t->device);
   if (t->stream) { cudaStreamSynchronize(t->stream); cudaStreamDestroy(t->stream); }
-  cudaFree(t->d_state); cudaFree(t->d_delay); cudaFree(t->d_line); cudaFree(t->d_ring); cudaFree(t->d_x);
-  cudaFree(t->d_done);
   delete t;
 }
 
@@ -101,20 +93,18 @@ extern "C" void sdb_tv_processor_destroy(sdb_tv_processor_t *t)
 // high", :206) -- and, here, without a CUDA device (no CPU fallback)
 extern "C" sdb_tv_processor_t *sdb_tv_processor_new(const sdb_tv_params *p, uint32_t batch, int device)
 {
-  if (!p || batch < 1) { sdb_set_error("invalid arguments"); return nullptr; }
-  if (sdb_device_count() <= 0) { sdb_set_error("no CUDA device: sigdigger_b200 has no CPU fallback"); return nullptr; }
-  if (!sdb_tv_params_valid(*p)) { sdb_set_error("TV processor: invalid parameters"); return nullptr; }
-  if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); sdb_set_error("cudaSetDevice failed"); return nullptr; }
+  if (!p || batch < 1) { fail("invalid arguments"); return nullptr; }
+  if (sdb_device_count() <= 0) { fail("no CUDA device: sigdigger_b200 has no CPU fallback"); return nullptr; }
+  if (!sdb_tv_params_valid(*p)) { fail("TV processor: invalid parameters"); return nullptr; }
+  if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); fail("cudaSetDevice failed"); return nullptr; }
   sdb_tv_processor *t = new sdb_tv_processor();
   t->device = device; t->batch = batch; t->prm = *p;
   sdb_tv_derive(*p, t->cfg);
   const SdbTvCfg &c = t->cfg;
   const size_t B = batch;
-  bool ok = cudaMalloc(&t->d_state, B * sizeof(SdbTvState)) == cudaSuccess &&
-            cudaMalloc(&t->d_delay, B * c.delay_len * sizeof(float)) == cudaSuccess &&
-            cudaMalloc(&t->d_line, B * c.W * sizeof(float)) == cudaSuccess &&
-            cudaMalloc(&t->d_ring, B * SDB_TV_RING * c.H * c.W * sizeof(float)) == cudaSuccess &&
-            cudaMalloc(&t->d_done, B * sizeof(unsigned)) == cudaSuccess &&
+  bool ok = t->d_state.alloc(B) == cudaSuccess && t->d_delay.alloc(B * c.delay_len) == cudaSuccess &&
+            t->d_line.alloc(B * c.W) == cudaSuccess && t->d_ring.alloc(B * SDB_TV_RING * c.H * c.W) == cudaSuccess &&
+            t->d_done.alloc(B) == cudaSuccess &&
             cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking) == cudaSuccess;
   if (ok) {
     SdbTvState s0; sdb_tv_state_init(c, s0);
@@ -124,7 +114,7 @@ extern "C" sdb_tv_processor_t *sdb_tv_processor_new(const sdb_tv_params *p, uint
          cudaMemset(t->d_line, 0, B * c.W * sizeof(float)) == cudaSuccess &&
          cudaMemset(t->d_ring, 0, B * SDB_TV_RING * c.H * c.W * sizeof(float)) == cudaSuccess;
   }
-  if (!ok) { cudaGetLastError(); sdb_set_error("out of device memory (TV processor)"); sdb_tv_processor_destroy(t); return nullptr; }
+  if (!ok) { cudaGetLastError(); fail("out of device memory (TV processor)"); sdb_tv_processor_destroy(t); return nullptr; }
   return t;
 }
 
@@ -132,20 +122,20 @@ extern "C" sdb_tv_processor_t *sdb_tv_processor_new(const sdb_tv_params *p, uint
 // (tolerances, time constants, sync / AGC / comb switches, pulse lengths) takes effect at the next sample
 extern "C" int sdb_tv_processor_set_params(sdb_tv_processor_t *t, const sdb_tv_params *p)
 {
-  if (!t || !p) return sdb_set_error("null argument");
-  if (!sdb_tv_params_valid(*p)) return sdb_set_error("TV processor: invalid parameters");
+  if (!t || !p) return fail("null argument");
+  if (!sdb_tv_params_valid(*p)) return fail("TV processor: invalid parameters");
   SdbTvCfg c; sdb_tv_derive(*p, c);
   if (c.W != t->cfg.W || c.delay_len != t->cfg.delay_len || c.H != t->cfg.H || c.interlace != t->cfg.interlace)
-    return sdb_set_error("TV processor: picture geometry cannot change while running");
-  TCK(cudaSetDevice(t->device));
-  TCK(cudaStreamSynchronize(t->stream));
+    return fail("TV processor: picture geometry cannot change while running");
+  CK(cudaSetDevice(t->device));
+  CK(cudaStreamSynchronize(t->stream));
   t->prm = *p; t->cfg = c;
   return 0;
 }
 
 extern "C" int sdb_tv_processor_geometry(const sdb_tv_processor_t *t, uint32_t *width, uint32_t *height)
 {
-  if (!t) return sdb_set_error("null argument");
+  if (!t) return fail("null argument");
   if (width) *width = (uint32_t) t->cfg.W;
   if (height) *height = (uint32_t) t->cfg.H;
   return 0;
@@ -157,10 +147,10 @@ static long tv_feed(sdb_tv_processor *t, const float *x_dev, size_t stride, size
   const size_t smem = (size_t) (c.W + c.delay_len) * sizeof(float);
   k_tv_feed<<<t->batch, 32, smem, t->stream>>>(c, t->d_state, t->d_delay, t->d_line, t->d_ring, x_dev, stride, n,
                                                t->d_done);
-  TCK(cudaGetLastError());
+  CK(cudaGetLastError());
   std::vector<unsigned> h(t->batch);
-  TCK(cudaMemcpyAsync(h.data(), t->d_done, t->batch * sizeof(unsigned), cudaMemcpyDeviceToHost, t->stream));
-  TCK(cudaStreamSynchronize(t->stream));
+  CK(cudaMemcpyAsync(h.data(), t->d_done, t->batch * sizeof(unsigned), cudaMemcpyDeviceToHost, t->stream));
+  CK(cudaStreamSynchronize(t->stream));
   long total = 0;
   for (unsigned b = 0; b < t->batch; ++b) { if (frames_done) frames_done[b] = h[b]; total += h[b]; }
   return total;
@@ -170,18 +160,16 @@ static long tv_feed(sdb_tv_processor *t, const float *x_dev, size_t stride, size
 // Returns the number of frames completed in this call over the batch.
 extern "C" long sdb_tv_processor_feed(sdb_tv_processor_t *t, const float *x, size_t stride, size_t n, uint32_t *frames_done)
 {
-  if (!t || !x) return sdb_set_error("null argument");
+  if (!t || !x) return fail("null argument");
   if (n == 0) return 0;
-  if (stride < n) return sdb_set_error("stride < n");
-  TCK(cudaSetDevice(t->device));
+  if (stride < n) return fail("stride < n");
+  CK(cudaSetDevice(t->device));
   const size_t need = (size_t) t->batch * n;
-  if (t->x_cap < need) {
-    TCK(cudaStreamSynchronize(t->stream));
-    cudaFree(t->d_x); t->d_x = nullptr; t->x_cap = 0;
-    TCK(cudaMalloc(&t->d_x, need * sizeof(float)));
-    t->x_cap = need;
+  if (t->d_x.size() < need) {
+    CK(cudaStreamSynchronize(t->stream));
+    CK(t->d_x.alloc(need));
   }
-  TCK(cudaMemcpy2DAsync(t->d_x, n * sizeof(float), x, stride * sizeof(float), n * sizeof(float), t->batch,
+  CK(cudaMemcpy2DAsync(t->d_x, n * sizeof(float), x, stride * sizeof(float), n * sizeof(float), t->batch,
                         cudaMemcpyHostToDevice, t->stream));
   return tv_feed(t, t->d_x, n, n, frames_done);
 }
@@ -189,18 +177,18 @@ extern "C" long sdb_tv_processor_feed(sdb_tv_processor_t *t, const float *x, siz
 extern "C" long sdb_tv_processor_feed_device(sdb_tv_processor_t *t, const float *x_dev, size_t stride, size_t n,
                                              uint32_t *frames_done)
 {
-  if (!t || !x_dev) return sdb_set_error("null argument");
+  if (!t || !x_dev) return fail("null argument");
   if (n == 0) return 0;
-  TCK(cudaSetDevice(t->device));
+  CK(cudaSetDevice(t->device));
   return tv_feed(t, x_dev, stride, n, frames_done);
 }
 
 extern "C" int sdb_tv_processor_frames(sdb_tv_processor_t *t, uint64_t *counts)
 {
-  if (!t || !counts) return sdb_set_error("null argument");
-  TCK(cudaSetDevice(t->device));
+  if (!t || !counts) return fail("null argument");
+  CK(cudaSetDevice(t->device));
   std::vector<SdbTvState> h(t->batch);
-  TCK(cudaMemcpy(h.data(), t->d_state, t->batch * sizeof(SdbTvState), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(h.data(), t->d_state, t->batch * sizeof(SdbTvState), cudaMemcpyDeviceToHost));
   for (unsigned b = 0; b < t->batch; ++b) counts[b] = h[b].frames;
   return 0;
 }
@@ -210,24 +198,24 @@ extern "C" int sdb_tv_processor_frames(sdb_tv_processor_t *t, uint64_t *counts)
 // reads the picture in progress)
 extern "C" int sdb_tv_processor_read_frame(sdb_tv_processor_t *t, uint32_t which, uint64_t frame_no, float *out, size_t cap)
 {
-  if (!t || !out || which >= t->batch) return sdb_set_error("invalid argument");
+  if (!t || !out || which >= t->batch) return fail("invalid argument");
   const size_t px = (size_t) t->cfg.W * t->cfg.H;
-  if (cap < px) return sdb_set_error("destination too small");
-  TCK(cudaSetDevice(t->device));
+  if (cap < px) return fail("destination too small");
+  CK(cudaSetDevice(t->device));
   SdbTvState s;
-  TCK(cudaMemcpy(&s, t->d_state + which, sizeof(s), cudaMemcpyDeviceToHost));
-  if (frame_no > s.frames || frame_no + SDB_TV_RING <= s.frames) return sdb_set_error("frame no longer (or not yet) in the ring");
-  TCK(cudaMemcpy(out, t->d_ring + ((size_t) which * SDB_TV_RING + frame_no % SDB_TV_RING) * px, px * sizeof(float),
+  CK(cudaMemcpy(&s, t->d_state + which, sizeof(s), cudaMemcpyDeviceToHost));
+  if (frame_no > s.frames || frame_no + SDB_TV_RING <= s.frames) return fail("frame no longer (or not yet) in the ring");
+  CK(cudaMemcpy(out, t->d_ring + ((size_t) which * SDB_TV_RING + frame_no % SDB_TV_RING) * px, px * sizeof(float),
                  cudaMemcpyDeviceToHost));
   return 0;
 }
 
 extern "C" int sdb_tv_processor_estimates(sdb_tv_processor_t *t, uint32_t which, float *line_len, float *hsync_len, float *gain)
 {
-  if (!t || which >= t->batch) return sdb_set_error("invalid argument");
-  TCK(cudaSetDevice(t->device));
+  if (!t || which >= t->batch) return fail("invalid argument");
+  CK(cudaSetDevice(t->device));
   SdbTvState s;
-  TCK(cudaMemcpy(&s, t->d_state + which, sizeof(s), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(&s, t->d_state + which, sizeof(s), cudaMemcpyDeviceToHost));
   if (line_len) *line_len = s.est_line_len;
   if (hsync_len) *hsync_len = s.est_hsync_len;
   if (gain) *gain = s.agc_gain;
@@ -236,20 +224,19 @@ extern "C" int sdb_tv_processor_estimates(sdb_tv_processor_t *t, uint32_t which,
 
 extern "C" int sdb_tv_feed_transform(const sdb_complex *x, size_t n, int mode, float k, float dc, float *out)
 {
-  if (!x || !out) return sdb_set_error("null argument");
-  if (mode != 0 && mode != 1) return sdb_set_error("mode: 0 modulus, 1 argument");
-  if (sdb_device_count() <= 0) return sdb_set_error("no CUDA device: sigdigger_b200 has no CPU fallback");
+  if (!x || !out) return fail("null argument");
+  if (mode != 0 && mode != 1) return fail("mode: 0 modulus, 1 argument");
+  if (sdb_device_count() <= 0) return fail("no CUDA device: sigdigger_b200 has no CPU fallback");
   if (n == 0) return 0;
-  float2 *dx = nullptr; float *dout = nullptr;
-  TCK(cudaMalloc(&dx, n * sizeof(float2)));
-  if (cudaMalloc(&dout, n * sizeof(float)) != cudaSuccess) { cudaFree(dx); return sdb_set_error("out of device memory"); }
+  DevBuf<float2> dx; DevBuf<float> dout;
+  CK(dx.alloc(n));
+  if (dout.alloc(n) != cudaSuccess) return fail("out of device memory");
   cudaError_t e = cudaMemcpy(dx, x, n * sizeof(float2), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) {
     k_tv_feed_transform<<<(unsigned) ((n + 255) / 256), 256>>>(dx, n, mode, k, dc, dout);
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaMemcpy(out, dout, n * sizeof(float), cudaMemcpyDeviceToHost);
-  cudaFree(dx); cudaFree(dout);
-  if (e != cudaSuccess) return sdb_set_error(cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(cudaGetErrorString(e));
   return 0;
 }
