@@ -16,6 +16,7 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 #include <cstdio>
@@ -42,22 +43,31 @@ struct Channel {
   int spect_kind = 0; unsigned spect_size = 0, est_mask = 0;   // SPEC U
 };
 
-struct TimedSpan { int family; cudaEvent_t a, b; };
+struct TimedSpan { int family; Event a, b; };
 enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
                                             "inspector" };
 
-struct sdb_engine {
-  sdb_engine_params prm;
-  double samp_rate;
-  cudaStream_t stream = nullptr;
-  uint64_t launches = 0;
-  bool committed = false, first_feed = true, timing = false, chains_fresh = true;
-  std::vector<Channel> channels;
-  std::map<unsigned, float2 *> tw;     // twiddle tables by size
-  std::vector<DevBuf<unsigned char>> allocs;   // every device buffer of the engine (dalloc), freed with it
+struct ChdetDeleter { void operator()(sdb_chdet *d) const { sdb_chdet_destroy(d); } };
 
-  unsigned Np = 0, W = 0;               // PSD size, channeliser window
+// Host-buffer pipeline: results are double-buffered by feed parity so that the D2H reads of feed i-1 overlap the
+// kernels of feed i (three copy/compute streams).  Each event guards its slot's buffers between the streams.
+struct Slot {
+  float *psd = nullptr;                             // [S][frames][Np]
+  // channel streams: the (latency-bound, 1-CTA-per-32-chains) inspector kernel of feed i runs on its own stream
+  // while the FFT kernels of feed i+1 fill the other slot
+  float2 *chan = nullptr;
+  float2 *soft = nullptr; uint8_t *hard = nullptr; uint32_t *counts = nullptr;
+  DevBuf<unsigned long long> sym_off;               // packed read-out: start of every chain, 16-symbol aligned
+  Event psd_ready, psd_read, sym_read, insp;
+};
+
+// Everything sdb_engine_commit builds, and the running state that exists only after a commit.  A commit builds it
+// whole and hands it to the engine only on success, so a failed commit leaves nothing behind.
+struct Plan {
+  std::vector<DevBuf<unsigned char>> allocs;   // every device buffer of the plan (dalloc), freed with it
+  std::map<unsigned, float2 *> tw;     // twiddle tables by size
+
   SdbFourStep fs_psd{}, fs_st{};       // transform plans (make_plan)
   float *d_window = nullptr;
   // four-step scratch of the two-kernel transforms (the F.5 and Stockham paths)
@@ -65,62 +75,47 @@ struct sdb_engine {
   // Two-kernel sizes with Np == W: the PSD transforms run on their own stream, concurrently with the channeliser
   // transforms of the same group of streams (feed_device): the two kernel chains fill each other's launch gaps
   // and partial waves, and both read the same input region while it is still in L2.
-  cudaStream_t psd_stream = nullptr; cudaEvent_t ev_feed = nullptr;
-  float2 *d_xin = nullptr;              // staging for host feeds
+  Stream psd_stream; Event ev_feed;
   float2 *d_hist = nullptr;             // [S][W/2]
-  float *d_psd = nullptr; size_t max_frames = 0, last_frames = 0;
   // channeliser
   int *d_binmap = nullptr; int n_bins = 0; unsigned ka_mask = 0;
-  float2 *d_cspec = nullptr; size_t max_hops = 0;
+  float2 *d_cspec = nullptr;
   std::vector<SdbChannelDev> h_chans; SdbChannelDev *d_chans = nullptr;
   struct Group { int size; int len; int *d_ids; int any_precise; };
   std::vector<Group> groups;
   float2 *d_tails = nullptr; size_t tail_stride = 0;
   float *d_lo_phase = nullptr;
-  // channel streams are double-buffered: the (latency-bound, 1-CTA-per-32-chains) inspector kernel of feed i
-  // runs on its own stream while the FFT kernels of feed i+1 fill the other buffer
-  float2 *d_chanb[2] = { nullptr, nullptr }; size_t chan_stride = 0;
-  cudaStream_t insp_stream = nullptr;
-  cudaEvent_t ev_chan[2] = { nullptr, nullptr }, ev_insp[2] = { nullptr, nullptr };
-  bool ev_insp_valid[2] = { false, false };
-  unsigned feed_index = 0; int last_buf = 0;
-  uint64_t n_fed = 0; std::vector<float2> last_x_tail;
-  // DC removal (SDB_FLAG_DC_REMOVE, SPEC R): per-stream estimate, the estimate the current block is corrected with,
-  // run sums, and the corrected float32 copy of the block the rest of the path reads
-  float2 *d_dc_state = nullptr, *d_dc_cur = nullptr, *d_xdc = nullptr; double2 *d_dc_part = nullptr;   // samples fed so far; (engines without channels keep no history)
-  // Host-buffer pipeline: results and input staging are double-buffered by feed parity so that the H2D
-  // copy of feed i+1 and the D2H reads of feed i-1 overlap the kernels of feed i (three copy/compute
-  // streams).  d_psd / d_soft / d_hard / d_counts always point at the buffers of the latest feed.
-  float *d_psdb[2] = { nullptr, nullptr };
-  float2 *d_softb[2] = { nullptr, nullptr }; uint8_t *d_hardb[2] = { nullptr, nullptr };
-  uint32_t *d_countsb[2] = { nullptr, nullptr };
-  unsigned long long *d_sym_off[2] = { nullptr, nullptr };   // packed read-out: start of every chain, 16-symbol aligned
-  float2 *d_xinb[2] = { nullptr, nullptr };
-  cudaStream_t h2d_stream = nullptr, d2h_stream = nullptr;
-  cudaEvent_t ev_psd_ready[2] = { nullptr, nullptr }, ev_psd_read[2] = { nullptr, nullptr },
-              ev_sym_read[2] = { nullptr, nullptr }, ev_h2d[2] = { nullptr, nullptr }, ev_xfree[2] = { nullptr, nullptr };
-  bool psd_read_valid[2] = { false, false }, sym_read_valid[2] = { false, false }, xfree_valid[2] = { false, false };
-  unsigned host_feeds = 0;
-  size_t last_hops = 0;
+  size_t chan_stride = 0;
+  Stream insp_stream; Event ev_chan;
+  Slot slot[2];
+  // Host-input staging has its own parity, host_feeds: device feeds between host feeds make it differ from the feed
+  // parity.  The H2D copy of feed i+1 overlaps the kernels of feed i.
+  struct Stage { DevBuf<float2> xin; Event xfree; } stage[2];
+  Stream h2d_stream, d2h_stream; Event ev_h2d;
   // chains
   SdbChainCfg *d_cfg = nullptr; std::vector<SdbChainCfg> h_cfg;
   SdbChainState *d_state = nullptr;
   float *d_pool = nullptr; size_t pool_stride = 0;
   int *d_chain_map = nullptr; int insp_ctas = 0; std::vector<int> h_chain_map;
   float *d_taps = nullptr;
-  float2 *d_soft = nullptr; uint8_t *d_hard = nullptr; uint32_t *d_counts = nullptr; size_t sym_cap = 0;
+  size_t sym_cap = 0;
   // channel detector on the main PSD (SPEC K; chdet_kernels.cu)
-  struct sdb_chdet *chdet = nullptr; bool cd_enabled = false;
-  float cd_alpha = 0, cd_gamma = 0, cd_snr = 0; unsigned cd_min_bins = 1;
+  std::unique_ptr<sdb_chdet, ChdetDeleter> chdet;
   // inspector spectrum sources / estimators (SPEC U)
-  std::map<unsigned, float *> bh_windows;
   std::vector<SdbSpectCfg> h_spect; SdbSpectCfg *d_spectcfg = nullptr;
   float *d_spect = nullptr; size_t spect_stride = 0; int spect_max_ns = 0;
   uint32_t *d_spect_size = nullptr; float *d_est = nullptr; int *d_est_valid = nullptr;
-  // timing
-  std::vector<TimedSpan> spans;
-  double fam_ms[FAM_COUNT] = {0}; uint64_t fam_n[FAM_COUNT] = {0};
+  // DC removal (SDB_FLAG_DC_REMOVE, SPEC R): per-stream estimate, the estimate the current block is corrected with,
+  // run sums, and the corrected float32 copy of the block the rest of the path reads
+  float2 *d_dc_state = nullptr, *d_dc_cur = nullptr, *d_xdc = nullptr; double2 *d_dc_part = nullptr;
+  // running state
+  unsigned feed_index = 0, host_feeds = 0;
+  bool first_feed = true;               // (engines without channels keep no history)
+  uint64_t n_fed = 0;                   // samples fed so far
+  size_t last_frames = 0, last_hops = 0;
 
+  // the slot of the latest feed (slot 0 before the first)
+  Slot &cur() { return slot[feed_index ? (feed_index - 1) & 1u : 0]; }
   template <typename T> T *dalloc(size_t n)
   {
     DevBuf<unsigned char> b;
@@ -140,33 +135,44 @@ struct sdb_engine {
     tw[n] = d;
     return d;
   }
+};
+
+struct sdb_engine {
+  sdb_engine_params prm;
+  double samp_rate;
+  Stream stream;
+  uint64_t launches = 0;
+  bool timing = false;
+  std::vector<Channel> channels;
+  unsigned Np = 0, W = 0;               // PSD size, channeliser window
+  // channel detector parameters
+  bool cd_enabled = false;
+  float cd_alpha = 0, cd_gamma = 0, cd_snr = 0; unsigned cd_min_bins = 1;
+  std::unique_ptr<Plan> plan;           // set by a successful sdb_engine_commit
+  // timing
+  std::vector<TimedSpan> spans;
+  double fam_ms[FAM_COUNT] = {0}; uint64_t fam_n[FAM_COUNT] = {0};
+
   void span_begin(int fam, cudaStream_t on = nullptr)
   {
     if (!timing) return;
     TimedSpan s; s.family = fam;
-    cudaEventCreate(&s.a); cudaEventCreate(&s.b);
-    cudaEventRecord(s.a, on ? on : stream);
-    spans.push_back(s);
+    s.a.create(cudaEventDefault); s.b.create(cudaEventDefault);
+    s.a.record(on ? on : stream.get());
+    spans.push_back(std::move(s));
   }
   void span_end(cudaStream_t on = nullptr)
   {
     if (!timing) return;
-    cudaEventRecord(spans.back().b, on ? on : stream);
+    spans.back().b.record(on ? on : stream.get());
   }
   // make the main stream wait for everything queued on the inspector stream
-  cudaError_t join()
-  {
-    if (!insp_stream) return cudaSuccess;
-    const int b = last_buf;
-    if (ev_insp_valid[b]) return cudaStreamWaitEvent(stream, ev_insp[b], 0);
-    return cudaSuccess;
-  }
+  cudaError_t join() { return plan ? plan->cur().insp.wait_on(stream) : cudaSuccess; }
   void collect_spans()
   {
     for (auto &s : spans) {
       float ms = 0;
       if (cudaEventElapsedTime(&ms, s.a, s.b) == cudaSuccess) { fam_ms[s.family] += ms; fam_n[s.family]++; }
-      cudaEventDestroy(s.a); cudaEventDestroy(s.b);
     }
     spans.clear();
   }
@@ -174,13 +180,13 @@ struct sdb_engine {
 
 // The transform plan of an N-point window for the main PSD (psd = true) or the channeliser: which kernels run
 // (SdbFftPath), the split N = N1 x N2 and the tables.  This is the one place that ties transform sizes to kernels.
-static bool make_plan(sdb_engine *e, unsigned N, bool psd, SdbFourStep *fs)
+static bool make_plan(Plan &pl, unsigned N, bool psd, SdbFourStep *fs)
 {
   *fs = SdbFourStep{};
   fs->N = (int) N;
   if (psd && N <= 4096) {
     fs->path = SDB_FFT_SMALL_PSD;
-    fs->twN = e->twiddle(N);
+    fs->twN = pl.twiddle(N);
     return fs->twN != nullptr;
   }
   fs->path = N == 65536 ? SDB_FFT_CLUSTER
@@ -189,14 +195,14 @@ static bool make_plan(sdb_engine *e, unsigned N, bool psd, SdbFourStep *fs)
   fs->N1 = 1 << (fs->path == SDB_FFT_STOCKHAM ? l / 2 : l - 8);   // cluster and F.5: N1 x 256
   fs->N2 = (int) N / fs->N1;
   fs->ka_shift = ilog2u(fs->N1);
-  fs->twN1 = e->twiddle(fs->N1); fs->twN2 = e->twiddle(fs->N2); fs->twN = e->twiddle(N);
+  fs->twN1 = pl.twiddle(fs->N1); fs->twN2 = pl.twiddle(fs->N2); fs->twN = pl.twiddle(N);
   if (!(fs->twN1 && fs->twN2 && fs->twN)) return false;
   if (fs->path == SDB_FFT_STOCKHAM) return true;
   // SPEC F.4 / F.5 inter-pass twiddle [k1][n2] = W_N1^(p >> 8) x W_N^(p & 255), p = n2 k1: the product of two table
   // look-ups, tabulated once with the arithmetic of SPEC F.1 (one rounded product + one fused multiply-add per
   // component)
-  auto it = e->tw.find(N | 1u);
-  if (it != e->tw.end()) { fs->twPQ = it->second; return true; }
+  auto it = pl.tw.find(N | 1u);
+  if (it != pl.tw.end()) { fs->twPQ = it->second; return true; }
   const unsigned N1 = (unsigned) fs->N1;
   std::vector<float2> c, f, pq((size_t) N);
   sdbh::twiddle_fill(N1, c); sdbh::twiddle_fill(N, f);
@@ -207,10 +213,10 @@ static bool make_plan(sdb_engine *e, unsigned N, bool psd, SdbFourStep *fs)
       pq[(size_t) k1 * 256 + n2].x = fmaf(a.x, b.x, -(a.y * b.y));
       pq[(size_t) k1 * 256 + n2].y = fmaf(a.x, b.y, a.y * b.x);
     }
-  float2 *d = e->dalloc<float2>(N);
+  float2 *d = pl.dalloc<float2>(N);
   if (!d) return false;
   cudaMemcpy(d, pq.data(), (size_t) N * sizeof(float2), cudaMemcpyHostToDevice);
-  e->tw[N | 1u] = d;
+  pl.tw[N | 1u] = d;
   fs->twPQ = d;
   return true;
 }
@@ -253,7 +259,7 @@ extern "C" sdb_engine_t *sdb_engine_new(const sdb_engine_params *p, double samp_
   CKP(cudaSetDevice(p->device));
   sdb_engine *e = new sdb_engine();
   e->prm = *p; e->samp_rate = samp_rate; e->Np = p->psd_size; e->W = W;
-  if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) {
+  if (e->stream.create(cudaStreamNonBlocking) != cudaSuccess) {
     g_err = "cudaStreamCreate failed"; delete e; return nullptr;
   }
   return e;
@@ -264,23 +270,12 @@ extern "C" void sdb_engine_destroy(sdb_engine_t *e)
   if (!e) return;
   cudaSetDevice(e->prm.device);
   cudaStreamSynchronize(e->stream);
-  if (e->insp_stream) cudaStreamSynchronize(e->insp_stream);
-  e->collect_spans();
-  if (e->l2_pinned_bytes) { cudaCtxResetPersistingL2Cache(); cudaGetLastError(); }
-  if (e->chdet) sdb_chdet_destroy(e->chdet);
-  for (int i = 0; i < 2; ++i) {
-    if (e->ev_chan[i]) cudaEventDestroy(e->ev_chan[i]);
-    if (e->ev_insp[i]) cudaEventDestroy(e->ev_insp[i]);
+  if (Plan *p = e->plan.get()) {
+    for (cudaStream_t s : { p->insp_stream.get(), p->psd_stream.get(), p->h2d_stream.get(), p->d2h_stream.get() })
+      if (s) cudaStreamSynchronize(s);
+    if (p->l2_pinned_bytes) { cudaCtxResetPersistingL2Cache(); cudaGetLastError(); }
   }
-  if (e->insp_stream) cudaStreamDestroy(e->insp_stream);
-  if (e->psd_stream) { cudaStreamSynchronize(e->psd_stream); cudaStreamDestroy(e->psd_stream); }
-  if (e->ev_feed) cudaEventDestroy(e->ev_feed);
-  if (e->h2d_stream) { cudaStreamSynchronize(e->h2d_stream); cudaStreamDestroy(e->h2d_stream); }
-  if (e->d2h_stream) { cudaStreamSynchronize(e->d2h_stream); cudaStreamDestroy(e->d2h_stream); }
-  for (int i = 0; i < 2; ++i)
-    for (cudaEvent_t ev : { e->ev_psd_ready[i], e->ev_psd_read[i], e->ev_sym_read[i], e->ev_h2d[i], e->ev_xfree[i] })
-      if (ev) cudaEventDestroy(ev);
-  cudaStreamDestroy(e->stream);
+  e->collect_spans();
   delete e;
 }
 
@@ -304,7 +299,7 @@ extern "C" int sdb_inspector_config_default(sdb_inspector_config *c, int insp_cl
 extern "C" int sdb_engine_open_channel(sdb_engine_t *e, const sdb_channel_params *p, sdb_channel_info *info)
 {
   if (!e || !p) return fail("null argument");
-  if (e->committed) return fail("engine already committed");
+  if (e->plan) return fail("engine already committed");
   if (!(p->guard >= 1.0f) || !(p->bw > 0.0f) || p->bw > 6.28318530717958647692f * 1.0001f)
     return fail("invalid channel: guard >= 1 and 0 < bw <= 2 pi required");   // INVALID_CHANNEL
   if (!(p->f0 >= 0.0f) || p->f0 >= 6.28318530717958647692f) return fail("invalid channel: f0 must be in [0, 2 pi)");
@@ -339,7 +334,7 @@ extern "C" int sdb_engine_set_inspector(sdb_engine_t *e, int handle, const sdb_i
 {
   if (!e || !cfg) return fail("null argument");
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");   // WRONG_HANDLE
-  if (e->committed) return fail("engine already committed");
+  if (e->plan) return fail("engine already committed");
   if (cfg->insp_class < SDB_INSP_PSK || cfg->insp_class > SDB_INSP_RAW) return fail("wrong kind");
   Channel &c = e->channels[handle];
   c.cfg = *cfg; c.has_insp = true;
@@ -352,7 +347,7 @@ extern "C" int sdb_engine_set_channel_detector(sdb_engine_t *e, float alpha, flo
 {
   (void) beta;
   if (!e) return fail("null argument");
-  if (e->committed) return fail("engine already committed");
+  if (e->plan) return fail("engine already committed");
   if (!e->prm.psd_size) return fail("the channel detector needs the main PSD");
   if (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) return fail("the channel detector needs a linear PSD");
   if (!(snr > 0.0f) || !(alpha >= 0.0f && alpha <= 1.0f) || !(gamma >= 0.0f && gamma <= 1.0f))
@@ -365,12 +360,13 @@ extern "C" long sdb_engine_read_channels(sdb_engine_t *e, uint32_t stream, doubl
                                          sdb_detected_channel *out, size_t cap, uint32_t *total)
 {
   if (!e) return fail("null argument");
-  if (!e->committed || !e->chdet) return fail("channel detector not enabled");
+  if (!e->plan || !e->plan->chdet) return fail("channel detector not enabled");
+  const Plan &p = *e->plan;
   if (stream >= e->prm.n_streams) return fail("stream out of range");
   CK(cudaSetDevice(e->prm.device));
-  CK(cudaStreamSynchronize(e->psd_stream ? e->psd_stream : e->stream));
+  CK(cudaStreamSynchronize(p.psd_stream ? p.psd_stream.get() : e->stream.get()));
   CK(cudaStreamSynchronize(e->stream));
-  const long n = sdb_chdet_read(e->chdet, stream, e->samp_rate, center_freq, out, cap, total);
+  const long n = sdb_chdet_read(p.chdet.get(), stream, e->samp_rate, center_freq, out, cap, total);
   if (n < 0) return fail("channel read failed");
   return n;
 }
@@ -380,11 +376,12 @@ extern "C" int sdb_engine_read_all_channels(sdb_engine_t *e, const double *cente
                                             uint32_t *counts)
 {
   if (!e || !centers || !out || !counts) return fail("null argument");
-  if (!e->committed || !e->chdet) return fail("channel detector not enabled");
+  if (!e->plan || !e->plan->chdet) return fail("channel detector not enabled");
+  const Plan &p = *e->plan;
   CK(cudaSetDevice(e->prm.device));
-  CK(cudaStreamSynchronize(e->psd_stream ? e->psd_stream : e->stream));
+  CK(cudaStreamSynchronize(p.psd_stream ? p.psd_stream.get() : e->stream.get()));
   CK(cudaStreamSynchronize(e->stream));
-  if (sdb_chdet_read_all(e->chdet, e->samp_rate, centers, out, cap, counts)) return fail("channel read failed");
+  if (sdb_chdet_read_all(p.chdet.get(), e->samp_rate, centers, out, cap, counts)) return fail("channel read failed");
   return 0;
 }
 
@@ -398,7 +395,7 @@ extern "C" int sdb_engine_set_spectrum_source(sdb_engine_t *e, int handle, int s
 {
   if (!e) return fail("null argument");
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
-  if (e->committed) return fail("engine already committed");
+  if (e->plan) return fail("engine already committed");
   if (spectsrc_id < 0 || spectsrc_id >= SDB_SPECTSRC_COUNT) return fail("unknown spectrum source");
   if (!is_pow2(size) || size < 64 || size > 4096) return fail("spectrum size must be a power of two in [64, 4096]");
   Channel &c = e->channels[handle];
@@ -411,7 +408,7 @@ extern "C" int sdb_engine_set_estimator(sdb_engine_t *e, int handle, int estimat
 {
   if (!e) return fail("null argument");
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
-  if (e->committed) return fail("engine already committed");
+  if (e->plan) return fail("engine already committed");
   if (estimator_id < 0 || estimator_id >= SDB_ESTIMATOR_COUNT) return fail("unknown estimator");
   Channel &c = e->channels[handle];
   if (enabled) c.est_mask |= 1u << estimator_id; else c.est_mask &= ~(1u << estimator_id);
@@ -421,16 +418,17 @@ extern "C" int sdb_engine_set_estimator(sdb_engine_t *e, int handle, int estimat
 extern "C" int sdb_engine_read_spectrum(sdb_engine_t *e, int handle, float *out, uint32_t *sizes)
 {
   if (!e || !out || !sizes) return fail("null argument");
-  if (!e->committed) return fail("engine not committed");
+  if (!e->plan) return fail("engine not committed");
+  const Plan &p = *e->plan;
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
-  if (!e->d_spect || e->h_spect[handle].kind == 0) return fail("no spectrum source on this channel");
+  if (!p.d_spect || p.h_spect[handle].kind == 0) return fail("no spectrum source on this channel");
   CK(cudaSetDevice(e->prm.device));
-  CK(cudaStreamSynchronize(e->insp_stream));
+  CK(cudaStreamSynchronize(p.insp_stream));
   const unsigned S = e->prm.n_streams; const int K = (int) e->channels.size();
-  const SdbSpectCfg &q = e->h_spect[handle];
-  CK(cudaMemcpy2D(out, (size_t) q.ns * sizeof(float), e->d_spect + q.out_off, e->spect_stride * sizeof(float),
+  const SdbSpectCfg &q = p.h_spect[handle];
+  CK(cudaMemcpy2D(out, (size_t) q.ns * sizeof(float), p.d_spect + q.out_off, p.spect_stride * sizeof(float),
                   (size_t) q.ns * sizeof(float), S, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy2D(sizes, sizeof(uint32_t), e->d_spect_size + handle, (size_t) K * sizeof(uint32_t), sizeof(uint32_t), S,
+  CK(cudaMemcpy2D(sizes, sizeof(uint32_t), p.d_spect_size + handle, (size_t) K * sizeof(uint32_t), sizeof(uint32_t), S,
                   cudaMemcpyDeviceToHost));
   return 0;
 }
@@ -438,16 +436,17 @@ extern "C" int sdb_engine_read_spectrum(sdb_engine_t *e, int handle, float *out,
 extern "C" int sdb_engine_read_estimate(sdb_engine_t *e, int handle, int estimator_id, float *values, int32_t *valid)
 {
   if (!e || !values || !valid) return fail("null argument");
-  if (!e->committed) return fail("engine not committed");
+  if (!e->plan) return fail("engine not committed");
+  const Plan &p = *e->plan;
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
   if (estimator_id < 0 || estimator_id >= SDB_ESTIMATOR_COUNT) return fail("unknown estimator");
-  if (!e->d_est || !(e->h_spect[handle].est_mask & (1u << estimator_id))) return fail("estimator not enabled on this channel");
+  if (!p.d_est || !(p.h_spect[handle].est_mask & (1u << estimator_id))) return fail("estimator not enabled on this channel");
   CK(cudaSetDevice(e->prm.device));
-  CK(cudaStreamSynchronize(e->insp_stream));
+  CK(cudaStreamSynchronize(p.insp_stream));
   const unsigned S = e->prm.n_streams; const int K = (int) e->channels.size();
   const size_t pitch = (size_t) K * 2 * sizeof(float), off = (size_t) handle * 2 + estimator_id;
-  CK(cudaMemcpy2D(values, sizeof(float), e->d_est + off, pitch, sizeof(float), S, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy2D(valid, sizeof(int32_t), e->d_est_valid + off, pitch, sizeof(int32_t), S, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy2D(values, sizeof(float), p.d_est + off, pitch, sizeof(float), S, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy2D(valid, sizeof(int32_t), p.d_est_valid + off, pitch, sizeof(int32_t), S, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -567,10 +566,37 @@ static SdbChainState chain_layout(SdbChainCfg &c)
   return s;
 }
 
+// Pin the four-step scratch in L2.  Without this the streamed input and output evict it between the two passes and
+// every window costs two extra HBM round trips.  Accesses of the transform streams inside the window are "persisting"
+// (a set-aside part of L2 that normal traffic cannot evict); the kernels additionally mark their one-shot outputs as
+// streaming (st.global.cs).  The set-aside is device-wide: only the F.5 plans claim it.
+static void pin_scratch(const sdb_engine *e, Plan &p, const SdbFourStep &big)
+{
+  int max_persist = 0, max_window = 0;
+  cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, e->prm.device);
+  cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, e->prm.device);
+  const size_t bytes = (size_t) p.chunk_windows * big.N * sizeof(float2);
+  if (max_persist > 0 && max_window > 0) {
+    const size_t set_aside = std::min(bytes, (size_t) max_persist);
+    if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, set_aside) == cudaSuccess) {
+      cudaStreamAttrValue av{};
+      av.accessPolicyWindow.base_ptr = p.d_scratch;
+      av.accessPolicyWindow.num_bytes = std::min(bytes, (size_t) max_window);
+      av.accessPolicyWindow.hitRatio = (float) std::min(1.0, (double) set_aside / (double) av.accessPolicyWindow.num_bytes);
+      av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+      av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
+      if (cudaStreamSetAttribute(e->stream, cudaStreamAttributeAccessPolicyWindow, &av) == cudaSuccess)
+        p.l2_pinned_bytes = set_aside;
+      if (p.psd_stream) cudaStreamSetAttribute(p.psd_stream, cudaStreamAttributeAccessPolicyWindow, &av);
+    }
+    cudaGetLastError();   // the pin is an optimisation: never fail the commit because of it
+  }
+}
+
 extern "C" int sdb_engine_commit(sdb_engine_t *e)
 {
   if (!e) return fail("null engine");
-  if (e->committed) return fail("already committed");
+  if (e->plan) return fail("already committed");
   CK(cudaSetDevice(e->prm.device));
   const unsigned S = e->prm.n_streams, W = e->W, Np = e->Np;
   const int K = (int) e->channels.size();
@@ -578,97 +604,71 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
   if (max_feed == 0) return fail("max_feed must be > 0");
   if (max_feed % (W / 2)) return fail("max_feed must be a multiple of st_window_size / 2");
   if (Np && max_feed % Np) return fail("max_feed must be a multiple of psd_size");
+  // built here and handed to the engine at the end: every early return frees what was built so far
+  auto plan = std::make_unique<Plan>();
+  Plan &p = *plan;
 
   // ---- PSD plan
   if (Np) {
     std::vector<float> w;
     if (e->prm.psd_window != SDB_WINDOW_NONE) {
       sdbh::window_fill(w, Np, e->prm.psd_window);
-      e->d_window = e->dalloc<float>(Np);
-      if (!e->d_window) return fail("out of device memory");
-      CK(cudaMemcpy(e->d_window, w.data(), Np * sizeof(float), cudaMemcpyHostToDevice));
+      p.d_window = p.dalloc<float>(Np);
+      if (!p.d_window) return fail("out of device memory");
+      CK(cudaMemcpy(p.d_window, w.data(), Np * sizeof(float), cudaMemcpyHostToDevice));
     }
-    if (!make_plan(e, Np, true, &e->fs_psd)) return fail("out of device memory");
-    e->max_frames = max_feed / Np;
-    for (int i = 0; i < 2; ++i) {
-      e->d_psdb[i] = e->dalloc<float>((size_t) S * e->max_frames * Np);
-      if (!e->d_psdb[i]) return fail("out of device memory (psd)");
+    if (!make_plan(p, Np, true, &p.fs_psd)) return fail("out of device memory");
+    const size_t max_frames = max_feed / Np;
+    for (Slot &sl : p.slot) {
+      sl.psd = p.dalloc<float>((size_t) S * max_frames * Np);
+      if (!sl.psd) return fail("out of device memory (psd)");
     }
-    e->d_psd = e->d_psdb[0];
     if (e->cd_enabled) {
-      e->chdet = sdb_chdet_new(e->prm.device, Np, S, e->cd_alpha, e->cd_gamma, e->cd_snr, e->cd_min_bins);
-      if (!e->chdet) return fail("out of device memory (channel detector)");
+      p.chdet.reset(sdb_chdet_new(e->prm.device, Np, S, e->cd_alpha, e->cd_gamma, e->cd_snr, e->cd_min_bins));
+      if (!p.chdet) return fail("out of device memory (channel detector)");
     }
   }
-  if (K > 0 && !make_plan(e, W, false, &e->fs_st)) return fail("out of device memory");
-  // ---- four-step scratch of the two-kernel paths: whole waves of both passes, pinned in L2.  The cluster path keeps
-  // its intermediate in the shared memory of a thread-block cluster and needs none.
-  {
-    const SdbFourStep *big = nullptr;
-    if (Np && uses_scratch(e->fs_psd)) big = &e->fs_psd;
-    if (K > 0 && uses_scratch(e->fs_st) && (!big || e->fs_st.N > big->N)) big = &e->fs_st;
-    if (big) {
-      e->chunk_windows = (int) scratch_chunk_windows(*big, e->prm.device);
-      e->d_scratch = e->dalloc<float2>((size_t) e->chunk_windows * big->N);
-      if (!e->d_scratch) return fail("out of device memory (scratch)");
-      if (Np && K > 0 && Np == W && uses_scratch(e->fs_psd)) {
-        CK(cudaStreamCreateWithFlags(&e->psd_stream, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&e->ev_feed, cudaEventDisableTiming));
-      }
-      // Pin the scratch in L2.  Without this the streamed input and output evict it between the two passes
-      // and every window costs two extra HBM round trips.  Accesses of the transform streams inside the window
-      // are "persisting" (a set-aside part of L2 that normal traffic cannot evict); the kernels additionally
-      // mark their one-shot outputs as streaming (st.global.cs).
-      if (big->path == SDB_FFT_F5) {   // the set-aside is device-wide: only the F.5 plans claim it
-        int max_persist = 0, max_window = 0;
-        cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, e->prm.device);
-        cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, e->prm.device);
-        const size_t bytes = (size_t) e->chunk_windows * big->N * sizeof(float2);
-        if (max_persist > 0 && max_window > 0) {
-          const size_t set_aside = std::min(bytes, (size_t) max_persist);
-          if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, set_aside) == cudaSuccess) {
-            cudaStreamAttrValue av{};
-            av.accessPolicyWindow.base_ptr = e->d_scratch;
-            av.accessPolicyWindow.num_bytes = std::min(bytes, (size_t) max_window);
-            av.accessPolicyWindow.hitRatio = (float) std::min(1.0, (double) set_aside / (double) av.accessPolicyWindow.num_bytes);
-            av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-            av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-            if (cudaStreamSetAttribute(e->stream, cudaStreamAttributeAccessPolicyWindow, &av) == cudaSuccess)
-              e->l2_pinned_bytes = set_aside;
-            if (e->psd_stream) cudaStreamSetAttribute(e->psd_stream, cudaStreamAttributeAccessPolicyWindow, &av);
-          }
-          cudaGetLastError();   // the pin is an optimisation: never fail the commit because of it
-        }
-      }
+  if (K > 0 && !make_plan(p, W, false, &p.fs_st)) return fail("out of device memory");
+  // ---- four-step scratch of the two-kernel paths: whole waves of both passes, pinned in L2 (pin_scratch).  The
+  // cluster path keeps its intermediate in the shared memory of a thread-block cluster and needs none.
+  const SdbFourStep *big = nullptr;
+  if (Np && uses_scratch(p.fs_psd)) big = &p.fs_psd;
+  if (K > 0 && uses_scratch(p.fs_st) && (!big || p.fs_st.N > big->N)) big = &p.fs_st;
+  if (big) {
+    p.chunk_windows = (int) scratch_chunk_windows(*big, e->prm.device);
+    p.d_scratch = p.dalloc<float2>((size_t) p.chunk_windows * big->N);
+    if (!p.d_scratch) return fail("out of device memory (scratch)");
+    if (Np && K > 0 && Np == W && uses_scratch(p.fs_psd)) {
+      CK(p.psd_stream.create(cudaStreamNonBlocking));
+      CK(p.ev_feed.create());
     }
   }
   // ---- channeliser plan
-  e->max_hops = max_feed / (W / 2);
+  const size_t max_hops = max_feed / (W / 2);
   if (K > 0) {
     std::vector<int> binmap(W, -1);
     std::vector<char> need(W, 0);
     for (auto &c : e->channels)
       for (unsigned i = 0; i < 2 * c.halfw; ++i) need[(c.center + W - c.halfw + i) % W] = 1;
     int nb = 0;
-    e->ka_mask = 0;
     // bin k = k1 + N1 (ka + 16 kb) on the cluster and F.5 paths; the Stockham passes ignore the mask
-    const int ka_shift = e->fs_st.ka_shift;
-    for (unsigned b = 0; b < W; ++b) if (need[b]) { binmap[b] = nb++; e->ka_mask |= 1u << ((b >> ka_shift) & 15u); }
-    e->n_bins = nb;
-    e->d_binmap = e->dalloc<int>(W);
-    if (!e->d_binmap) return fail("out of device memory");
-    CK(cudaMemcpy(e->d_binmap, binmap.data(), W * sizeof(int), cudaMemcpyHostToDevice));
-    e->d_cspec = e->dalloc<float2>((size_t) S * e->max_hops * nb);
-    e->d_hist = e->dalloc<float2>((size_t) S * (W / 2));
-    if (!e->d_cspec || !e->d_hist) return fail("out of device memory (cspec)");
-    CK(cudaMemset(e->d_hist, 0, (size_t) S * (W / 2) * sizeof(float2)));
+    const int ka_shift = p.fs_st.ka_shift;
+    for (unsigned b = 0; b < W; ++b) if (need[b]) { binmap[b] = nb++; p.ka_mask |= 1u << ((b >> ka_shift) & 15u); }
+    p.n_bins = nb;
+    p.d_binmap = p.dalloc<int>(W);
+    if (!p.d_binmap) return fail("out of device memory");
+    CK(cudaMemcpy(p.d_binmap, binmap.data(), W * sizeof(int), cudaMemcpyHostToDevice));
+    p.d_cspec = p.dalloc<float2>((size_t) S * max_hops * nb);
+    p.d_hist = p.dalloc<float2>((size_t) S * (W / 2));
+    if (!p.d_cspec || !p.d_hist) return fail("out of device memory (cspec)");
+    CK(cudaMemset(p.d_hist, 0, (size_t) S * (W / 2) * sizeof(float2)));
 
-    e->h_chans.resize(K);
+    p.h_chans.resize(K);
     size_t out_off = 0, tail_off = 0;
     std::map<int, std::vector<int>> by_size;
     for (int k = 0; k < K; ++k) {
       Channel &c = e->channels[k];
-      SdbChannelDev &d = e->h_chans[k];
+      SdbChannelDev &d = p.h_chans[k];
       memset(&d, 0, sizeof(d));
       d.center = (int) c.center; d.size = (int) c.size; d.log2size = ilog2u(c.size);
       d.halfw = (int) c.halfw; d.halfsz = (int) c.halfsz;
@@ -686,48 +686,45 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       std::vector<float> kh, xf;
       sdbh::channel_weights(W, c.halfw, kh);
       sdbh::xfade_fill(c.size, xf);
-      float *dkh = e->dalloc<float>(kh.size()), *dxf = e->dalloc<float>(xf.size());
+      float *dkh = p.dalloc<float>(kh.size()), *dxf = p.dalloc<float>(xf.size());
       if (!dkh || !dxf) return fail("out of device memory");
       CK(cudaMemcpy(dkh, kh.data(), kh.size() * sizeof(float), cudaMemcpyHostToDevice));
       CK(cudaMemcpy(dxf, xf.data(), xf.size() * sizeof(float), cudaMemcpyHostToDevice));
-      d.kh = dkh; d.xfade = dxf; d.tw = e->twiddle(c.size);
+      d.kh = dkh; d.xfade = dxf; d.tw = p.twiddle(c.size);
       if (!d.tw) return fail("out of device memory");
-      d.out_off = out_off; d.out_cap = e->max_hops * c.halfsz; out_off += d.out_cap;
+      d.out_off = out_off; d.out_cap = max_hops * c.halfsz; out_off += d.out_cap;
       d.tail_off = tail_off; tail_off += c.halfsz;
       by_size[(int) c.size].push_back(k);
     }
-    e->chan_stride = out_off; e->tail_stride = tail_off;
-    e->d_chans = e->dalloc<SdbChannelDev>(K);
-    e->d_chanb[0] = e->dalloc<float2>((size_t) S * out_off);
-    e->d_chanb[1] = e->dalloc<float2>((size_t) S * out_off);
-    e->d_tails = e->dalloc<float2>((size_t) S * tail_off);
-    e->d_lo_phase = e->dalloc<float>((size_t) S * K);
-    if (!e->d_chans || !e->d_chanb[0] || !e->d_chanb[1] || !e->d_tails || !e->d_lo_phase)
+    p.chan_stride = out_off; p.tail_stride = tail_off;
+    p.d_chans = p.dalloc<SdbChannelDev>(K);
+    for (Slot &sl : p.slot) sl.chan = p.dalloc<float2>((size_t) S * out_off);
+    p.d_tails = p.dalloc<float2>((size_t) S * tail_off);
+    p.d_lo_phase = p.dalloc<float>((size_t) S * K);
+    if (!p.d_chans || !p.slot[0].chan || !p.slot[1].chan || !p.d_tails || !p.d_lo_phase)
       return fail("out of device memory (channels)");
     // The inspector kernel of feed i runs beside the transforms of feed i + 1.  Its CTAs are few and long-lived; the
     // highest priority places them as soon as SM space frees up instead of after every CTA of a transform grid
     // queued before them (the cluster path: one grid per feed) has been dispatched.
     int prio_least = 0, prio_greatest = 0;
     CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
-    CK(cudaStreamCreateWithPriority(&e->insp_stream, cudaStreamNonBlocking, prio_greatest));
-    for (int i = 0; i < 2; ++i) {
-      CK(cudaEventCreateWithFlags(&e->ev_chan[i], cudaEventDisableTiming));
-      CK(cudaEventCreateWithFlags(&e->ev_insp[i], cudaEventDisableTiming));
-    }
-    CK(cudaMemcpy(e->d_chans, e->h_chans.data(), K * sizeof(SdbChannelDev), cudaMemcpyHostToDevice));
-    CK(cudaMemset(e->d_tails, 0, (size_t) S * tail_off * sizeof(float2)));
-    CK(cudaMemset(e->d_lo_phase, 0, (size_t) S * K * sizeof(float)));
+    CK(p.insp_stream.create(cudaStreamNonBlocking, prio_greatest));
+    CK(p.ev_chan.create());
+    CK(cudaMemcpy(p.d_chans, p.h_chans.data(), K * sizeof(SdbChannelDev), cudaMemcpyHostToDevice));
+    CK(cudaMemset(p.d_tails, 0, (size_t) S * tail_off * sizeof(float2)));
+    CK(cudaMemset(p.d_lo_phase, 0, (size_t) S * K * sizeof(float)));
     for (auto &kv : by_size) {
-      sdb_engine::Group g; g.size = kv.first; g.len = (int) kv.second.size(); g.any_precise = 0;
-      for (int id : kv.second) if (e->h_chans[id].precise) g.any_precise = 1;
-      g.d_ids = e->dalloc<int>(kv.second.size());
+      Plan::Group g; g.size = kv.first; g.len = (int) kv.second.size(); g.any_precise = 0;
+      for (int id : kv.second) if (p.h_chans[id].precise) g.any_precise = 1;
+      g.d_ids = p.dalloc<int>(kv.second.size());
       if (!g.d_ids) return fail("out of device memory");
       CK(cudaMemcpy(g.d_ids, kv.second.data(), kv.second.size() * sizeof(int), cudaMemcpyHostToDevice));
-      e->groups.push_back(g);
+      p.groups.push_back(g);
     }
     // ---- inspector spectrum sources / estimators (SPEC U)
     {
       std::vector<SdbSpectCfg> sc(K);
+      std::map<unsigned, float *> bh_windows;   // Blackman-Harris windows by size
       size_t off = 0; int max_ns = 0; bool any = false;
       for (int k = 0; k < K; ++k) {
         const Channel &c = e->channels[k];
@@ -738,115 +735,110 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
         const unsigned ns = c.spect_size ? c.spect_size : 1024u;
         q.kind = c.spect_kind; q.ns = (int) ns; q.logns = ilog2u(ns); q.est_mask = c.est_mask;
         q.fs_ch = (float) (e->samp_rate * (double) c.size / (double) W);
-        q.tw = e->twiddle(ns);
+        q.tw = p.twiddle(ns);
         if (!q.tw) return fail("out of device memory");
-        auto it = e->bh_windows.find(ns);
-        if (it == e->bh_windows.end()) {
+        auto it = bh_windows.find(ns);
+        if (it == bh_windows.end()) {
           std::vector<float> w;
           sdbh::window_fill(w, ns, SDB_WINDOW_BLACKMANN_HARRIS);
-          float *d = e->dalloc<float>(ns);
+          float *d = p.dalloc<float>(ns);
           if (!d) return fail("out of device memory");
           CK(cudaMemcpy(d, w.data(), ns * sizeof(float), cudaMemcpyHostToDevice));
-          it = e->bh_windows.emplace(ns, d).first;
+          it = bh_windows.emplace(ns, d).first;
         }
         q.window = it->second;
         q.out_off = off; off += ns;
         max_ns = std::max(max_ns, (int) ns);
       }
       if (any) {
-        e->spect_stride = off; e->spect_max_ns = max_ns; e->h_spect = sc;
-        e->d_spectcfg = e->dalloc<SdbSpectCfg>(K);
-        e->d_spect = e->dalloc<float>((size_t) S * off);
-        e->d_spect_size = e->dalloc<uint32_t>((size_t) S * K);
-        e->d_est = e->dalloc<float>((size_t) S * K * 2);
-        e->d_est_valid = e->dalloc<int>((size_t) S * K * 2);
-        if (!e->d_spectcfg || !e->d_spect || !e->d_spect_size || !e->d_est || !e->d_est_valid)
+        p.spect_stride = off; p.spect_max_ns = max_ns; p.h_spect = sc;
+        p.d_spectcfg = p.dalloc<SdbSpectCfg>(K);
+        p.d_spect = p.dalloc<float>((size_t) S * off);
+        p.d_spect_size = p.dalloc<uint32_t>((size_t) S * K);
+        p.d_est = p.dalloc<float>((size_t) S * K * 2);
+        p.d_est_valid = p.dalloc<int>((size_t) S * K * 2);
+        if (!p.d_spectcfg || !p.d_spect || !p.d_spect_size || !p.d_est || !p.d_est_valid)
           return fail("out of device memory (spectrum sources)");
-        CK(cudaMemcpy(e->d_spectcfg, sc.data(), K * sizeof(SdbSpectCfg), cudaMemcpyHostToDevice));
-        CK(cudaMemset(e->d_spect_size, 0, (size_t) S * K * sizeof(uint32_t)));
-        CK(cudaMemset(e->d_est_valid, 0, (size_t) S * K * 2 * sizeof(int)));
+        CK(cudaMemcpy(p.d_spectcfg, sc.data(), K * sizeof(SdbSpectCfg), cudaMemcpyHostToDevice));
+        CK(cudaMemset(p.d_spect_size, 0, (size_t) S * K * sizeof(uint32_t)));
+        CK(cudaMemset(p.d_est_valid, 0, (size_t) S * K * 2 * sizeof(int)));
       }
     }
     // ---- chains
-    e->h_cfg.resize(K);
+    p.h_cfg.resize(K);
     std::vector<float> taps_pool;
     std::vector<SdbChainState> st0(K);
     size_t pool = 1, cap = 1;
     for (int k = 0; k < K; ++k) {
-      if (!build_chain_cfg(e->channels[k], e->h_cfg[k], taps_pool)) return fail("invalid inspector configuration");
-      SdbChainCfg &c = e->h_cfg[k];
+      if (!build_chain_cfg(e->channels[k], p.h_cfg[k], taps_pool)) return fail("invalid inspector configuration");
+      SdbChainCfg &c = p.h_cfg[k];
       st0[k] = chain_layout(c);
       pool = std::max<size_t>(pool, (size_t) c.st_pool);
-      cap = std::max<size_t>(cap, e->max_hops * e->channels[k].halfsz);
+      cap = std::max<size_t>(cap, max_hops * e->channels[k].halfsz);
     }
-    e->pool_stride = pool; e->sym_cap = cap;
+    p.pool_stride = pool; p.sym_cap = cap;
     const size_t chains = (size_t) S * K;
-    e->d_cfg = e->dalloc<SdbChainCfg>(K);
-    e->d_state = e->dalloc<SdbChainState>(chains);
-    e->insp_ctas = sdb_build_chain_map(e->h_cfg.data(), K, (int) S, e->h_chain_map);
-    e->d_chain_map = e->dalloc<int>(e->h_chain_map.size());
-    if (!e->d_chain_map) return fail("out of device memory (chain map)");
-    CK(cudaMemcpy(e->d_chain_map, e->h_chain_map.data(), e->h_chain_map.size() * sizeof(int), cudaMemcpyHostToDevice));
-    const size_t pool_floats = (size_t) e->insp_ctas * 32 * pool;   // per-CTA interleaved [slot][lane]
-    e->d_pool = e->dalloc<float>(pool_floats);
-    e->d_taps = e->dalloc<float>(taps_pool.size());
-    for (int i = 0; i < 2; ++i) {
-      e->d_softb[i] = e->dalloc<float2>(chains * cap);
-      e->d_hardb[i] = e->dalloc<uint8_t>(chains * cap);
-      e->d_countsb[i] = e->dalloc<uint32_t>(chains);
-      if (!e->d_softb[i] || !e->d_hardb[i] || !e->d_countsb[i]) return fail("out of device memory (symbols)");
-      CK(cudaMemset(e->d_countsb[i], 0, chains * sizeof(uint32_t)));
+    p.d_cfg = p.dalloc<SdbChainCfg>(K);
+    p.d_state = p.dalloc<SdbChainState>(chains);
+    p.insp_ctas = sdb_build_chain_map(p.h_cfg.data(), K, (int) S, p.h_chain_map);
+    p.d_chain_map = p.dalloc<int>(p.h_chain_map.size());
+    if (!p.d_chain_map) return fail("out of device memory (chain map)");
+    CK(cudaMemcpy(p.d_chain_map, p.h_chain_map.data(), p.h_chain_map.size() * sizeof(int), cudaMemcpyHostToDevice));
+    const size_t pool_floats = (size_t) p.insp_ctas * 32 * pool;   // per-CTA interleaved [slot][lane]
+    p.d_pool = p.dalloc<float>(pool_floats);
+    p.d_taps = p.dalloc<float>(taps_pool.size());
+    for (Slot &sl : p.slot) {
+      sl.soft = p.dalloc<float2>(chains * cap);
+      sl.hard = p.dalloc<uint8_t>(chains * cap);
+      sl.counts = p.dalloc<uint32_t>(chains);
+      if (!sl.soft || !sl.hard || !sl.counts) return fail("out of device memory (symbols)");
+      CK(cudaMemset(sl.counts, 0, chains * sizeof(uint32_t)));
     }
-    e->d_soft = e->d_softb[0]; e->d_hard = e->d_hardb[0]; e->d_counts = e->d_countsb[0];
-    if (!e->d_cfg || !e->d_state || !e->d_pool || !e->d_taps || !e->d_soft || !e->d_hard || !e->d_counts)
-      return fail("out of device memory (chains)");
-    CK(cudaMemcpy(e->d_cfg, e->h_cfg.data(), K * sizeof(SdbChainCfg), cudaMemcpyHostToDevice));
+    if (!p.d_cfg || !p.d_state || !p.d_pool || !p.d_taps) return fail("out of device memory (chains)");
+    CK(cudaMemcpy(p.d_cfg, p.h_cfg.data(), K * sizeof(SdbChainCfg), cudaMemcpyHostToDevice));
     if (!taps_pool.empty())
-      CK(cudaMemcpy(e->d_taps, taps_pool.data(), taps_pool.size() * sizeof(float), cudaMemcpyHostToDevice));
+      CK(cudaMemcpy(p.d_taps, taps_pool.data(), taps_pool.size() * sizeof(float), cudaMemcpyHostToDevice));
     std::vector<SdbChainState> st(chains);
     for (size_t ci = 0; ci < chains; ++ci) st[ci] = st0[ci % K];
-    CK(cudaMemcpy(e->d_state, st.data(), chains * sizeof(SdbChainState), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(p.d_state, st.data(), chains * sizeof(SdbChainState), cudaMemcpyHostToDevice));
     {
       // lines start empty: delay line and filter line 0, magnitude history at the -160 dB floor (SPEC A); the engine
       // never asks the kernel for a `fresh` start, so that a re-planned engine can take over running chains
       std::vector<float> hp(pool_floats, 0.0f);
-      for (size_t q = 0; q < e->h_chain_map.size(); ++q) {
-        const int g = e->h_chain_map[q];
+      for (size_t q = 0; q < p.h_chain_map.size(); ++q) {
+        const int g = p.h_chain_map[q];
         if (g < 0) continue;
-        const SdbChainCfg &c = e->h_cfg[g / (int) S];
+        const SdbChainCfg &c = p.h_cfg[g / (int) S];
         if (!c.have_agc) continue;
         float *base = hp.data() + (q / 32) * 32 * pool + (q % 32);
         for (unsigned i = 0; i < c.mh_size; ++i) base[(size_t) (c.st_mh_off + (int) i) * 32] = -160.0f;
       }
-      CK(cudaMemcpy(e->d_pool, hp.data(), pool_floats * sizeof(float), cudaMemcpyHostToDevice));
+      CK(cudaMemcpy(p.d_pool, hp.data(), pool_floats * sizeof(float), cudaMemcpyHostToDevice));
     }
-    e->chains_fresh = false;
-    CK(cudaMemset(e->d_counts, 0, chains * sizeof(uint32_t)));
   }
   if (e->prm.flags & SDB_FLAG_DC_REMOVE) {
-    e->d_dc_state = e->dalloc<float2>(S); e->d_dc_cur = e->dalloc<float2>(S);
-    e->d_dc_part = e->dalloc<double2>((size_t) S * ((max_feed + 255) / 256));
-    e->d_xdc = e->dalloc<float2>((size_t) S * max_feed);
-    if (!e->d_dc_state || !e->d_dc_cur || !e->d_dc_part || !e->d_xdc) return fail("out of device memory (DC removal)");
-    CK(cudaMemset(e->d_dc_state, 0, S * sizeof(float2)));
+    p.d_dc_state = p.dalloc<float2>(S); p.d_dc_cur = p.dalloc<float2>(S);
+    p.d_dc_part = p.dalloc<double2>((size_t) S * ((max_feed + 255) / 256));
+    p.d_xdc = p.dalloc<float2>((size_t) S * max_feed);
+    if (!p.d_dc_state || !p.d_dc_cur || !p.d_dc_part || !p.d_xdc) return fail("out of device memory (DC removal)");
+    CK(cudaMemset(p.d_dc_state, 0, S * sizeof(float2)));
   }
-  CK(cudaStreamCreateWithFlags(&e->h2d_stream, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&e->d2h_stream, cudaStreamNonBlocking));
-  for (int i = 0; i < 2; ++i) {
-    CK(cudaEventCreateWithFlags(&e->ev_psd_ready[i], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&e->ev_psd_read[i], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&e->ev_sym_read[i], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&e->ev_h2d[i], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&e->ev_xfree[i], cudaEventDisableTiming));
-  }
-  e->committed = true;
+  CK(p.h2d_stream.create(cudaStreamNonBlocking));
+  CK(p.d2h_stream.create(cudaStreamNonBlocking));
+  for (Slot &sl : p.slot)
+    for (Event *ev : { &sl.psd_ready, &sl.psd_read, &sl.sym_read, &sl.insp }) CK(ev->create());
+  for (Plan::Stage &sg : p.stage) CK(sg.xfree.create());
+  CK(p.ev_h2d.create());
+  if (big && big->path == SDB_FFT_F5) pin_scratch(e, p, *big);
+  e->plan = std::move(plan);
   return 0;
 }
 
 extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, size_t stride, size_t n)
 {
   if (!e || !xv) return fail("null argument");
-  if (!e->committed) return fail("engine not committed");
+  if (!e->plan) return fail("engine not committed");
+  Plan &p = *e->plan;
   const unsigned S = e->prm.n_streams, W = e->W, Np = e->Np;
   const int K = (int) e->channels.size();
   if (n == 0 || n > e->prm.max_feed) return fail("feed size out of range");
@@ -855,38 +847,36 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
   CK(cudaSetDevice(e->prm.device));
   const void *x = reinterpret_cast<const void *>(xv);
   int fmt = e->prm.input_format | ((e->prm.flags & SDB_FLAG_IQ_REVERSE) ? SDB_FMT_SWAP : 0);
-  if (e->d_xdc) {
+  if (p.d_xdc) {
     // SPEC R: the block is corrected with the estimate of the blocks before it; everything downstream reads the
     // corrected float32 copy (format conversion and I/Q swap happen in this pass)
     const float alpha = (float) (1.0 - exp(-(double) n / (e->samp_rate * 0.1)));
-    CK(sdb_launch_dc_remove(e->stream, x, fmt, stride, n, (int) S, alpha, e->d_dc_state, e->d_dc_cur, e->d_dc_part,
-                            e->d_xdc));
+    CK(sdb_launch_dc_remove(e->stream, x, fmt, stride, n, (int) S, alpha, p.d_dc_state, p.d_dc_cur, p.d_dc_part,
+                            p.d_xdc));
     e->launches += 3;
-    x = e->d_xdc; fmt = SDB_FMT_F32; stride = n;
+    x = p.d_xdc; fmt = SDB_FMT_F32; stride = n;
   }
-  const size_t bps = sdb_fmt_bytes(fmt);
   SdbLaunchCtx ctx{ e->stream, &e->launches };
   const int shift_db = (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) ? 1 : 0;
-  const int ob = (int) (e->feed_index & 1u);     // result buffers of this feed
+  Slot &sl = p.slot[p.feed_index & 1u];     // result buffers of this feed
 
   const int frames = Np ? (int) (n / Np) : 0;
   const int H = K ? (int) (n / (W / 2)) : 0;
-  const int first = (K && e->first_feed) ? 1 : 0;
+  const int first = (K && p.first_feed) ? 1 : 0;
   const int wps = K ? H - first : 0;
   // arguments of the two-kernel transforms: PSD frames (hop Np, no history) and channeliser windows (hop W / 2 over
   // the W / 2-sample history followed by x)
   SdbPassAArgs psd_a{}, chan_a{};
   psd_a.x = chan_a.x = x; psd_a.fmt = chan_a.fmt = fmt; psd_a.stream_stride = chan_a.stream_stride = stride;
-  psd_a.windows_per_stream = frames; psd_a.hop = (int) Np; psd_a.window = e->d_window;
-  chan_a.hist = e->d_hist; chan_a.hist_len = (int) (W / 2);
+  psd_a.windows_per_stream = frames; psd_a.hop = (int) Np; psd_a.window = p.d_window;
+  chan_a.hist = p.d_hist; chan_a.hist_len = (int) (W / 2);
   chan_a.windows_per_stream = wps; chan_a.first_window = first; chan_a.hop = (int) (W / 2);
   SdbPassBArgs psd_b{}, chan_b{};
   psd_b.shift_db = shift_db;
-  chan_b.binmap = e->d_binmap; chan_b.cspec = e->d_cspec; chan_b.n_bins = e->n_bins; chan_b.ka_mask = e->ka_mask;
+  chan_b.binmap = p.d_binmap; chan_b.cspec = p.d_cspec; chan_b.n_bins = p.n_bins; chan_b.ka_mask = p.ka_mask;
   if (Np) {
-    e->last_frames = frames;
-    e->d_psd = e->d_psdb[ob];
-    psd_b.psd = e->d_psd; psd_b.inv_n = 1.0f / (float) Np;
+    p.last_frames = frames;
+    psd_b.psd = sl.psd; psd_b.inv_n = 1.0f / (float) Np;
   }
   // windows [w0, w0 + cw) of the flattened [stream][window] order through scratch region `scr`; pass B is timed as
   // family `fam_b` (FAM_ROWS_PSD: PSD epilogue, FAM_ROWS_CHAN: channeliser scatter)
@@ -914,146 +904,133 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
   // that fits the pinned scratch is the fastest (cfg2, 2048 streams: 12 streams 64.7 GS/s, 9 streams -- whole waves
   // for either kernel alone -- 63.1, 8: 60.2, 6: 54.2; the two chains overlap, so wave quantisation of a single
   // launch does not matter).
-  const int G = e->psd_stream && wps > 0 ? std::min(e->chunk_windows / (frames + wps), (int) S) : 0;
+  const int G = p.psd_stream && wps > 0 ? std::min(p.chunk_windows / (frames + wps), (int) S) : 0;
   if (G >= 1) {
     // timing mode (sdb_engine_timing): every kernel on the main stream, so that the CUDA-event spans are the
     // kernels' own durations and not those of two chains sharing the SMs
-    SdbLaunchCtx pctx{ e->timing ? e->stream : e->psd_stream, &e->launches };
-    CK(cudaEventRecord(e->ev_feed, e->stream));              // the input is valid from here on
-    CK(cudaStreamWaitEvent(e->psd_stream, e->ev_feed, 0));
-    if (e->psd_read_valid[ob]) CK(cudaStreamWaitEvent(e->psd_stream, e->ev_psd_read[ob], 0));   // async read of feed i-2
-    float2 *scr_psd = e->d_scratch, *scr_ch = e->d_scratch + (size_t) G * frames * Np;
+    SdbLaunchCtx pctx{ e->timing ? e->stream.get() : p.psd_stream.get(), &e->launches };
+    CK(p.ev_feed.record(e->stream));              // the input is valid from here on
+    CK(p.ev_feed.wait_on(p.psd_stream));
+    CK(sl.psd_read.wait_on(p.psd_stream));        // async read of feed i-2
+    float2 *scr_psd = p.d_scratch, *scr_ch = p.d_scratch + (size_t) G * frames * Np;
     for (int s0 = 0; s0 < (int) S; s0 += G) {
       const int g = std::min(G, (int) S - s0);
-      if (chunk(pctx, e->fs_psd, psd_a, psd_b, FAM_ROWS_PSD, s0 * frames, g * frames, scr_psd)) return -1;
-      if (chunk(ctx, e->fs_st, chan_a, chan_b, FAM_ROWS_CHAN, s0 * wps, g * wps, scr_ch)) return -1;
+      if (chunk(pctx, p.fs_psd, psd_a, psd_b, FAM_ROWS_PSD, s0 * frames, g * frames, scr_psd)) return -1;
+      if (chunk(ctx, p.fs_st, chan_a, chan_b, FAM_ROWS_CHAN, s0 * wps, g * wps, scr_ch)) return -1;
     }
-    if (e->chdet) CK(sdb_chdet_feed_stream(e->chdet, e->d_psd, (uint32_t) frames, (size_t) frames * Np, e->psd_stream,
-                                           &e->launches));
-    CK(cudaEventRecord(e->ev_psd_ready[ob], e->psd_stream));
-    CK(cudaStreamWaitEvent(e->stream, e->ev_psd_ready[ob], 0));   // the main stream stays the engine's timeline
+    if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, p.psd_stream,
+                                          &e->launches));
+    CK(sl.psd_ready.record(p.psd_stream));
+    CK(sl.psd_ready.wait_on(e->stream));          // the main stream stays the engine's timeline
   } else {
-    if (Np && e->psd_read_valid[ob]) CK(cudaStreamWaitEvent(e->stream, e->ev_psd_read[ob], 0));   // async read of feed i-2
+    CK(sl.psd_read.wait_on(e->stream));           // async read of feed i-2
     // ---- cluster-path PSD frames and channeliser windows: one launch, both passes fused, ordered by stream
-    const bool fused_psd = Np && e->fs_psd.path == SDB_FFT_CLUSTER, fused_chan = K && e->fs_st.path == SDB_FFT_CLUSTER;
+    const bool fused_psd = Np && p.fs_psd.path == SDB_FFT_CLUSTER, fused_chan = K && p.fs_st.path == SDB_FFT_CLUSTER;
     if ((fused_psd && frames > 0) || (fused_chan && wps > 0)) {
-      const SdbFourStep &fs = fused_psd ? e->fs_psd : e->fs_st;
+      const SdbFourStep &fs = fused_psd ? p.fs_psd : p.fs_st;
       SdbFft65536Args f{};
       f.x = x; f.fmt = fmt; f.stream_stride = stride; f.n_streams = (int) S;
       f.n_psd = fused_psd ? frames : 0; f.n_chan = fused_chan ? wps : 0; f.first_chan = first;
-      f.window = e->d_window; f.psd = e->d_psd; f.inv_n = 1.0f / (float) fs.N; f.shift_db = shift_db;
-      f.hist = e->d_hist; f.binmap = e->d_binmap; f.cspec = e->d_cspec; f.n_bins = e->n_bins; f.ka_mask = e->ka_mask;
+      f.window = p.d_window; f.psd = sl.psd; f.inv_n = 1.0f / (float) fs.N; f.shift_db = shift_db;
+      f.hist = p.d_hist; f.binmap = p.d_binmap; f.cspec = p.d_cspec; f.n_bins = p.n_bins; f.ka_mask = p.ka_mask;
       e->span_begin(FAM_COLS);
       CK(sdb_launch_fft65536(ctx, fs, f));
       e->span_end();
     }
     // ---- main PSD
     if (Np) {
-      if (e->fs_psd.path == SDB_FFT_SMALL_PSD) {
+      if (p.fs_psd.path == SDB_FFT_SMALL_PSD) {
         e->span_begin(FAM_ROWS_PSD);
-        CK(sdb_launch_small_psd(ctx, (int) Np, e->fs_psd.twN, x, fmt, stride, frames, (int) S, e->d_window,
-                                e->d_psd, shift_db));
+        CK(sdb_launch_small_psd(ctx, (int) Np, p.fs_psd.twN, x, fmt, stride, frames, (int) S, p.d_window,
+                                sl.psd, shift_db));
         e->span_end();
       } else if (!fused_psd) {
         const int total = frames * (int) S;
-        for (int w0 = 0; w0 < total; w0 += e->chunk_windows)
-          if (chunk(ctx, e->fs_psd, psd_a, psd_b, FAM_ROWS_PSD, w0, std::min(e->chunk_windows, total - w0),
-                    e->d_scratch)) return -1;
+        for (int w0 = 0; w0 < total; w0 += p.chunk_windows)
+          if (chunk(ctx, p.fs_psd, psd_a, psd_b, FAM_ROWS_PSD, w0, std::min(p.chunk_windows, total - w0),
+                    p.d_scratch)) return -1;
       }
-      if (e->chdet) CK(sdb_chdet_feed_stream(e->chdet, e->d_psd, (uint32_t) frames, (size_t) frames * Np, e->stream,
-                                             &e->launches));
-      CK(cudaEventRecord(e->ev_psd_ready[ob], e->stream));
+      if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, e->stream,
+                                            &e->launches));
+      CK(sl.psd_ready.record(e->stream));
     }
     // ---- channeliser forward transforms
     if (K && wps > 0 && !fused_chan) {
       const int total = wps * (int) S;
-      for (int w0 = 0; w0 < total; w0 += e->chunk_windows)
-        if (chunk(ctx, e->fs_st, chan_a, chan_b, FAM_ROWS_CHAN, w0, std::min(e->chunk_windows, total - w0),
-                  e->d_scratch)) return -1;
+      for (int w0 = 0; w0 < total; w0 += p.chunk_windows)
+        if (chunk(ctx, p.fs_st, chan_a, chan_b, FAM_ROWS_CHAN, w0, std::min(p.chunk_windows, total - w0),
+                  p.d_scratch)) return -1;
     }
   }
   // ---- per-channel inverse transforms + inspectors
   if (K) {
-    e->last_hops = wps > 0 ? wps : 0;
+    p.last_hops = wps > 0 ? wps : 0;
     if (wps > 0) {
-      const int b = (int) (e->feed_index & 1u);
-      e->last_buf = b;
-      // buffer b was last read by the inspector launch of feed i-2
-      if (e->ev_insp_valid[b]) CK(cudaStreamWaitEvent(e->stream, e->ev_insp[b], 0));
+      CK(sl.insp.wait_on(e->stream));             // the slot was last read by the inspector launch of feed i-2
       e->span_begin(FAM_CHAN_IFFT);
-      for (auto &g : e->groups)
-        CK(sdb_launch_chan_ifft_group(ctx, e->d_chans, g.d_ids, g.len, g.size, K, (int) S, e->d_cspec,
-                                      e->n_bins, wps, e->d_tails, e->tail_stride, e->d_lo_phase, e->d_chanb[b],
-                                      e->chan_stride, g.any_precise));
+      for (auto &g : p.groups)
+        CK(sdb_launch_chan_ifft_group(ctx, p.d_chans, g.d_ids, g.len, g.size, K, (int) S, p.d_cspec,
+                                      p.n_bins, wps, p.d_tails, p.tail_stride, p.d_lo_phase, sl.chan,
+                                      p.chan_stride, g.any_precise));
       e->span_end();
-      CK(cudaEventRecord(e->ev_chan[b], e->stream));
-      CK(cudaStreamWaitEvent(e->insp_stream, e->ev_chan[b], 0));
-      e->d_soft = e->d_softb[b]; e->d_hard = e->d_hardb[b]; e->d_counts = e->d_countsb[b];
-      if (e->sym_read_valid[b]) CK(cudaStreamWaitEvent(e->insp_stream, e->ev_sym_read[b], 0));
-      SdbLaunchCtx ictx{ e->timing ? e->stream : e->insp_stream, &e->launches };
-      if (e->d_spectcfg)
-        CK(sdb_launch_spectsrc(ictx, e->d_spectcfg, e->d_chans, K, (int) S, e->spect_max_ns, e->d_chanb[b],
-                               e->chan_stride, (uint32_t) wps, e->d_spect, e->spect_stride, e->d_spect_size,
-                               e->d_est, e->d_est_valid));
+      CK(p.ev_chan.record(e->stream));
+      CK(p.ev_chan.wait_on(p.insp_stream));
+      CK(sl.sym_read.wait_on(p.insp_stream));
+      SdbLaunchCtx ictx{ e->timing ? e->stream.get() : p.insp_stream.get(), &e->launches };
+      if (p.d_spectcfg)
+        CK(sdb_launch_spectsrc(ictx, p.d_spectcfg, p.d_chans, K, (int) S, p.spect_max_ns, sl.chan,
+                               p.chan_stride, (uint32_t) wps, p.d_spect, p.spect_stride, p.d_spect_size,
+                               p.d_est, p.d_est_valid));
       e->span_begin(FAM_INSPECTOR, ictx.stream);
-      CK(sdb_launch_inspectors_n(ictx, e->d_cfg, K, (int) S, e->d_chain_map, e->insp_ctas, e->d_state, e->d_pool,
-                                 e->pool_stride, e->d_taps,
-                                 e->d_chans, e->d_chanb[b], e->chan_stride, (uint32_t) wps, e->d_soft, e->d_hard,
-                                 e->d_counts, e->sym_cap, e->chains_fresh ? 1 : 0,
-                                 sdb_insp_dyn(e->h_cfg.data(), K)));
-      e->chains_fresh = false;
+      CK(sdb_launch_inspectors_n(ictx, p.d_cfg, K, (int) S, p.d_chain_map, p.insp_ctas, p.d_state, p.d_pool,
+                                 p.pool_stride, p.d_taps,
+                                 p.d_chans, sl.chan, p.chan_stride, (uint32_t) wps, sl.soft, sl.hard,
+                                 sl.counts, p.sym_cap, 0, sdb_insp_dyn(p.h_cfg.data(), K)));
       e->span_end(ictx.stream);
-      CK(cudaEventRecord(e->ev_insp[b], ictx.stream));
-      e->ev_insp_valid[b] = true;
+      CK(sl.insp.record(ictx.stream));
     } else {
-      e->d_counts = e->d_countsb[ob];
-      e->last_buf = ob;
-      if (e->sym_read_valid[ob]) CK(cudaStreamWaitEvent(e->insp_stream, e->ev_sym_read[ob], 0));
-      CK(cudaMemsetAsync(e->d_counts, 0, (size_t) S * K * sizeof(uint32_t), e->insp_stream));
-      CK(cudaEventRecord(e->ev_insp[ob], e->insp_stream));
-      e->ev_insp_valid[ob] = true;
+      CK(sl.sym_read.wait_on(p.insp_stream));
+      CK(cudaMemsetAsync(sl.counts, 0, (size_t) S * K * sizeof(uint32_t), p.insp_stream));
+      CK(sl.insp.record(p.insp_stream));
     }
     // keep the last half window of every stream as history for the next feed
     if (fmt == SDB_FMT_F32)
-      CK(cudaMemcpy2DAsync(e->d_hist, (W / 2) * sizeof(float2), reinterpret_cast<const float2 *>(x) + (n - W / 2),
+      CK(cudaMemcpy2DAsync(p.d_hist, (W / 2) * sizeof(float2), reinterpret_cast<const float2 *>(x) + (n - W / 2),
                            stride * sizeof(float2), (W / 2) * sizeof(float2), S, cudaMemcpyDeviceToDevice, e->stream));
     else
-      CK(sdb_launch_hist_convert(e->stream, x, fmt, stride, n - W / 2, e->d_hist, (int) (W / 2), (int) S));
-    e->first_feed = false;
+      CK(sdb_launch_hist_convert(e->stream, x, fmt, stride, n - W / 2, p.d_hist, (int) (W / 2), (int) S));
+    p.first_feed = false;
   }
-  ++e->feed_index;
-  e->n_fed += n;
+  ++p.feed_index;
+  p.n_fed += n;
   return 0;
 }
 
 extern "C" int sdb_engine_feed_host(sdb_engine_t *e, const sdb_complex *x, size_t stride, size_t n)
 {
   if (!e || !x) return fail("null argument");
-  if (!e->committed) return fail("engine not committed");
+  if (!e->plan) return fail("engine not committed");
+  Plan &p = *e->plan;
   if (n == 0 || n > e->prm.max_feed) return fail("feed size out of range");
   CK(cudaSetDevice(e->prm.device));
   const unsigned S = e->prm.n_streams;
-  const int hb = (int) (e->host_feeds & 1u);
+  Plan::Stage &sg = p.stage[p.host_feeds & 1u];
   const size_t bps = sdb_fmt_bytes(e->prm.input_format);
-  if (!e->d_xinb[hb]) {
-    e->d_xinb[hb] = e->dalloc<float2>((size_t) S * e->prm.max_feed);
-    if (!e->d_xinb[hb]) return fail("out of device memory (input staging)");
-  }
-  // H2D on its own stream into staging buffer hb, as soon as the kernels of feed i-2 are done with it;
+  if (!sg.xin.size() && sg.xin.alloc((size_t) S * e->prm.max_feed) != cudaSuccess)
+    return fail("out of device memory (input staging)");
+  // H2D on its own stream into this staging buffer, as soon as the kernels of host feed i-2 are done with it;
   // the kernels of this feed wait for the copy.  Copies of consecutive feeds overlap compute.
-  if (e->xfree_valid[hb]) CK(cudaStreamWaitEvent(e->h2d_stream, e->ev_xfree[hb], 0));
+  CK(sg.xfree.wait_on(p.h2d_stream));
   if (stride == n)
-    CK(cudaMemcpyAsync(e->d_xinb[hb], x, (size_t) S * n * bps, cudaMemcpyHostToDevice, e->h2d_stream));
+    CK(cudaMemcpyAsync(sg.xin, x, (size_t) S * n * bps, cudaMemcpyHostToDevice, p.h2d_stream));
   else
-    CK(cudaMemcpy2DAsync(e->d_xinb[hb], n * bps, x, stride * bps, n * bps, S,
-                         cudaMemcpyHostToDevice, e->h2d_stream));
-  CK(cudaEventRecord(e->ev_h2d[hb], e->h2d_stream));
-  CK(cudaStreamWaitEvent(e->stream, e->ev_h2d[hb], 0));
-  int rc = sdb_engine_feed_device(e, reinterpret_cast<const sdb_complex *>(e->d_xinb[hb]), n, n);
+    CK(cudaMemcpy2DAsync(sg.xin, n * bps, x, stride * bps, n * bps, S, cudaMemcpyHostToDevice, p.h2d_stream));
+  CK(p.ev_h2d.record(p.h2d_stream));
+  CK(p.ev_h2d.wait_on(e->stream));
+  int rc = sdb_engine_feed_device(e, reinterpret_cast<const sdb_complex *>(sg.xin.get()), n, n);
   if (rc) return rc;
-  CK(cudaEventRecord(e->ev_xfree[hb], e->stream));
-  e->xfree_valid[hb] = true;
-  ++e->host_feeds;
+  CK(sg.xfree.record(e->stream));
+  ++p.host_feeds;
   return 0;
 }
 
@@ -1063,8 +1040,10 @@ extern "C" int sdb_engine_sync(sdb_engine_t *e)
   CK(cudaSetDevice(e->prm.device));
   CK(e->join());
   CK(cudaStreamSynchronize(e->stream));
-  if (e->d2h_stream) CK(cudaStreamSynchronize(e->d2h_stream));
-  if (e->h2d_stream) CK(cudaStreamSynchronize(e->h2d_stream));
+  if (e->plan) {
+    CK(cudaStreamSynchronize(e->plan->d2h_stream));
+    CK(cudaStreamSynchronize(e->plan->h2d_stream));
+  }
   e->collect_spans();
   return 0;
 }
@@ -1080,16 +1059,14 @@ extern "C" int sdb_engine_join(sdb_engine_t *e)
   return 0;
 }
 
-extern "C" size_t sdb_engine_psd_frames(const sdb_engine_t *e) { return e ? e->last_frames : 0; }
-extern "C" const float *sdb_engine_psd_device(const sdb_engine_t *e) { return e ? e->d_psd : nullptr; }
+extern "C" size_t sdb_engine_psd_frames(const sdb_engine_t *e) { return e && e->plan ? e->plan->last_frames : 0; }
+extern "C" const float *sdb_engine_psd_device(const sdb_engine_t *e) { return e && e->plan ? e->plan->cur().psd : nullptr; }
 
 extern "C" int sdb_engine_read_psd(sdb_engine_t *e, float *dst, size_t cap)
 {
   if (!e || !dst) return fail("null argument");
-  const size_t n = (size_t) e->prm.n_streams * e->last_frames * e->Np;
-  if (cap < n) return fail("destination too small");
   if (sdb_engine_read_psd_async(e, dst, cap)) return -1;
-  CK(cudaStreamSynchronize(e->d2h_stream));
+  CK(cudaStreamSynchronize(e->plan->d2h_stream));
   return 0;
 }
 
@@ -1100,15 +1077,15 @@ extern "C" int sdb_engine_read_psd(sdb_engine_t *e, float *dst, size_t cap)
 extern "C" int sdb_engine_read_psd_async(sdb_engine_t *e, float *dst, size_t cap)
 {
   if (!e || !dst) return fail("null argument");
-  if (!e->committed || !e->Np || e->feed_index == 0) return fail("no PSD available");
-  const size_t n = (size_t) e->prm.n_streams * e->last_frames * e->Np;
+  if (!e->plan || !e->Np || e->plan->feed_index == 0) return fail("no PSD available");
+  Plan &p = *e->plan;
+  const size_t n = (size_t) e->prm.n_streams * p.last_frames * e->Np;
   if (cap < n) return fail("destination too small");
-  const int ob = (int) ((e->feed_index - 1) & 1u);
+  Slot &sl = p.cur();
   CK(cudaSetDevice(e->prm.device));
-  CK(cudaStreamWaitEvent(e->d2h_stream, e->ev_psd_ready[ob], 0));
-  CK(cudaMemcpyAsync(dst, e->d_psdb[ob], n * sizeof(float), cudaMemcpyDeviceToHost, e->d2h_stream));
-  CK(cudaEventRecord(e->ev_psd_read[ob], e->d2h_stream));
-  e->psd_read_valid[ob] = true;
+  CK(sl.psd_ready.wait_on(p.d2h_stream));
+  CK(cudaMemcpyAsync(dst, sl.psd, n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
+  CK(sl.psd_read.record(p.d2h_stream));
   return 0;
 }
 
@@ -1117,11 +1094,13 @@ extern "C" long sdb_engine_read_channel(sdb_engine_t *e, uint32_t stream, int ha
   if (!e || !dst) return fail("null argument");
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
   if (stream >= e->prm.n_streams) return fail("stream out of range");
-  const SdbChannelDev &d = e->h_chans[handle];
-  size_t n = e->last_hops * (size_t) d.halfsz;
+  if (!e->plan) return fail("engine not committed");
+  Plan &p = *e->plan;
+  const SdbChannelDev &d = p.h_chans[handle];
+  size_t n = p.last_hops * (size_t) d.halfsz;
   if (n > cap) n = cap;
   CK(cudaSetDevice(e->prm.device));
-  CK(cudaMemcpyAsync(dst, e->d_chanb[e->last_buf] + (size_t) stream * e->chan_stride + d.out_off, n * sizeof(float2),
+  CK(cudaMemcpyAsync(dst, p.cur().chan + (size_t) stream * p.chan_stride + d.out_off, n * sizeof(float2),
                      cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return (long) n;
@@ -1134,16 +1113,19 @@ extern "C" long sdb_engine_read_symbols(sdb_engine_t *e, uint32_t stream, int ha
   const int K = (int) e->channels.size();
   if (handle < 0 || handle >= K) return fail("wrong handle");
   if (stream >= e->prm.n_streams) return fail("stream out of range");
+  if (!e->plan) return fail("engine not committed");
+  Plan &p = *e->plan;
+  const Slot &sl = p.cur();
   const size_t chain = (size_t) stream * K + handle;
   uint32_t cnt = 0;
   CK(cudaSetDevice(e->prm.device));
   CK(e->join());
-  CK(cudaMemcpyAsync(&cnt, e->d_counts + chain, sizeof(cnt), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(&cnt, sl.counts + chain, sizeof(cnt), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   size_t n = cnt;
   if (n > cap) n = cap;
-  if (soft) CK(cudaMemcpyAsync(soft, e->d_soft + chain * e->sym_cap, n * sizeof(float2), cudaMemcpyDeviceToHost, e->stream));
-  if (hard) CK(cudaMemcpyAsync(hard, e->d_hard + chain * e->sym_cap, n, cudaMemcpyDeviceToHost, e->stream));
+  if (soft) CK(cudaMemcpyAsync(soft, sl.soft + chain * p.sym_cap, n * sizeof(float2), cudaMemcpyDeviceToHost, e->stream));
+  if (hard) CK(cudaMemcpyAsync(hard, sl.hard + chain * p.sym_cap, n, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return (long) n;
 }
@@ -1155,7 +1137,7 @@ extern "C" int sdb_engine_read_all_symbols(sdb_engine_t *e, uint32_t *counts, sd
   const size_t chains = (size_t) e->prm.n_streams * e->channels.size();
   if (chains == 0) return 0;
   if (sdb_engine_read_all_symbols_async(e, counts, soft, hard, cap)) return -1;
-  CK(cudaStreamSynchronize(e->d2h_stream));
+  CK(cudaStreamSynchronize(e->plan->d2h_stream));
   return 0;
 }
 
@@ -1165,18 +1147,18 @@ extern "C" int sdb_engine_read_all_symbols_async(sdb_engine_t *e, uint32_t *coun
   if (!e || !counts) return fail("null argument");
   const size_t chains = (size_t) e->prm.n_streams * e->channels.size();
   if (chains == 0) return 0;
-  if (e->feed_index == 0) return fail("no symbols available");
-  const int ob = (int) ((e->feed_index - 1) & 1u);
+  if (!e->plan || e->plan->feed_index == 0) return fail("no symbols available");
+  Plan &p = *e->plan;
+  Slot &sl = p.cur();
   CK(cudaSetDevice(e->prm.device));
   // everything queued so far on the inspector stream (including this feed's launch or its count reset)
-  if (e->ev_insp_valid[ob]) CK(cudaStreamWaitEvent(e->d2h_stream, e->ev_insp[ob], 0));
-  CK(cudaMemcpyAsync(counts, e->d_countsb[ob], chains * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->d2h_stream));
-  const size_t w = std::min(cap, e->sym_cap);
-  if (soft) CK(cudaMemcpy2DAsync(soft, cap * sizeof(float2), e->d_softb[ob], e->sym_cap * sizeof(float2),
-                                 w * sizeof(float2), chains, cudaMemcpyDeviceToHost, e->d2h_stream));
-  if (hard) CK(cudaMemcpy2DAsync(hard, cap, e->d_hardb[ob], e->sym_cap, w, chains, cudaMemcpyDeviceToHost, e->d2h_stream));
-  CK(cudaEventRecord(e->ev_sym_read[ob], e->d2h_stream));
-  e->sym_read_valid[ob] = true;
+  CK(sl.insp.wait_on(p.d2h_stream));
+  CK(cudaMemcpyAsync(counts, sl.counts, chains * sizeof(uint32_t), cudaMemcpyDeviceToHost, p.d2h_stream));
+  const size_t w = std::min(cap, p.sym_cap);
+  if (soft) CK(cudaMemcpy2DAsync(soft, cap * sizeof(float2), sl.soft, p.sym_cap * sizeof(float2),
+                                 w * sizeof(float2), chains, cudaMemcpyDeviceToHost, p.d2h_stream));
+  if (hard) CK(cudaMemcpy2DAsync(hard, cap, sl.hard, p.sym_cap, w, chains, cudaMemcpyDeviceToHost, p.d2h_stream));
+  CK(sl.sym_read.record(p.d2h_stream));
   return 0;
 }
 
@@ -1201,22 +1183,20 @@ extern "C" int sdb_engine_read_symbols_packed_async(sdb_engine_t *e, uint32_t *c
   if (!e || !counts || !offsets) return fail("null argument");
   const size_t chains = (size_t) e->prm.n_streams * e->channels.size();
   if (chains == 0) return 0;
-  if (e->feed_index == 0) return fail("no symbols available");
-  const int ob = (int) ((e->feed_index - 1) & 1u);
+  if (!e->plan || e->plan->feed_index == 0) return fail("no symbols available");
+  Plan &p = *e->plan;
+  Slot &sl = p.cur();
   CK(cudaSetDevice(e->prm.device));
   void *dsoft = nullptr, *dhard = nullptr;
   if (device_writable(soft, &dsoft, "soft") || device_writable(hard, &dhard, "hard")) return -1;
-  if (!e->d_sym_off[ob]) {
-    e->d_sym_off[ob] = e->dalloc<unsigned long long>(chains + 1);
-    if (!e->d_sym_off[ob]) return fail("out of device memory (symbol offsets)");
-  }
-  if (e->ev_insp_valid[ob]) CK(cudaStreamWaitEvent(e->d2h_stream, e->ev_insp[ob], 0));
-  CK(sdb_launch_sym_pack(e->d2h_stream, e->d_countsb[ob], e->d_sym_off[ob], chains, e->d_softb[ob], e->d_hardb[ob],
-                         e->sym_cap, dsoft, dhard, (unsigned long long) cap_total, &e->launches));
-  CK(cudaMemcpyAsync(counts, e->d_countsb[ob], chains * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->d2h_stream));
-  CK(cudaMemcpyAsync(offsets, e->d_sym_off[ob], (chains + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->d2h_stream));
-  CK(cudaEventRecord(e->ev_sym_read[ob], e->d2h_stream));
-  e->sym_read_valid[ob] = true;
+  if (!sl.sym_off.size() && sl.sym_off.alloc(chains + 1) != cudaSuccess)
+    return fail("out of device memory (symbol offsets)");
+  CK(sl.insp.wait_on(p.d2h_stream));
+  CK(sdb_launch_sym_pack(p.d2h_stream, sl.counts, sl.sym_off, chains, sl.soft, sl.hard,
+                         p.sym_cap, dsoft, dhard, (unsigned long long) cap_total, &e->launches));
+  CK(cudaMemcpyAsync(counts, sl.counts, chains * sizeof(uint32_t), cudaMemcpyDeviceToHost, p.d2h_stream));
+  CK(cudaMemcpyAsync(offsets, sl.sym_off, (chains + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, p.d2h_stream));
+  CK(sl.sym_read.record(p.d2h_stream));
   return 0;
 }
 
@@ -1224,13 +1204,16 @@ extern "C" int sdb_engine_read_symbols_packed(sdb_engine_t *e, uint32_t *counts,
                                               uint8_t *hard, size_t cap_total)
 {
   if (sdb_engine_read_symbols_packed_async(e, counts, offsets, soft, hard, cap_total)) return -1;
-  CK(cudaStreamSynchronize(e->d2h_stream));
+  if (e->plan) CK(cudaStreamSynchronize(e->plan->d2h_stream));   // (no chains: an engine may read before its commit)
   return 0;
 }
 
-extern "C" const uint32_t *sdb_engine_symbol_counts_device(const sdb_engine_t *e) { return e ? e->d_counts : nullptr; }
-extern "C" size_t sdb_engine_symbol_capacity(const sdb_engine_t *e) { return e ? e->sym_cap : 0; }
-extern "C" void *sdb_engine_stream(const sdb_engine_t *e) { return e ? (void *) e->stream : nullptr; }
+extern "C" const uint32_t *sdb_engine_symbol_counts_device(const sdb_engine_t *e)
+{
+  return e && e->plan ? e->plan->cur().counts : nullptr;
+}
+extern "C" size_t sdb_engine_symbol_capacity(const sdb_engine_t *e) { return e && e->plan ? e->plan->sym_cap : 0; }
+extern "C" void *sdb_engine_stream(const sdb_engine_t *e) { return e ? (void *) e->stream.get() : nullptr; }
 extern "C" uint64_t sdb_engine_launch_count(const sdb_engine_t *e) { return e ? e->launches : 0; }
 extern "C" void sdb_engine_timing(sdb_engine_t *e, int enable)
 {
@@ -1261,56 +1244,58 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
 {
   CK(cudaSetDevice(dst->prm.device));
   if (sdb_engine_sync(src)) return -1;
+  Plan &to = *dst->plan;
+  const Plan &from = *src->plan;
   const unsigned S = dst->prm.n_streams, W = dst->W;
   const int Kn = (int) dst->channels.size(), Ko = (int) src->channels.size();
-  if (dst->d_hist && src->d_hist)
-    CK(cudaMemcpy(dst->d_hist, src->d_hist, (size_t) S * (W / 2) * sizeof(float2), cudaMemcpyDeviceToDevice));
-  if (dst->d_dc_state && src->d_dc_state)
-    CK(cudaMemcpy(dst->d_dc_state, src->d_dc_state, S * sizeof(float2), cudaMemcpyDeviceToDevice));
+  if (to.d_hist && from.d_hist)
+    CK(cudaMemcpy(to.d_hist, from.d_hist, (size_t) S * (W / 2) * sizeof(float2), cudaMemcpyDeviceToDevice));
+  if (to.d_dc_state && from.d_dc_state)
+    CK(cudaMemcpy(to.d_dc_state, from.d_dc_state, S * sizeof(float2), cudaMemcpyDeviceToDevice));
   // an engine that had no channel so far kept no input history: its first window starts with this feed
-  dst->first_feed = src->d_hist ? src->first_feed : true;
-  dst->n_fed = src->n_fed;
-  auto slot_of = [](const sdb_engine_t *e, int chain_g) {
-    for (size_t q = 0; q < e->h_chain_map.size(); ++q) if (e->h_chain_map[q] == chain_g) return (long) q;
+  to.first_feed = from.d_hist ? from.first_feed : true;
+  to.n_fed = from.n_fed;
+  auto slot_of = [](const Plan &p, int chain_g) {
+    for (size_t q = 0; q < p.h_chain_map.size(); ++q) if (p.h_chain_map[q] == chain_g) return (long) q;
     return -1L;
   };
   for (int kn = 0; kn < Kn; ++kn) {
     const int ko = kn < (int) old_of_new.size() ? old_of_new[kn] : -1;
     if (ko < 0 || ko >= Ko) continue;
     const Channel &cn = dst->channels[kn], &co = src->channels[ko];
-    const SdbChannelDev &dn = dst->h_chans[kn], &dold = src->h_chans[ko];
+    const SdbChannelDev &dn = to.h_chans[kn], &dold = from.h_chans[ko];
     const bool same_channel = co.p.f0 == cn.p.f0 && co.p.bw == cn.p.bw && co.p.guard == cn.p.guard &&
                               co.p.precise == cn.p.precise && co.size == cn.size && co.center == cn.center;
-    if (same_channel && !src->first_feed) {
-      CK(cudaMemcpy2D(dst->d_tails + dn.tail_off, dst->tail_stride * sizeof(float2), src->d_tails + dold.tail_off,
-                      src->tail_stride * sizeof(float2), (size_t) cn.halfsz * sizeof(float2), S, cudaMemcpyDeviceToDevice));
-      CK(cudaMemcpy2D(dst->d_lo_phase + kn, (size_t) Kn * sizeof(float), src->d_lo_phase + ko, (size_t) Ko * sizeof(float),
+    if (same_channel && !from.first_feed) {
+      CK(cudaMemcpy2D(to.d_tails + dn.tail_off, to.tail_stride * sizeof(float2), from.d_tails + dold.tail_off,
+                      from.tail_stride * sizeof(float2), (size_t) cn.halfsz * sizeof(float2), S, cudaMemcpyDeviceToDevice));
+      CK(cudaMemcpy2D(to.d_lo_phase + kn, (size_t) Kn * sizeof(float), from.d_lo_phase + ko, (size_t) Ko * sizeof(float),
                       sizeof(float), S, cudaMemcpyDeviceToDevice));
     }
     if (!cn.has_insp || !co.has_insp) continue;
-    const SdbChainCfg &a = dst->h_cfg[kn], &b = src->h_cfg[ko];
+    const SdbChainCfg &a = to.h_cfg[kn], &b = from.h_cfg[ko];
     if (a.cls != b.cls || a.have_agc != b.have_agc || a.dl_size != b.dl_size || a.mh_size != b.mh_size ||
         a.have_mf != b.have_mf || a.mf_n != b.mf_n || a.af_n != b.af_n || a.alpf_n != b.alpf_n ||
         a.have_costas != b.have_costas || a.have_pll != b.have_pll || a.eq_type != b.eq_type ||
         a.clock_type != b.clock_type)
       continue;                                            // structural change: this inspector restarts
-    CK(cudaMemcpy2D(dst->d_state + kn, (size_t) Kn * sizeof(SdbChainState), src->d_state + ko,
+    CK(cudaMemcpy2D(to.d_state + kn, (size_t) Kn * sizeof(SdbChainState), from.d_state + ko,
                     (size_t) Ko * sizeof(SdbChainState), sizeof(SdbChainState), S, cudaMemcpyDeviceToDevice));
     // clock.baud is a parameter AND the start value of the Gardner loop's own estimate: a new baud restarts it
     if (a.bnor != b.bnor) {
       std::vector<SdbChainState> st(S);
-      CK(cudaMemcpy2D(st.data(), sizeof(SdbChainState), dst->d_state + kn, (size_t) Kn * sizeof(SdbChainState),
+      CK(cudaMemcpy2D(st.data(), sizeof(SdbChainState), to.d_state + kn, (size_t) Kn * sizeof(SdbChainState),
                       sizeof(SdbChainState), S, cudaMemcpyDeviceToHost));
       for (auto &q : st) q.k_bnor = a.bnor;
-      CK(cudaMemcpy2D(dst->d_state + kn, (size_t) Kn * sizeof(SdbChainState), st.data(), sizeof(SdbChainState),
+      CK(cudaMemcpy2D(to.d_state + kn, (size_t) Kn * sizeof(SdbChainState), st.data(), sizeof(SdbChainState),
                       sizeof(SdbChainState), S, cudaMemcpyHostToDevice));
     }
     const size_t rows = (size_t) std::min(a.st_pool, b.st_pool);
     for (unsigned s = 0; s < S; ++s) {
-      const long qn = slot_of(dst, kn * (int) S + (int) s), qo = slot_of(src, ko * (int) S + (int) s);
+      const long qn = slot_of(to, kn * (int) S + (int) s), qo = slot_of(from, ko * (int) S + (int) s);
       if (qn < 0 || qo < 0) continue;
-      float *pd = dst->d_pool + (size_t) (qn / 32) * 32 * dst->pool_stride + (qn % 32);
-      const float *ps = src->d_pool + (size_t) (qo / 32) * 32 * src->pool_stride + (qo % 32);
+      float *pd = to.d_pool + (size_t) (qn / 32) * 32 * to.pool_stride + (qn % 32);
+      const float *ps = from.d_pool + (size_t) (qo / 32) * 32 * from.pool_stride + (qo % 32);
       CK(cudaMemcpy2D(pd, 32 * sizeof(float), ps, 32 * sizeof(float), sizeof(float), rows, cudaMemcpyDeviceToDevice));
     }
   }
@@ -1320,7 +1305,7 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
 static int migrate_check(sdb_engine_t *dst, sdb_engine_t *src)
 {
   if (!dst || !src) return fail("null engine");
-  if (!dst->committed || !src->committed) return fail("both engines must be committed");
+  if (!dst->plan || !src->plan) return fail("both engines must be committed");
   if (dst->prm.n_streams != src->prm.n_streams || dst->W != src->W || dst->prm.device != src->prm.device)
     return fail("engines differ in streams / window / device");
   return 0;
@@ -1398,7 +1383,7 @@ extern "C" long sdb_task_inspector(const sdb_inspector_config *cfg, const sdb_co
 int sdb_engine_pack_channels_device(sdb_engine_t *e, const double *centers_dev, sdb_detected_channel *out_dev, size_t cap,
                                     int *counts_dev, cudaStream_t st)
 {
-  if (!e || !e->committed || !e->chdet) return fail("channel detector not enabled");
-  CK(sdb_chdet_pack_device(e->chdet, e->samp_rate, centers_dev, out_dev, cap, counts_dev, st));
+  if (!e || !e->plan || !e->plan->chdet) return fail("channel detector not enabled");
+  CK(sdb_chdet_pack_device(e->plan->chdet.get(), e->samp_rate, centers_dev, out_dev, cap, counts_dev, st));
   return 0;
 }

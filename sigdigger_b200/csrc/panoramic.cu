@@ -121,7 +121,7 @@ struct sdb_panoramic {
   sdb_panoramic_params prm;
   int rank = 0, world = 1;
   ncclComm_t comm = nullptr;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   sdb_engine_t *eng = nullptr; size_t eng_hops = 0;
   sdb_sview_t *view = nullptr;
   size_t mb = 0;
@@ -133,8 +133,8 @@ struct sdb_panoramic {
   DevBuf<int32_t> d_off; DevBuf<sdb_detected_channel> d_dense; size_t dense_cap = 0;
   std::vector<sdb_detected_channel> h_full; std::vector<int32_t> h_full_cnt; bool full_valid = false;   // overflow path
   std::vector<double> centers_last;            // hop centres of the last sweep (already on the device)
-  cudaEvent_t ev_chan = nullptr, ev_eng = nullptr; bool chan_pending = false;
-  cudaEvent_t ev[4] = { nullptr, nullptr, nullptr, nullptr };
+  Event ev_chan, ev_eng; bool chan_pending = false;   // chan_pending: ev_chan recorded, not yet synchronised
+  Event ev[4];                                          // phase times of the last sweep
   sdb_panoramic_timing last{};
 };
 
@@ -168,10 +168,10 @@ extern "C" sdb_panoramic_t *sdb_panoramic_new(const sdb_panoramic_params *p, int
     ncclUniqueId id; memcpy(&id, id128, sizeof(id));
     if (g_nccl.CommInitRank(&s->comm, world, id, rank) != ncclSuccess) { g_perr = "ncclCommInitRank failed"; delete s; return nullptr; }
   }
-  cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-  for (auto &e : s->ev) cudaEventCreate(&e);
-  cudaEventCreateWithFlags(&s->ev_chan, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&s->ev_eng, cudaEventDisableTiming);
+  bool ok = s->stream.create(cudaStreamNonBlocking) == cudaSuccess && s->ev_chan.create() == cudaSuccess &&
+            s->ev_eng.create() == cudaSuccess;
+  for (auto &e : s->ev) ok = ok && e.create(cudaEventDefault) == cudaSuccess;
+  if (!ok) { g_perr = "CUDA stream or event creation failed"; sdb_panoramic_destroy(s); return nullptr; }
   s->view = sdb_sview_new(p->device);
   if (!s->view || sdb_sview_set_range(s->view, p->freq_min, p->freq_max, p->fft_bandwidth, p->rel_bw > 0 ? p->rel_bw : 0.5f)) {
     g_perr = "SpectrumView set-up failed"; sdb_panoramic_destroy(s); return nullptr;
@@ -188,10 +188,6 @@ extern "C" void sdb_panoramic_destroy(sdb_panoramic_t *s)
   if (s->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(s->comm);
   if (s->eng) sdb_engine_destroy(s->eng);
   if (s->view) sdb_sview_destroy(s->view);
-  for (auto &e : s->ev) if (e) cudaEventDestroy(e);
-  if (s->ev_chan) cudaEventDestroy(s->ev_chan);
-  if (s->ev_eng) cudaEventDestroy(s->ev_eng);
-  if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
 }
 

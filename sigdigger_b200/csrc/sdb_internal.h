@@ -60,6 +60,76 @@ private:
 };
 template <typename T> using PinnedBuf = DevBuf<T, true>;
 
+// A CUDA stream with one owner.  Move-only; the destructor destroys the stream without synchronising it, so an object
+// that queues work on its streams synchronises them before it releases anything.
+class Stream {
+public:
+  Stream() = default;
+  Stream(const Stream &) = delete;
+  Stream &operator=(const Stream &) = delete;
+  Stream(Stream &&o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+  Stream &operator=(Stream &&o) noexcept
+  {
+    if (this != &o) { release(); h_ = o.h_; o.h_ = nullptr; }
+    return *this;
+  }
+  ~Stream() { release(); }
+  cudaError_t create(unsigned flags, int priority = 0)
+  {
+    release();
+    cudaStream_t h = nullptr;
+    const cudaError_t e = cudaStreamCreateWithPriority(&h, flags, priority);
+    if (e != cudaSuccess) { cudaGetLastError(); return e; }
+    h_ = h;
+    return cudaSuccess;
+  }
+  void release() { if (h_) cudaStreamDestroy(h_); h_ = nullptr; }
+  cudaStream_t get() const { return h_; }
+  operator cudaStream_t() const { return h_; }
+private:
+  cudaStream_t h_ = nullptr;
+};
+
+// A CUDA event with one owner, which knows whether it has been recorded: wait_on() is a no-op until the first record(),
+// so "the buffer this event guards has never been used" needs no flag beside it.  Move-only; the destructor destroys.
+class Event {
+public:
+  Event() = default;
+  Event(const Event &) = delete;
+  Event &operator=(const Event &) = delete;
+  Event(Event &&o) noexcept : h_(o.h_), recorded_(o.recorded_) { o.h_ = nullptr; o.recorded_ = false; }
+  Event &operator=(Event &&o) noexcept
+  {
+    if (this != &o) { release(); h_ = o.h_; recorded_ = o.recorded_; o.h_ = nullptr; o.recorded_ = false; }
+    return *this;
+  }
+  ~Event() { release(); }
+  // cudaEventDefault for an event that times a span
+  cudaError_t create(unsigned flags = cudaEventDisableTiming)
+  {
+    release();
+    cudaEvent_t h = nullptr;
+    const cudaError_t e = cudaEventCreateWithFlags(&h, flags);
+    if (e != cudaSuccess) { cudaGetLastError(); return e; }
+    h_ = h;
+    return cudaSuccess;
+  }
+  void release() { if (h_) cudaEventDestroy(h_); h_ = nullptr; recorded_ = false; }
+  cudaError_t record(cudaStream_t s)
+  {
+    const cudaError_t e = cudaEventRecord(h_, s);
+    if (e == cudaSuccess) recorded_ = true;
+    return e;
+  }
+  // make stream s wait for the last record (nothing to wait for before the first)
+  cudaError_t wait_on(cudaStream_t s) const { return recorded_ ? cudaStreamWaitEvent(s, h_, 0) : cudaSuccess; }
+  cudaEvent_t get() const { return h_; }
+  operator cudaEvent_t() const { return h_; }
+private:
+  cudaEvent_t h_ = nullptr;
+  bool recorded_ = false;
+};
+
 // cudaFuncSetAttribute applies to the CURRENT device: a process that drives several GPUs (one GUI process, two
 // analyzers) must set it once per device, not once per process.  Returns true the first time on each device.
 static inline bool sdb_first_on_device(std::atomic<unsigned long long> &mask)

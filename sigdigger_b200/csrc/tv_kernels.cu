@@ -75,7 +75,7 @@ struct sdb_tv_processor {
   int device = 0; unsigned batch = 0;
   sdb_tv_params prm; SdbTvCfg cfg;
   DevBuf<SdbTvState> d_state; DevBuf<float> d_delay, d_line, d_ring, d_x; DevBuf<unsigned> d_done;
-  cudaStream_t stream = nullptr;
+  Stream stream;
 };
 
 extern "C" void sdb_tv_params_pal(sdb_tv_params *p, float samp_rate) { if (p) sdb_tv_preset(*p, samp_rate, true); }
@@ -85,7 +85,7 @@ extern "C" void sdb_tv_processor_destroy(sdb_tv_processor_t *t)
 {
   if (!t) return;
   cudaSetDevice(t->device);
-  if (t->stream) { cudaStreamSynchronize(t->stream); cudaStreamDestroy(t->stream); }
+  if (t->stream) cudaStreamSynchronize(t->stream);
   delete t;
 }
 
@@ -105,7 +105,7 @@ extern "C" sdb_tv_processor_t *sdb_tv_processor_new(const sdb_tv_params *p, uint
   bool ok = t->d_state.alloc(B) == cudaSuccess && t->d_delay.alloc(B * c.delay_len) == cudaSuccess &&
             t->d_line.alloc(B * c.W) == cudaSuccess && t->d_ring.alloc(B * SDB_TV_RING * c.H * c.W) == cudaSuccess &&
             t->d_done.alloc(B) == cudaSuccess &&
-            cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking) == cudaSuccess;
+            t->stream.create(cudaStreamNonBlocking) == cudaSuccess;
   if (ok) {
     SdbTvState s0; sdb_tv_state_init(c, s0);
     std::vector<SdbTvState> h(B, s0);
