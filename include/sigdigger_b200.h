@@ -456,6 +456,11 @@ typedef struct {
   int32_t device;
   int32_t input_format;           /* SDB_FORMAT_* of `data` (length counts IQ pairs); callback sources deliver float32 */
   int (*set_frequency)(void *priv, double freq);   /* tuner of the source; used by the wide-spectrum mode (may be NULL) */
+  /* suscan_source_config_set_average (Suscan/Source.cpp:195-201): source decimation D (0 or 1 = none, at most
+   * SDB_DECIMATION_MAX; channel mode only).  Every block reads D x read_size source samples, the FIR decimator
+   * (SPEC L) brings them to samp_rate / D, and everything downstream -- PSD, inspectors, channel detector, baseband
+   * filters, history -- runs at samp_rate / D.  Source time, seek and the throttle stay in source samples. */
+  uint32_t decimation;
 } sdb_source_config;
 
 /* Wide-spectrum (panoramic) mode, sdb_analyzer_params.mode = SDB_ANALYZER_MODE_WIDE_SPECTRUM
@@ -589,6 +594,27 @@ int          sdb_averager_reset(sdb_averager_t *a);                       /* Ave
 int          sdb_averager_feed_device(sdb_averager_t *a, const float *psd_dev, size_t frames, size_t stream_stride);
 const float *sdb_averager_device(const sdb_averager_t *a);                /* [n_streams][psd_size] */
 int          sdb_averager_read(sdb_averager_t *a, float *dst, size_t cap);
+/* Source decimator (SPEC L, oracle/SPEC_L.md; the source config's `average`, Suscan/Source.cpp:195-201): anti-aliased FIR decimation
+ * by D in [1, SDB_DECIMATION_MAX] with the brick-wall low-pass of 16 D + 1 taps at fc = 1/D (SPEC I.3), over
+ * n_streams streams fed together.  Output k of a stream is sum_i h_i x[kD - i]; the last 16 D input samples and the
+ * input phase are carried per stream on the device, so the outputs do not depend on how the input is split into
+ * feeds (a feed of m D samples yields m outputs).  Input: [n_streams] rows of n samples in input_format, stream_stride
+ * samples apart.  A device feed must be readable by the time the decimator's stream runs (synchronise its producer
+ * first).  Each feed returns its outputs per stream and overwrites the previous feed's output: [n_streams] rows,
+ * sdb_decimator_output_stride() complex samples apart, valid after sdb_decimator_sync. */
+#define SDB_DECIMATION_MAX 256
+typedef struct sdb_decimator sdb_decimator_t;
+sdb_decimator_t *sdb_decimator_new(int device, uint32_t n_streams, uint32_t decimation, int32_t input_format,
+                                   size_t max_feed);
+void     sdb_decimator_destroy(sdb_decimator_t *d);
+long     sdb_decimator_feed_device(sdb_decimator_t *d, const void *x, size_t stream_stride, size_t n);
+long     sdb_decimator_feed_host(sdb_decimator_t *d, const void *x, size_t stream_stride, size_t n);
+const sdb_complex *sdb_decimator_output_device(const sdb_decimator_t *d);
+size_t   sdb_decimator_output_stride(const sdb_decimator_t *d);
+void    *sdb_decimator_stream(const sdb_decimator_t *d);                          /* cudaStream_t of the feeds */
+int      sdb_decimator_sync(sdb_decimator_t *d);
+int      sdb_decimator_read(sdb_decimator_t *d, sdb_complex *dst, size_t cap);   /* [n_streams][outputs of last feed] */
+int      sdb_decimator_reset(sdb_decimator_t *d);                                 /* zero carry, phase 0 */
 /* device pointers of the last projection: j0[n_hops], nb[n_hops], va/vc[n_hops][max_bins] */
 int      sdb_sview_contrib(sdb_sview_t *v, int32_t **j0, int32_t **nb, float **va, float **vc);
 /* copy them into caller-owned device buffers (e.g. the send buffers of the NCCL gather) */

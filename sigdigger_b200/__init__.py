@@ -387,6 +387,16 @@ _PROTOS = {
     "sdb_averager_feed_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
     "sdb_averager_device": (C.c_void_p, [C.c_void_p]),
     "sdb_averager_read": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "sdb_decimator_new": (C.c_void_p, [C.c_int, C.c_uint32, C.c_uint32, C.c_int32, C.c_size_t]),
+    "sdb_decimator_destroy": (None, [C.c_void_p]),
+    "sdb_decimator_feed_device": (C.c_long, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
+    "sdb_decimator_feed_host": (C.c_long, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
+    "sdb_decimator_output_device": (C.c_void_p, [C.c_void_p]),
+    "sdb_decimator_output_stride": (C.c_size_t, [C.c_void_p]),
+    "sdb_decimator_stream": (C.c_void_p, [C.c_void_p]),
+    "sdb_decimator_sync": (C.c_int, [C.c_void_p]),
+    "sdb_decimator_read": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "sdb_decimator_reset": (C.c_int, [C.c_void_p]),
     "sdb_sview_contrib": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                     C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
     "sdb_sview_contrib_copy": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
@@ -880,6 +890,72 @@ class Averager:
         out = np.empty((self.n_streams, self.psd_size), np.float32)
         _check(self._L.sdb_averager_read(self._h, out.ctypes.data, out.size))
         return out
+
+
+class Decimator:
+    """Source decimator (SPEC L): FIR decimation by `decimation` of n_streams streams in a native sample format."""
+
+    def __init__(self, decimation, n_streams=1, input_format="f32", max_feed=1 << 20, device=0):
+        self._L = load_library()
+        self.decimation, self.n_streams, self.max_feed = decimation, n_streams, max_feed
+        self.input_format = FORMAT[input_format] if isinstance(input_format, str) else int(input_format)
+        self._h = self._L.sdb_decimator_new(device, n_streams, decimation, self.input_format, max_feed)
+        if not self._h:
+            raise SdbError(last_error())
+        self.last_out = 0
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.sdb_decimator_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def _rows(self, x):
+        """x: [n_streams, n] complex64 (f32) or [n_streams, 2 n] interleaved integers -> (array, n)"""
+        x = np.ascontiguousarray(x)
+        if x.ndim == 1:
+            x = x.reshape(1, -1)
+        assert x.shape[0] == self.n_streams
+        return x, x.shape[1] if self.input_format == FORMAT["f32"] else x.shape[1] // 2
+
+    def feed(self, x):
+        """Host feed; returns the outputs per stream of this feed (read them with read())."""
+        x, n = self._rows(x)
+        self.last_out = _check(self._L.sdb_decimator_feed_host(self._h, x.ctypes.data, n, n))
+        return self.last_out
+
+    def feed_ptr(self, ptr, n, stream_stride=None):
+        """Device feed: n samples per stream in the input format, stream_stride samples apart."""
+        self.last_out = _check(self._L.sdb_decimator_feed_device(self._h, ptr, n if stream_stride is None
+                                                                 else stream_stride, n))
+        return self.last_out
+
+    @property
+    def output_ptr(self):
+        return self._L.sdb_decimator_output_device(self._h)
+
+    @property
+    def output_stride(self):
+        return self._L.sdb_decimator_output_stride(self._h)
+
+    @property
+    def stream_ptr(self):
+        """cudaStream_t the feeds run on (e.g. for torch.cuda.ExternalStream)"""
+        return self._L.sdb_decimator_stream(self._h)
+
+    def sync(self):
+        _check(self._L.sdb_decimator_sync(self._h))
+
+    def read(self):
+        """-> complex64 [n_streams, outputs of the last feed]"""
+        out = np.empty((self.n_streams, self.last_out), np.complex64)
+        _check(self._L.sdb_decimator_read(self._h, out.ctypes.data, out.shape[0] * out.shape[1]))
+        return out
+
+    def reset(self):
+        _check(self._L.sdb_decimator_reset(self._h))
+        self.last_out = 0
 
 
 class PanoramicParams(C.Structure):

@@ -41,7 +41,13 @@ SETF_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_double)
 class SourceConfig(C.Structure):
     _fields_ = [("samp_rate", C.c_double), ("freq", C.c_double), ("read_size", C.c_size_t), ("read", READ_FN),
                 ("priv", C.c_void_p), ("data", C.c_void_p), ("length", C.c_size_t), ("loop", C.c_int32),
-                ("device", C.c_int32), ("input_format", C.c_int32), ("set_frequency", SETF_FN)]
+                ("device", C.c_int32), ("input_format", C.c_int32), ("set_frequency", SETF_FN),
+                ("decimation", C.c_uint32)]
+
+
+class SourceInfo(C.Structure):
+    _fields_ = [("permissions", C.c_uint64), ("source_samp_rate", C.c_uint64), ("effective_samp_rate", C.c_uint64),
+                ("measured_samp_rate", C.c_float), ("frequency", C.c_double), ("seekable", C.c_int32)]
 
 
 class PsdMsg(C.Structure):
@@ -75,7 +81,8 @@ class StatusMsg(C.Structure):
 class Analyzer:
     def __init__(self, samp_rate, window_size=8192, window="hann", psd_update_int=0.04, data=None, read=None,
                  read_size=0, loop=False, freq=0.0, device=0, channel_update_int=0.0, alpha=0.25, beta=0.25,
-                 gamma=0.5, snr=8.0, wide=False, min_freq=0.0, max_freq=0.0, set_frequency=None):
+                 gamma=0.5, snr=8.0, wide=False, min_freq=0.0, max_freq=0.0, set_frequency=None, decimation=1):
+        """decimation: source decimation D (SPEC L); the analyzer then runs at samp_rate / D."""
         self._L = load_library()
         p = AnalyzerParams()
         p.mode = 1 if wide else 0                      # SDB_ANALYZER_MODE_{CHANNEL, WIDE_SPECTRUM}
@@ -89,6 +96,7 @@ class Analyzer:
         self.params = p
         s = SourceConfig()
         s.samp_rate, s.freq, s.read_size, s.loop, s.device = samp_rate, freq, read_size, int(loop), device
+        s.decimation = decimation
         if data is not None:
             data = np.asarray(data)
             if data.dtype in (np.uint8, np.int8, np.int16):       # native capture formats: interleaved I,Q
@@ -233,6 +241,10 @@ class Analyzer:
                 arr = C.cast(m.channel_list, C.POINTER(DetectedChannel))
                 out = dict(channels=[dict(fc=arr[i].fc, f_lo=arr[i].f_lo, f_hi=arr[i].f_hi, bw=arr[i].bw,
                                           snr=arr[i].snr, S0=arr[i].S0, N0=arr[i].N0) for i in range(m.channel_count)])
+            elif name == "SOURCE_INFO":
+                m = C.cast(ptr, C.POINTER(SourceInfo)).contents
+                out = dict(source_samp_rate=m.source_samp_rate, effective_samp_rate=m.effective_samp_rate,
+                           frequency=m.frequency, seekable=m.seekable)
             elif name in ("EOS", "READ_ERROR", "HALT", "SOURCE_INIT"):
                 m = C.cast(ptr, C.POINTER(StatusMsg)).contents
                 out = dict(code=m.code, err_msg=(m.err_msg or b"").decode())

@@ -16,7 +16,7 @@
 // Differences stated openly: the channel plan is rebuilt at a block boundary whenever an inspector is
 // opened, closed or reconfigured, which restarts the loops of the inspectors that stay open (suscan keeps
 // them running); one source per analyzer; no estimators / spectrum sources (section 8(f)).
-#include "../../include/sigdigger_b200.h"
+#include "sdb_internal.h"
 
 #include <algorithm>
 #include <atomic>
@@ -121,7 +121,13 @@ struct sdb_analyzer {
     return nullptr;
   }
   bool plan_dirty = true;
-  size_t block = 0;
+  size_t block = 0;                               // samples per block at the analysis rate
+  // source decimation (SPEC L, suscan_source_config_set_average): each block reads block * decim source samples and
+  // the decimator brings them to `rate`.  It belongs to the analyzer, not to an engine, so that re-plans keep its carry.
+  uint32_t decim = 1;
+  double rate = 0;                                // analysis sample rate: src.samp_rate / decim
+  sdb_decimator_t *dec = nullptr;
+  std::vector<sdb_complex> raw;                   // one block of source samples in their native format
   std::atomic<double> measured_rate{ 0.0 };   // written by the worker, read by sdb_analyzer_get_measured_samp_rate
   uint64_t total_samples = 0;
   std::atomic<uint64_t> total_samples_pub{ 0 };   // copy for readers on other threads
@@ -157,7 +163,7 @@ struct sdb_analyzer {
     m->kind = kind; m->req_id = c.req_id; m->handle = i ? i->handle : c.handle;
     m->inspector_id = i ? i->inspector_id : c.inspector_id;
     m->class_name = dupstr(i ? (const char *[]){ "psk", "fsk", "ask", "audio", "raw" }[i->cls] : c.cls.c_str());
-    if (i) { m->channel = i->channel; m->config = i->cfg; m->fs = (float) src.samp_rate; m->equiv_fs = i->fs;
+    if (i) { m->channel = i->channel; m->config = i->cfg; m->fs = (float) rate; m->equiv_fs = i->fs;
              m->bandwidth = i->bandwidth; m->lo = i->lo; m->spectsrc_id = i->spectsrc_id; }
     else m->channel = c.channel;
     m->spectsrc_count = SDB_SPECTSRC_COUNT - 1; m->estimator_count = SDB_ESTIMATOR_COUNT;
@@ -208,17 +214,17 @@ struct sdb_analyzer {
     ep.max_feed = (uint32_t) block;
     ep.device = src.device;
     ep.flags = (iq_reverse ? SDB_FLAG_IQ_REVERSE : 0) | (dc_remove ? SDB_FLAG_DC_REMOVE : 0);
-    ep.input_format = src.read ? SDB_FORMAT_FLOAT32 : src.input_format;
-    eng = sdb_engine_new(&ep, src.samp_rate);
+    ep.input_format = src.read || dec ? SDB_FORMAT_FLOAT32 : src.input_format;
+    eng = sdb_engine_new(&ep, rate);
     if (!eng) { drop_old(); post_status(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INIT, SDB_ANALYZER_INIT_FAILURE, sdb_last_error()); return false; }
     std::vector<int32_t> old_of_new;
     for (auto &i : insps) {
       i.engine_handle = -1;
       if (!i.open || i.parent >= 0) continue;
       sdb_channel_params cp;
-      double f = fmod(i.channel.fc / src.samp_rate + 1.0, 1.0);
+      double f = fmod(i.channel.fc / rate + 1.0, 1.0);
       cp.f0 = (float) (2.0 * 3.14159265358979323846 * f);
-      cp.bw = (float) (2.0 * 3.14159265358979323846 * (i.channel.f_hi - i.channel.f_lo) / src.samp_rate);
+      cp.bw = (float) (2.0 * 3.14159265358979323846 * (i.channel.f_hi - i.channel.f_lo) / rate);
       cp.guard = 1.0f; cp.precise = i.precise;
       sdb_channel_info info;
       int h = sdb_engine_open_channel(eng, &cp, &info);
@@ -226,7 +232,7 @@ struct sdb_analyzer {
       i.engine_handle = h;
       old_of_new.push_back(old_handle[(size_t) i.handle]);
       i.size = info.size;
-      i.fs = (float) (src.samp_rate / info.decimation);
+      i.fs = (float) (rate / info.decimation);
       i.bandwidth = (float) (i.channel.f_hi - i.channel.f_lo);
       i.lo = (float) i.channel.fc;
       i.cfg.insp_class = i.cls;
@@ -330,7 +336,7 @@ struct sdb_analyzer {
           double bw = c.channel.f_hi - c.channel.f_lo;
           if (cls < 0) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_KIND, c, nullptr); break; }
           // the input of the new inspector: the baseband, or (sub-carrier inspection) the channel of `parent`
-          double in_rate = src.samp_rate;
+          double in_rate = rate;
           uint32_t in_window = (uint32_t) params.detector_params.window_size;
           if (c.parent >= 0) {
             if (c.parent >= (int32_t) insps.size() || !insps[c.parent].open || insps[c.parent].size < 16) {
@@ -439,12 +445,12 @@ struct sdb_analyzer {
           // re-planned at the next block boundary (see the a18 limits in DESIGN.md).
           if (c.handle < 0 || c.handle >= (int32_t) insps.size() || !insps[c.handle].open) break;
           Insp &i = insps[c.handle];
-          const double rate = i.parent >= 0 ? (double) insps[i.parent].fs : src.samp_rate;
+          const double in_rate = i.parent >= 0 ? (double) insps[i.parent].fs : rate;
           if (c.kind == Cmd::SET_FREQ) {
-            if (fabs(c.value) > rate / 2) break;
+            if (fabs(c.value) > in_rate / 2) break;
             i.channel.fc = c.value; i.lo = (float) c.value;
           } else {
-            if (!(c.value > 0) || c.value > rate) break;
+            if (!(c.value > 0) || c.value > in_rate) break;
             i.channel.f_lo = -0.5 * c.value; i.channel.f_hi = 0.5 * c.value; i.channel.bw = (float) c.value;
             i.bandwidth = (float) c.value;
           }
@@ -613,7 +619,7 @@ struct sdb_analyzer {
     }
     {
       sdb_source_info *si = (sdb_source_info *) calloc(1, sizeof(*si));
-      si->source_samp_rate = (uint64_t) src.samp_rate; si->effective_samp_rate = (uint64_t) src.samp_rate;
+      si->source_samp_rate = (uint64_t) src.samp_rate; si->effective_samp_rate = (uint64_t) rate;
       si->measured_samp_rate = 0; si->frequency = src.freq; si->seekable = src.read ? 0 : 1;
       post(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INFO, si);
     }
@@ -625,9 +631,19 @@ struct sdb_analyzer {
       const size_t N = (size_t) params.detector_params.window_size;
       if (block % N) block = std::max<size_t>(N, (block / N) * N);     // after a PARAMS change
       if (buf.size() != block) buf.resize(block);
+      if (decim > 1 && raw.size() < block * decim) {    // first block, or a PARAMS change that grew the block
+        if (dec) sdb_decimator_destroy(dec);
+        raw.resize(block * decim);
+        dec = sdb_decimator_new(src.device, 1, decim, src.read ? SDB_FORMAT_FLOAT32 : src.input_format, raw.size());
+        if (!dec) {
+          post_status(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INIT, SDB_ANALYZER_INIT_FAILURE, sdb_last_error());
+          exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
+        }
+      }
       if (plan_dirty && !rebuild()) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
       long got;
-      const bool f32_src = src.read || src.input_format == SDB_FORMAT_FLOAT32;
+      const bool f32_src = src.read || src.input_format == SDB_FORMAT_FLOAT32 || dec;
+      bool on_device = false;                      // the decimated block is only in the decimator's device output
       if (replaying && hist_fill > 0) {
         // suscan_analyzer_replay: the source is paused and the history ring is played back, oldest sample first
         for (size_t i = 0; i < block; ++i) {
@@ -637,7 +653,27 @@ struct sdb_analyzer {
         }
         got = (long) block;
       } else {
-        got = source_read(buf.data(), block);
+        if (dec) {
+          // SPEC L: block * decim source samples in their native format -> block float32 samples at `rate`.  Baseband
+          // filters and the history see the decimated samples on the host; otherwise the engine reads them in place.
+          const long g = source_read(raw.data(), block * decim);
+          got = g < 0 ? g : g / (long) decim;
+          if (got == (long) block) {
+            if (sdb_decimator_feed_host(dec, raw.data(), raw.size(), block * decim) != (long) block) {
+              exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
+            }
+            bool host = !hist.empty();
+            { std::lock_guard<std::mutex> l(cmd_m); host = host || !bb_filters.empty(); }
+            if (!host) {
+              if (sdb_decimator_sync(dec)) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
+              on_device = true;
+            } else if (sdb_decimator_read(dec, buf.data(), buf.size())) {
+              exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
+            }
+          }
+        } else {
+          got = source_read(buf.data(), block);
+        }
         if (got == (long) block && f32_src && !hist.empty()) {       // suscan_analyzer_set_history_size: keep the tail
           for (size_t i = 0; i < block; ++i) {
             hist[(hist_start + hist_fill) % hist.size()] = buf[i];
@@ -647,16 +683,23 @@ struct sdb_analyzer {
       }
       if (got < 0) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
       if ((size_t) got < block) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_EOS; break; }   // partial tail blocks are dropped
-      // baseband filters see (and may rewrite) every float32 block before the analyzer does, in registration order
-      if (src.read || src.input_format == SDB_FORMAT_FLOAT32) {
+      // baseband filters see (and may rewrite) every float32 block before the analyzer does, in registration order;
+      // with decimation the block and the offset are at the decimated rate
+      if (f32_src) {
         std::vector<BbFilter> fl;
         { std::lock_guard<std::mutex> l(cmd_m); fl = bb_filters; }
-        for (auto &f : fl) f.fn(f.priv, this, buf.data(), (uint64_t) block, total_samples);
+        if (on_device && !fl.empty()) {                  // a filter registered while the block was being read
+          if (sdb_decimator_read(dec, buf.data(), buf.size())) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
+          on_device = false;
+        }
+        for (auto &f : fl) f.fn(f.priv, this, buf.data(), (uint64_t) block, total_samples / decim);
       }
-      if (sdb_engine_feed_host(eng, buf.data(), block, block) || sdb_engine_sync(eng)) {
+      const int fed = on_device ? sdb_engine_feed_device(eng, sdb_decimator_output_device(dec), block, block)
+                                : sdb_engine_feed_host(eng, buf.data(), block, block);
+      if (fed || sdb_engine_sync(eng)) {
         exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
       }
-      total_samples += block;
+      total_samples += block * decim;                   // source samples
       total_samples_pub.store(total_samples);
       if (throttle > 0) {                                // suscan_analyzer_set_throttle_async: pace to `throttle` samples/s
         const double due = (double) (total_samples - throttle_s0) / throttle;
@@ -669,15 +712,15 @@ struct sdb_analyzer {
       const size_t frames = block / N;
       psd.resize(frames * N);
       if (sdb_engine_read_psd(eng, psd.data(), psd.size()) == 0) {
-        const double per_frame = (double) N / src.samp_rate;
+        const double per_frame = (double) N / rate;
         for (size_t f = 0; f < frames; ++f) {
           psd_credit += per_frame;
           if (psd_credit + 1e-12 >= params.psd_update_int) {
             psd_credit = params.psd_update_int > 0 ? fmod(psd_credit, params.psd_update_int) : 0;
             sdb_analyzer_psd_msg *m = (sdb_analyzer_psd_msg *) calloc(1, sizeof(*m));
-            m->fc = (int64_t) src.freq; m->samp_rate = (float) src.samp_rate; m->measured_samp_rate = (float) measured_rate.load();
+            m->fc = (int64_t) src.freq; m->samp_rate = (float) rate; m->measured_samp_rate = (float) measured_rate.load();
             gettimeofday(&m->rt_time, nullptr);
-            double ts = (double) (total_samples - block + f * N) / src.samp_rate;
+            double ts = (double) (total_samples - block * decim + f * N * decim) / src.samp_rate;
             m->timestamp.tv_sec = (time_t) ts; m->timestamp.tv_usec = (suseconds_t) ((ts - floor(ts)) * 1e6);
             m->looped = looped; m->history_size = (uint64_t) hist_fill;
             m->psd_size = N;
@@ -726,7 +769,7 @@ struct sdb_analyzer {
             m->kind = SDB_INSPECTOR_MSGKIND_SPECTRUM; m->handle = i.handle; m->inspector_id = i.inspector_id;
             m->class_name = dupstr((const char *[]){ "psk", "fsk", "ask", "audio", "raw" }[i.cls]);
             m->spectsrc_id = i.spectsrc_id; m->spectrum_size = emitted; m->samp_rate = (uint64_t) i.fs;
-            m->fs = (float) src.samp_rate; m->equiv_fs = i.fs;
+            m->fs = (float) rate; m->equiv_fs = i.fs;
             m->spectrum_data = (float *) malloc(emitted * sizeof(float));
             memcpy(m->spectrum_data, sp.data(), emitted * sizeof(float));
             post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
@@ -746,7 +789,7 @@ struct sdb_analyzer {
       }
       // MESSAGE_TYPE_CHANNEL at channel_update_int cadence of signal time
       if (params.channel_update_int > 0) {
-        chan_credit += (double) block / src.samp_rate;
+        chan_credit += (double) block / rate;
         if (chan_credit + 1e-12 >= params.channel_update_int) {
           chan_credit = fmod(chan_credit, params.channel_update_int);
           std::vector<sdb_detected_channel> ch(256);
@@ -766,6 +809,7 @@ struct sdb_analyzer {
       if (i.has_id && pending.count(i.handle)) deliver(i, nullptr, nullptr, 0, true);
     drop_subs();
     if (eng) { sdb_engine_destroy(eng); eng = nullptr; }
+    if (dec) { sdb_decimator_destroy(dec); dec = nullptr; }
     post_status(exit_type, 0, exit_type == SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR ? sdb_last_error() : nullptr);
   }
 };
@@ -777,9 +821,21 @@ extern "C" sdb_analyzer_t *sdb_analyzer_new(const sdb_analyzer_params *params, c
   const uint64_t N = params->detector_params.window_size;
   if (N < 16 || (N & (N - 1)) || !(src->samp_rate > 0) || (!src->read && !src->data)) return nullptr;
   if (src->input_format < SDB_FORMAT_FLOAT32 || src->input_format > SDB_FORMAT_SIGNED16) return nullptr;
+  const uint32_t D = src->decimation ? src->decimation : 1;
+  if (D > SDB_DECIMATION_MAX) {
+    fail("source decimation must be at most " + std::to_string(SDB_DECIMATION_MAX) + ", got " + std::to_string(D));
+    return nullptr;
+  }
+  // a wide-spectrum hop would carry the decimator's history across a retune
+  if (D > 1 && params->mode == SDB_ANALYZER_MODE_WIDE_SPECTRUM) {
+    fail("source decimation is not supported in wide-spectrum mode");
+    return nullptr;
+  }
   sdb_analyzer *a = new sdb_analyzer();
   a->params = *params;
   a->src = *src;
+  a->decim = D;
+  a->rate = src->samp_rate / (double) D;
   size_t blk = src->read_size ? src->read_size : (size_t) N * 8;
   blk = std::max<size_t>(N, (blk / N) * N);
   a->block = blk;
@@ -1014,5 +1070,5 @@ extern "C" int sdb_analyzer_set_params_async(sdb_analyzer_t *a, const sdb_analyz
   Cmd c; c.kind = Cmd::SET_PARAMS; c.req_id = req_id; c.params = *p;
   return push_cmd(a, std::move(c));
 }
-extern "C" uint64_t sdb_analyzer_get_samp_rate(const sdb_analyzer_t *a) { return a ? (uint64_t) a->src.samp_rate : 0; }
+extern "C" uint64_t sdb_analyzer_get_samp_rate(const sdb_analyzer_t *a) { return a ? (uint64_t) a->rate : 0; }
 extern "C" float sdb_analyzer_get_measured_samp_rate(const sdb_analyzer_t *a) { return a ? (float) a->measured_rate.load() : 0; }

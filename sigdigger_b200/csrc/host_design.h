@@ -111,6 +111,18 @@ inline void taps_rrc(std::vector<float> &h, unsigned n, float T, float beta)
   }
 }
 
+// SPEC I.3 (su_taps_brickwall_lp_init): h_i = fc sinc(fc (i - floor(n / 2))) x Hamming, binary64 rounded once
+inline void taps_brickwall_lp(float *h, unsigned n, float fc)
+{
+  for (unsigned i = 0; i < n; ++i) {
+    const double t = (double) i - (double) (n >> 1);
+    const double xx = kPi * (double) fc * t;
+    double v = fabs(xx) < 1e-12 ? (double) fc : (double) fc * sin(xx) / xx;
+    if (n > 1) v *= 0.54 - 0.46 * cos(2.0 * kPi * (double) i / (double) (n - 1));
+    h[i] = (float) v;
+  }
+}
+
 inline unsigned mf_span(float T)  // include/WaveSampler.h:29-30
 {
   double s = ceil(6.0 * (double) T);

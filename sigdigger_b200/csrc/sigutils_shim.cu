@@ -356,14 +356,7 @@ void su_taps_rrc_init(SUFLOAT *h, SUFLOAT T, SUFLOAT beta, SUSCOUNT size)
 }
 void su_taps_brickwall_lp_init(SUFLOAT *h, SUFLOAT fc, SUSCOUNT n)
 {
-  // SPEC I.3: h_i = fc sinc(fc (i - floor(n / 2))) x Hamming, binary64 rounded once
-  for (SUSCOUNT i = 0; i < n; ++i) {
-    const double t = (double) i - (double) (n >> 1);
-    const double xx = sdbh::kPi * (double) fc * t;
-    double v = fabs(xx) < 1e-12 ? (double) fc : (double) fc * sin(xx) / xx;
-    if (n > 1) v *= 0.54 - 0.46 * cos(2.0 * sdbh::kPi * (double) i / (double) (n - 1));
-    h[i] = (float) v;
-  }
+  sdbh::taps_brickwall_lp(h, (unsigned) n, fc);
 }
 
 }  // extern "C"

@@ -620,7 +620,9 @@ suscan_analyzer_t *suscan_analyzer_new(const struct suscan_analyzer_params *para
   suscan_source_info_init(&sa->info);
   sdb_source_config sc;
   memset(&sc, 0, sizeof(sc));
-  sc.samp_rate = (double) config->samp_rate / (double) (config->average ? config->average : 1);
+  // `average` is the source decimation (SPEC L): the analyzer reads samp_rate and runs at samp_rate / average
+  sc.samp_rate = (double) config->samp_rate;
+  sc.decimation = config->average ? config->average : 1;
   sc.freq = config->freq; sc.read_size = (size_t) config->read_size; sc.device = config->gpu;
   sc.loop = config->loop ? 1 : 0;
   static const int fmt_of[] = { -1, SDB_FORMAT_FLOAT32, SDB_FORMAT_UNSIGNED8, SDB_FORMAT_SIGNED16, SDB_FORMAT_SIGNED8, -1, -1 };
@@ -651,7 +653,8 @@ suscan_analyzer_t *suscan_analyzer_new(const struct suscan_analyzer_params *para
   }
   sa->info.permissions = SUSCAN_ANALYZER_PERM_ALL & ~(SUSCAN_ANALYZER_PERM_SET_GAIN | SUSCAN_ANALYZER_PERM_SET_ANTENNA |
                                                       SUSCAN_ANALYZER_PERM_SET_AGC | SUSCAN_ANALYZER_PERM_SET_PPM);
-  sa->info.source_samp_rate = (SUSCOUNT) sc.samp_rate; sa->info.effective_samp_rate = (SUSCOUNT) sc.samp_rate;
+  sa->info.source_samp_rate = (SUSCOUNT) sc.samp_rate;
+  sa->info.effective_samp_rate = (SUSCOUNT) (sc.samp_rate / (double) sc.decimation);
   sa->info.frequency = sc.freq; sa->info.freq_min = -3e11; sa->info.freq_max = 3e11; sa->info.lnb = config->lnb;
   sa->info.bandwidth = config->bandwidth; sa->info.dc_remove = config->dc_remove;
   sa->info.seekable = (sc.data != nullptr) ? SU_TRUE : SU_FALSE;
