@@ -26,6 +26,7 @@
 #include <cstring>
 #include <deque>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -41,7 +42,7 @@ struct Cmd {
   double value2 = 0;
   uint32_t req_id = 0;
   uint32_t aux_id = 0; int enabled = 0;       // spectrum source id / estimator id + enable flag
-  double value = 0;                           // throttle rate
+  double value = 0;                           // the request's number: rate, watermark, size, position, frequency...
   int32_t handle = -1;
   int32_t parent = -1;                        // open_ex: handle of the inspector whose channel is the input
   uint32_t inspector_id = 0;
@@ -70,23 +71,29 @@ struct Insp {
   uint32_t spect_size;    // frame size chosen at rebuild time (0 = too few channel samples per block)
 };
 
+// class names in SDB_INSP_* order, as requests and inspector messages carry them
+const char *const kClassNames[] = { "psk", "fsk", "ask", "audio", "raw" };
+
 int class_id(const std::string &c)
 {
-  if (c == "psk") return SDB_INSP_PSK;
-  if (c == "fsk") return SDB_INSP_FSK;
-  if (c == "ask") return SDB_INSP_ASK;
-  if (c == "audio") return SDB_INSP_AUDIO;
-  if (c == "raw") return SDB_INSP_RAW;
+  for (int k = SDB_INSP_PSK; k <= SDB_INSP_RAW; ++k)
+    if (c == kClassNames[k]) return k;
   return -1;
 }
 
-char *dupstr(const char *s)
+// a sigutils channel (Hz, relative to the input's centre) as channeliser parameters at the input rate in_rate
+sdb_channel_params channel_params(const sdb_sigutils_channel &ch, double in_rate, int precise)
 {
-  size_t n = strlen(s) + 1;
-  char *p = (char *) malloc(n);
-  memcpy(p, s, n);
-  return p;
+  sdb_channel_params cp;
+  cp.f0 = (float) (2.0 * 3.14159265358979323846 * fmod(ch.fc / in_rate + 1.0, 1.0));
+  cp.bw = (float) (2.0 * 3.14159265358979323846 * (ch.f_hi - ch.f_lo) / in_rate);
+  cp.guard = 1.0f; cp.precise = precise;
+  return cp;
 }
+
+struct EngineDeleter { void operator()(sdb_engine_t *e) const { sdb_engine_destroy(e); } };
+struct DecimatorDeleter { void operator()(sdb_decimator_t *d) const { sdb_decimator_destroy(d); } };
+using EnginePtr = std::unique_ptr<sdb_engine_t, EngineDeleter>;
 
 }  // namespace
 
@@ -104,20 +111,19 @@ struct sdb_analyzer {
   bool halt_req = false;
   std::thread worker;
   std::vector<Insp> insps;
-  sdb_engine_t *eng = nullptr;
+  EnginePtr eng;
   // Sub-carrier inspection (GenericInspector.cpp:502-525: openInspectorTab(..., parent = this handle)): every
   // inspector with open children -- at any depth: a sub-carrier inspector can be a parent itself -- gets an engine
   // whose input is its channel stream and whose channeliser window equals its channel size, so that one parent hop
   // is exactly one child hop.  Children have inspector chains, spectrum sources and estimators like any other.
-  struct Sub { int32_t parent; sdb_engine_t *eng; };
+  struct Sub { int32_t parent; EnginePtr eng; };
   std::vector<Sub> subs;
-  void drop_subs() { for (auto &s : subs) if (s.eng) sdb_engine_destroy(s.eng); subs.clear(); }
   // the engine that runs inspector i's chain: the analyzer's own for a baseband inspector, its parent's
   // sub-carrier engine otherwise
-  template <class I> sdb_engine_t *engine_of(const I &i) const
+  sdb_engine_t *engine_of(const Insp &i) const
   {
-    if (i.parent < 0) return eng;
-    for (auto &sb : subs) if (sb.parent == i.parent) return sb.eng;
+    if (i.parent < 0) return eng.get();
+    for (auto &sb : subs) if (sb.parent == i.parent) return sb.eng.get();
     return nullptr;
   }
   bool plan_dirty = true;
@@ -126,12 +132,22 @@ struct sdb_analyzer {
   // the decimator brings them to `rate`.  It belongs to the analyzer, not to an engine, so that re-plans keep its carry.
   uint32_t decim = 1;
   double rate = 0;                                // analysis sample rate: src.samp_rate / decim
-  sdb_decimator_t *dec = nullptr;
+  std::unique_ptr<sdb_decimator_t, DecimatorDeleter> dec;
   std::vector<sdb_complex> raw;                   // one block of source samples in their native format
+  std::vector<sdb_complex> buf;                   // one block at `rate` on the host (a sweep's hops in wide mode)
+  std::vector<sdb_complex> drop;                  // samples a sweep reads and discards after a retune
+  std::vector<float> psd;
+  std::vector<sdb_complex> soft;
+  std::vector<uint8_t> hard;
+  std::chrono::steady_clock::time_point t0;       // start of the worker loop, for the measured rate
+  uint32_t exit_type = SDB_WORKER_MSG_TYPE_HALT;  // the status that ends the worker, set by stop()
   std::atomic<double> measured_rate{ 0.0 };   // written by the worker, read by sdb_analyzer_get_measured_samp_rate
   uint64_t total_samples = 0;
   std::atomic<uint64_t> total_samples_pub{ 0 };   // copy for readers on other threads
-  std::mutex insp_m;                              // guards insps against readers on other threads
+  // Guards insps against readers on other threads (sdb_analyzer_get_inspector_config).  The worker changes insps
+  // under it in handle_cmds; outside it, it writes only fields that no other thread reads (the engine mapping and
+  // geometry set by rebuild).
+  std::mutex insp_m;
   double psd_credit = 0;
   // source-side options of the worker loop (Suscan/Analyzer.cpp:117-135, 229-244; SourceWidget.cpp:1156-1184)
   bool iq_reverse = false, dc_remove = false;
@@ -144,6 +160,15 @@ struct sdb_analyzer {
   struct BbFilter { sdb_baseband_filter_fn fn; void *priv; int64_t prio; };
   std::vector<BbFilter> bb_filters;
 
+  Insp *open_insp(int32_t handle)
+  {
+    return handle >= 0 && handle < (int32_t) insps.size() && insps[handle].open ? &insps[handle] : nullptr;
+  }
+  // bytes per IQ pair of what source_read() delivers: float32 from a read callback, else the capture's own format
+  size_t src_bytes() const { return src.read ? 8 : sdb_fmt_bytes(src.input_format); }
+  // the blocks the analyzer sees are float32 (baseband filters and the history need that)
+  bool f32_src() const { return src.read || src.input_format == SDB_FORMAT_FLOAT32 || dec; }
+
   void post(uint32_t type, void *payload)
   {
     std::lock_guard<std::mutex> l(mq_m);
@@ -154,15 +179,42 @@ struct sdb_analyzer {
   {
     sdb_analyzer_status_msg *m = (sdb_analyzer_status_msg *) calloc(1, sizeof(*m));
     m->code = code;
-    m->err_msg = msg ? dupstr(msg) : nullptr;
+    m->err_msg = msg ? strdup(msg) : nullptr;
     post(type, m);
   }
-  void post_inspector(int kind, const Cmd &c, const Insp *i)
+  // the steps of the worker return true to go on, or stop(): false, with the status that ends the worker
+  bool stop(uint32_t type) { exit_type = type; return false; }
+  bool init_failure()
+  {
+    post_status(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INIT, SDB_ANALYZER_INIT_FAILURE, sdb_last_error());
+    return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+  }
+  // ts: signal time of the first sample of the frame, in seconds
+  void post_psd(int64_t fc, double samp_rate, const float *data, size_t n, double ts, int looped_, uint64_t history)
+  {
+    sdb_analyzer_psd_msg *m = (sdb_analyzer_psd_msg *) calloc(1, sizeof(*m));
+    m->fc = fc; m->samp_rate = (float) samp_rate; m->measured_samp_rate = (float) measured_rate.load();
+    gettimeofday(&m->rt_time, nullptr);
+    m->timestamp.tv_sec = (time_t) ts; m->timestamp.tv_usec = (suseconds_t) ((ts - floor(ts)) * 1e6);
+    m->looped = looped_; m->history_size = history;
+    m->psd_size = n;
+    m->psd_data = (float *) malloc(n * sizeof(float));
+    memcpy(m->psd_data, data, n * sizeof(float));
+    post(SDB_ANALYZER_MESSAGE_TYPE_PSD, m);
+  }
+  // an inspector message with the fields every kind carries; the caller fills the rest and posts it
+  static sdb_analyzer_inspector_msg *inspector_msg(int kind, int32_t handle, uint32_t inspector_id, const char *cls)
   {
     sdb_analyzer_inspector_msg *m = (sdb_analyzer_inspector_msg *) calloc(1, sizeof(*m));
-    m->kind = kind; m->req_id = c.req_id; m->handle = i ? i->handle : c.handle;
-    m->inspector_id = i ? i->inspector_id : c.inspector_id;
-    m->class_name = dupstr(i ? (const char *[]){ "psk", "fsk", "ask", "audio", "raw" }[i->cls] : c.cls.c_str());
+    m->kind = kind; m->handle = handle; m->inspector_id = inspector_id; m->class_name = strdup(cls);
+    return m;
+  }
+  // the reply to request c: about inspector i, or (i null) an error that echoes the request
+  void post_inspector(int kind, const Cmd &c, const Insp *i)
+  {
+    sdb_analyzer_inspector_msg *m = i ? inspector_msg(kind, i->handle, i->inspector_id, kClassNames[i->cls])
+                                      : inspector_msg(kind, c.handle, c.inspector_id, c.cls.c_str());
+    m->req_id = c.req_id;
     if (i) { m->channel = i->channel; m->config = i->cfg; m->fs = (float) rate; m->equiv_fs = i->fs;
              m->bandwidth = i->bandwidth; m->lo = i->lo; m->spectsrc_id = i->spectsrc_id; }
     else m->channel = c.channel;
@@ -193,18 +245,65 @@ struct sdb_analyzer {
     post(SDB_ANALYZER_MESSAGE_TYPE_SAMPLES, m);
   }
 
-  // (re)build the engine from the open inspectors at a block boundary.  The new engine takes over the running
-  // state of the old one (sdb_engine_migrate_map): input history, DC estimate, and for every inspector that stays
-  // open its cross-fade tail, LO phase and loop state -- opening, closing, retuning or reconfiguring ONE inspector
-  // leaves the sample streams of the others untouched (suscan keeps them running too, Suscan/Analyzer.cpp:459-537).
-  // Returns false on failure (status message posted).
+  // Plans one engine level: the baseband (parent -1, with the channel detector) or the children of inspector
+  // `parent`, whose channel stream at in_rate is the input.  Every open inspector of the level gets a channel, in
+  // handle order; one whose channel cannot be opened stays unmapped.  After the commit the engine takes over the
+  // running state of `old` where the geometry allows (old_handle: each inspector's handle in the engines being
+  // replaced).  Returns null when the engine cannot be created or committed; sdb_last_error() says why.
+  EnginePtr plan_level(const sdb_engine_params &ep, double in_rate, int32_t parent, const std::vector<int> &old_handle,
+                       sdb_engine_t *old)
+  {
+    EnginePtr e(sdb_engine_new(&ep, in_rate));
+    if (!e) return nullptr;
+    const size_t hops_per_block = block / (params.detector_params.window_size / 2);
+    std::vector<int32_t> old_of_new;
+    for (auto &i : insps) {
+      if (!i.open || i.parent != parent) continue;
+      const sdb_channel_params cp = channel_params(i.channel, in_rate, i.precise);
+      sdb_channel_info info;
+      const int h = sdb_engine_open_channel(e.get(), &cp, &info);
+      if (h < 0) continue;
+      i.engine_handle = h; i.size = info.size;
+      old_of_new.push_back(old_handle[(size_t) i.handle]);
+      i.fs = (float) (in_rate / info.decimation);
+      i.bandwidth = (float) (i.channel.f_hi - i.channel.f_lo); i.lo = (float) i.channel.fc;
+      sdb_engine_set_inspector(e.get(), h, &i.cfg);
+      // spectrum source / estimators: the largest frame (<= 4096) a steady-state block can fill (SPEC U.1)
+      i.spect_size = 0;
+      if (i.spectsrc_id || i.est_mask) {
+        const size_t n_ch = hops_per_block * (info.size / 2);
+        uint32_t ns = 4096;
+        while (ns >= 64 && (size_t) ns + 1 > n_ch) ns >>= 1;
+        if (ns >= 64) {
+          i.spect_size = ns;
+          sdb_engine_set_spectrum_source(e.get(), h, (int) i.spectsrc_id, ns);
+          for (int k = 0; k < SDB_ESTIMATOR_COUNT; ++k)
+            if (i.est_mask & (1u << k)) sdb_engine_set_estimator(e.get(), h, k, 1);
+        }
+      }
+    }
+    if (parent < 0 && params.channel_update_int > 0)
+      sdb_engine_set_channel_detector(e.get(), params.detector_params.alpha, params.detector_params.beta,
+                                      params.detector_params.gamma,
+                                      params.detector_params.snr > 0 ? params.detector_params.snr : 4.0f, 2);
+    if (sdb_engine_commit(e.get())) return nullptr;
+    if (old && sdb_engine_same_geometry(e.get(), old))
+      sdb_engine_migrate_map(e.get(), old, old_of_new.data(), old_of_new.size());
+    return e;
+  }
+
+  // (re)plan the engines from the open inspectors at a block boundary.  A new engine takes over the running state of
+  // the one it replaces (sdb_engine_migrate_map): input history, DC estimate, and for every inspector that stays open
+  // its cross-fade tail, LO phase and loop state -- opening, closing, retuning or reconfiguring ONE inspector leaves
+  // the sample streams of the others untouched (suscan keeps them running too, Suscan/Analyzer.cpp:459-537).  The old
+  // engines are released only once every new level has migrated from them.  Returns false when the baseband engine
+  // cannot be planned (sdb_last_error() says why).
   bool rebuild()
   {
-    sdb_engine_t *old = eng; eng = nullptr;
+    EnginePtr old = std::move(eng);
     std::vector<Sub> old_subs; old_subs.swap(subs);
     std::vector<int> old_handle(insps.size(), -1);
-    for (size_t q = 0; q < insps.size(); ++q) old_handle[q] = insps[q].engine_handle;
-    auto drop_old = [&] { if (old) sdb_engine_destroy(old); for (auto &s : old_subs) if (s.eng) sdb_engine_destroy(s.eng); };
+    for (size_t q = 0; q < insps.size(); ++q) { old_handle[q] = insps[q].engine_handle; insps[q].engine_handle = -1; }
     sdb_engine_params ep;
     memset(&ep, 0, sizeof(ep));
     ep.n_streams = 1;
@@ -215,111 +314,27 @@ struct sdb_analyzer {
     ep.device = src.device;
     ep.flags = (iq_reverse ? SDB_FLAG_IQ_REVERSE : 0) | (dc_remove ? SDB_FLAG_DC_REMOVE : 0);
     ep.input_format = src.read || dec ? SDB_FORMAT_FLOAT32 : src.input_format;
-    eng = sdb_engine_new(&ep, rate);
-    if (!eng) { drop_old(); post_status(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INIT, SDB_ANALYZER_INIT_FAILURE, sdb_last_error()); return false; }
-    std::vector<int32_t> old_of_new;
-    for (auto &i : insps) {
-      i.engine_handle = -1;
-      if (!i.open || i.parent >= 0) continue;
-      sdb_channel_params cp;
-      double f = fmod(i.channel.fc / rate + 1.0, 1.0);
-      cp.f0 = (float) (2.0 * 3.14159265358979323846 * f);
-      cp.bw = (float) (2.0 * 3.14159265358979323846 * (i.channel.f_hi - i.channel.f_lo) / rate);
-      cp.guard = 1.0f; cp.precise = i.precise;
-      sdb_channel_info info;
-      int h = sdb_engine_open_channel(eng, &cp, &info);
-      if (h < 0) continue;
-      i.engine_handle = h;
-      old_of_new.push_back(old_handle[(size_t) i.handle]);
-      i.size = info.size;
-      i.fs = (float) (rate / info.decimation);
-      i.bandwidth = (float) (i.channel.f_hi - i.channel.f_lo);
-      i.lo = (float) i.channel.fc;
-      i.cfg.insp_class = i.cls;
-      sdb_engine_set_inspector(eng, h, &i.cfg);
-      // spectrum source / estimators: the largest frame (<= 4096) a steady-state block can fill (SPEC U.1)
-      i.spect_size = 0;
-      if (i.spectsrc_id || i.est_mask) {
-        const size_t n_ch = block / (ep.psd_size / 2) * (info.size / 2);
-        uint32_t ns = 4096;
-        while (ns >= 64 && (size_t) ns + 1 > n_ch) ns >>= 1;
-        if (ns >= 64) {
-          i.spect_size = ns;
-          sdb_engine_set_spectrum_source(eng, h, (int) i.spectsrc_id, ns);
-          for (int e = 0; e < SDB_ESTIMATOR_COUNT; ++e)
-            if (i.est_mask & (1u << e)) sdb_engine_set_estimator(eng, h, e, 1);
-        }
-      }
-    }
-    if (params.channel_update_int > 0)
-      sdb_engine_set_channel_detector(eng, params.detector_params.alpha, params.detector_params.beta,
-                                      params.detector_params.gamma,
-                                      params.detector_params.snr > 0 ? params.detector_params.snr : 4.0f, 2);
-    if (sdb_engine_commit(eng)) {
-      drop_old();
-      post_status(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INIT, SDB_ANALYZER_INIT_FAILURE, sdb_last_error());
-      return false;
-    }
-    if (old && sdb_engine_same_geometry(eng, old))
-      sdb_engine_migrate_map(eng, old, old_of_new.data(), old_of_new.size());
+    eng = plan_level(ep, rate, -1, old_handle, old.get());
+    if (!eng) return false;
     // sub-carrier engines: one per inspector that has open children, parents before children (an inspector's handle
     // is larger than its parent's, so one pass in handle order visits every parent after it was planned itself).
     // Every level runs the same number of hops per block: a child's window is its parent's channel size.
     const size_t hops_per_block = block / (ep.psd_size / 2);
-    for (size_t pi = 0; pi < insps.size(); ++pi) {
-      Insp &p = insps[pi];
-      if (!p.open || p.engine_handle < 0) continue;
-      bool any = false;
-      for (auto &c : insps) any = any || (c.open && c.parent == p.handle);
-      if (!any || p.size < 16) continue;
+    for (const Insp &p : insps) {
+      if (!p.open || p.engine_handle < 0 || p.size < 16) continue;
+      if (std::none_of(insps.begin(), insps.end(), [&](const Insp &c) { return c.open && c.parent == p.handle; }))
+        continue;
       sdb_engine_params sp;
       memset(&sp, 0, sizeof(sp));
       sp.n_streams = 1; sp.psd_size = 0; sp.st_window_size = p.size;
       sp.max_feed = (uint32_t) (hops_per_block * (p.size / 2));
       sp.device = src.device; sp.input_format = SDB_FORMAT_FLOAT32;
-      sdb_engine_t *se = sdb_engine_new(&sp, (double) p.fs);
-      if (!se) continue;
-      std::vector<int32_t> sub_old_of_new;
-      for (auto &c : insps) {
-        if (!c.open || c.parent != p.handle) continue;
-        sdb_channel_params cp;
-        cp.f0 = (float) (2.0 * 3.14159265358979323846 * fmod(c.channel.fc / (double) p.fs + 1.0, 1.0));
-        cp.bw = (float) (2.0 * 3.14159265358979323846 * (c.channel.f_hi - c.channel.f_lo) / (double) p.fs);
-        cp.guard = 1.0f; cp.precise = c.precise;
-        sdb_channel_info info;
-        int h = sdb_engine_open_channel(se, &cp, &info);
-        if (h < 0) continue;
-        c.engine_handle = h; c.size = info.size;
-        sub_old_of_new.push_back(old_handle[(size_t) c.handle]);
-        c.fs = (float) ((double) p.fs / info.decimation);
-        c.bandwidth = (float) (c.channel.f_hi - c.channel.f_lo); c.lo = (float) c.channel.fc;
-        c.cfg.insp_class = c.cls;
-        sdb_engine_set_inspector(se, h, &c.cfg);
-        // spectrum source / estimators of a sub-carrier inspector: as for a baseband one (SPEC U.1)
-        c.spect_size = 0;
-        if (c.spectsrc_id || c.est_mask) {
-          const size_t n_ch = hops_per_block * (info.size / 2);
-          uint32_t ns = 4096;
-          while (ns >= 64 && (size_t) ns + 1 > n_ch) ns >>= 1;
-          if (ns >= 64) {
-            c.spect_size = ns;
-            sdb_engine_set_spectrum_source(se, h, (int) c.spectsrc_id, ns);
-            for (int e = 0; e < SDB_ESTIMATOR_COUNT; ++e)
-              if (c.est_mask & (1u << e)) sdb_engine_set_estimator(se, h, e, 1);
-          }
-        }
-      }
-      if (sdb_engine_commit(se)) {
-        sdb_engine_destroy(se);
-        for (auto &c : insps) if (c.open && c.parent == p.handle) c.engine_handle = -1;
-        continue;
-      }
-      for (auto &os : old_subs)
-        if (os.parent == p.handle && os.eng && sdb_engine_same_geometry(se, os.eng))
-          sdb_engine_migrate_map(se, os.eng, sub_old_of_new.data(), sub_old_of_new.size());
-      subs.push_back(Sub{ p.handle, se });
+      sdb_engine_t *old_sub = nullptr;
+      for (auto &os : old_subs) if (os.parent == p.handle) old_sub = os.eng.get();
+      EnginePtr se = plan_level(sp, (double) p.fs, p.handle, old_handle, old_sub);
+      if (se) subs.push_back(Sub{ p.handle, std::move(se) });
+      else for (auto &c : insps) if (c.open && c.parent == p.handle) c.engine_handle = -1;
     }
-    drop_old();
     plan_dirty = false;
     return true;
   }
@@ -339,36 +354,29 @@ struct sdb_analyzer {
           double in_rate = rate;
           uint32_t in_window = (uint32_t) params.detector_params.window_size;
           if (c.parent >= 0) {
-            if (c.parent >= (int32_t) insps.size() || !insps[c.parent].open || insps[c.parent].size < 16) {
+            const Insp *p = open_insp(c.parent);
+            if (!p || p->size < 16) {
               Cmd w = c; w.handle = c.parent;
               post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_HANDLE, w, nullptr); break;
             }
-            in_rate = (double) insps[c.parent].fs; in_window = insps[c.parent].size;
+            in_rate = (double) p->fs; in_window = p->size;
           }
           if (!(bw > 0) || bw > in_rate || fabs(c.channel.fc) > in_rate / 2) {
+            post_inspector(SDB_INSPECTOR_MSGKIND_INVALID_CHANNEL, c, nullptr); break;
+          }
+          // geometry -> equivalent rate, needed for the default config the OPEN reply carries; the engine's
+          // shared-memory channel IFFT takes at most 16384 bins
+          const sdb_channel_params cp = channel_params(c.channel, in_rate, c.precise);
+          sdb_channel_info info;
+          if (sdb_channel_geometry(in_window, &cp, &info) || info.size > 16384) {
             post_inspector(SDB_INSPECTOR_MSGKIND_INVALID_CHANNEL, c, nullptr); break;
           }
           Insp i;
           memset(&i, 0, sizeof(i));
           i.handle = (int32_t) insps.size(); i.open = true; i.has_id = false; i.cls = cls; i.channel = c.channel;
           i.precise = c.precise; i.engine_handle = -1; i.parent = c.parent;
-          // geometry -> equivalent rate, needed for the default config the OPEN reply carries
-          {
-            sdb_engine_params ep; memset(&ep, 0, sizeof(ep));
-            ep.n_streams = 1; ep.psd_size = c.parent >= 0 ? 0 : in_window; ep.st_window_size = in_window;
-            ep.max_feed = c.parent >= 0 ? in_window : (uint32_t) block;
-            ep.device = src.device;
-            sdb_engine_t *probe = sdb_engine_new(&ep, in_rate);
-            sdb_channel_params cp;
-            cp.f0 = (float) (2.0 * 3.14159265358979323846 * fmod(c.channel.fc / in_rate + 1.0, 1.0));
-            cp.bw = (float) (2.0 * 3.14159265358979323846 * bw / in_rate); cp.guard = 1.0f; cp.precise = c.precise;
-            sdb_channel_info info; memset(&info, 0, sizeof(info));
-            int h = probe ? sdb_engine_open_channel(probe, &cp, &info) : -1;
-            if (probe) sdb_engine_destroy(probe);
-            if (h < 0) { post_inspector(SDB_INSPECTOR_MSGKIND_INVALID_CHANNEL, c, nullptr); break; }
-            i.fs = (float) (in_rate / info.decimation);
-            i.size = info.size;
-          }
+          i.fs = (float) (in_rate / info.decimation);
+          i.size = info.size;
           i.bandwidth = (float) bw; i.lo = (float) c.channel.fc;
           sdb_inspector_config_default(&i.cfg, cls, i.fs);
           i.cfg.clock_running = 0;       // "by default ... no samples are being delivered" (manual p.62)
@@ -382,10 +390,9 @@ struct sdb_analyzer {
         case Cmd::SET_SPECTRUM:
         case Cmd::ESTIMATOR_CMD:
         case Cmd::CLOSE: {
-          if (c.handle < 0 || c.handle >= (int32_t) insps.size() || !insps[c.handle].open) {
-            post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_HANDLE, c, nullptr); break;
-          }
-          Insp &i = insps[c.handle];
+          Insp *ip = open_insp(c.handle);
+          if (!ip) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_HANDLE, c, nullptr); break; }
+          Insp &i = *ip;
           if (c.kind == Cmd::SET_SPECTRUM) {
             if (c.aux_id >= (uint32_t) SDB_SPECTSRC_COUNT) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, c, nullptr); break; }
             i.spectsrc_id = c.aux_id; plan_dirty = true;
@@ -411,9 +418,7 @@ struct sdb_analyzer {
           break;
         }
         case Cmd::SET_WATERMARK:
-          if (c.handle < 0 || c.handle >= (int32_t) insps.size() || !insps[c.handle].open) {
-            post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_HANDLE, c, nullptr); break;
-          }
+          if (!open_insp(c.handle)) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_HANDLE, c, nullptr); break; }
           pending[c.handle].watermark = (uint64_t) c.value;
           break;
         case Cmd::SET_HISTORY:
@@ -443,8 +448,9 @@ struct sdb_analyzer {
         case Cmd::SET_BANDWIDTH: {
           // "overridable" setters (Suscan/Analyzer.cpp:509-526): no reply; the latest value wins.  The channel is
           // re-planned at the next block boundary (see the a18 limits in DESIGN.md).
-          if (c.handle < 0 || c.handle >= (int32_t) insps.size() || !insps[c.handle].open) break;
-          Insp &i = insps[c.handle];
+          Insp *ip = open_insp(c.handle);
+          if (!ip) break;
+          Insp &i = *ip;
           const double in_rate = i.parent >= 0 ? (double) insps[i.parent].fs : rate;
           if (c.kind == Cmd::SET_FREQ) {
             if (fabs(c.value) > in_rate / 2) break;
@@ -484,7 +490,7 @@ struct sdb_analyzer {
     if (src.read) return src.read(src.priv, dst, n);
     if (!src.data) return -1;
     // in-memory capture in its native sample format (bps bytes per IQ pair); dst is a byte buffer of n * 8
-    const size_t bps = src.input_format == SDB_FORMAT_FLOAT32 ? 8 : src.input_format == SDB_FORMAT_SIGNED16 ? 4 : 2;
+    const size_t bps = src_bytes();
     const unsigned char *base = reinterpret_cast<const unsigned char *>(src.data);
     unsigned char *out = reinterpret_cast<unsigned char *>(dst);
     size_t got = 0;
@@ -527,289 +533,276 @@ struct sdb_analyzer {
     return hop_min + u * (hop_max - hop_min);
   }
 
-  void run_wide()
+  // one sweep of HB hops
+  bool sweep()
   {
-    const size_t HB = 16;
-    uint32_t exit_type = SDB_WORKER_MSG_TYPE_HALT;
-    std::vector<sdb_complex> buf, drop;
-    std::vector<float> psd;
-    std::vector<double> fcs(HB);
-    hop_min = params.min_freq; hop_max = params.max_freq;
-    for (;;) {
-      { std::lock_guard<std::mutex> l(cmd_m); if (halt_req) break; }
-      handle_cmds();
-      const size_t N = (size_t) params.detector_params.window_size;
-      if (plan_dirty) {
-        if (eng) { sdb_engine_destroy(eng); eng = nullptr; }
-        sdb_engine_params ep;
-        memset(&ep, 0, sizeof(ep));
-        ep.n_streams = (uint32_t) HB; ep.psd_size = (uint32_t) N; ep.psd_window = params.detector_params.window;
-        ep.max_feed = (uint32_t) N; ep.device = src.device;
-        ep.flags = iq_reverse ? SDB_FLAG_IQ_REVERSE : 0;
-        ep.input_format = src.read ? SDB_FORMAT_FLOAT32 : src.input_format;   // in-memory captures keep their format
-        eng = sdb_engine_new(&ep, src.samp_rate);
-        if (!eng || sdb_engine_commit(eng)) {
-          post_status(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INIT, SDB_ANALYZER_INIT_FAILURE, sdb_last_error());
-          exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
-        }
-        plan_dirty = false;
-      }
-      // hops are packed back to back in the source's native sample format: bps bytes per IQ pair
-      const size_t bps = src.read || src.input_format == SDB_FORMAT_FLOAT32 ? 8
-                         : src.input_format == SDB_FORMAT_SIGNED16 ? 4 : 2;
-      unsigned char *bytes = nullptr;
-      buf.resize(HB * N);
-      bytes = reinterpret_cast<unsigned char *>(buf.data());
-      size_t got_hops = 0;
-      bool eos = false, err = false;
-      for (size_t h = 0; h < HB && !eos && !err; ++h) {
-        fcs[h] = next_hop();
-        if (src.set_frequency && src.set_frequency(src.priv, fcs[h]) != 0) { err = true; break; }
-        for (uint64_t left = buffering; left > 0 && !eos && !err;) {          // the tuner's round trip
-          const size_t take = (size_t) std::min<uint64_t>(left, 65536);
-          drop.resize(take);
-          const long g = source_read(drop.data(), take);
-          if (g < 0) err = true; else if ((size_t) g < take) eos = true;
-          left -= take;
-        }
-        if (eos || err) break;
-        const long g = source_read(reinterpret_cast<sdb_complex *>(bytes + h * N * bps), N);
-        if (g < 0) err = true; else if ((size_t) g < N) eos = true; else ++got_hops;
-      }
-      if (err) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
-      if (got_hops) {
-        for (size_t h = got_hops; h < HB; ++h)
-          memset(bytes + h * N * bps, src.input_format == SDB_FORMAT_UNSIGNED8 && !src.read ? 0x80 : 0, N * bps);
-        if (sdb_engine_feed_host(eng, buf.data(), N, N) || sdb_engine_sync(eng)) {
-          exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
-        }
-        psd.resize(HB * N);
-        if (sdb_engine_read_psd(eng, psd.data(), psd.size())) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
-        for (size_t h = 0; h < got_hops; ++h) {
-          sdb_analyzer_psd_msg *m = (sdb_analyzer_psd_msg *) calloc(1, sizeof(*m));
-          m->fc = (int64_t) llround(fcs[h]); m->samp_rate = (float) src.samp_rate;
-          m->measured_samp_rate = (float) measured_rate.load();
-          gettimeofday(&m->rt_time, nullptr);
-          m->psd_size = N;
-          m->psd_data = (float *) malloc(N * sizeof(float));
-          memcpy(m->psd_data, &psd[h * N], N * sizeof(float));
-          post(SDB_ANALYZER_MESSAGE_TYPE_PSD, m);
-        }
-        total_samples += got_hops * (N + buffering);
-      }
-      if (eos) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_EOS; break; }
+    const size_t HB = 16, N = (size_t) params.detector_params.window_size;
+    if (plan_dirty) {
+      eng.reset();
+      sdb_engine_params ep;
+      memset(&ep, 0, sizeof(ep));
+      ep.n_streams = (uint32_t) HB; ep.psd_size = (uint32_t) N; ep.psd_window = params.detector_params.window;
+      ep.max_feed = (uint32_t) N; ep.device = src.device;
+      ep.flags = iq_reverse ? SDB_FLAG_IQ_REVERSE : 0;
+      ep.input_format = src.read ? SDB_FORMAT_FLOAT32 : src.input_format;   // in-memory captures keep their format
+      eng.reset(sdb_engine_new(&ep, src.samp_rate));
+      if (!eng || sdb_engine_commit(eng.get())) return init_failure();
+      plan_dirty = false;
     }
-    if (eng) { sdb_engine_destroy(eng); eng = nullptr; }
-    post_status(exit_type, 0, exit_type == SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR ? sdb_last_error() : nullptr);
+    // hops are packed back to back in the source's native sample format: bps bytes per IQ pair
+    const size_t bps = src_bytes();
+    double fcs[HB];
+    buf.resize(HB * N);
+    unsigned char *bytes = reinterpret_cast<unsigned char *>(buf.data());
+    size_t got_hops = 0;
+    bool eos = false, err = false;
+    for (size_t h = 0; h < HB && !eos && !err; ++h) {
+      fcs[h] = next_hop();
+      if (src.set_frequency && src.set_frequency(src.priv, fcs[h]) != 0) { err = true; break; }
+      for (uint64_t left = buffering; left > 0 && !eos && !err;) {          // the tuner's round trip
+        const size_t take = (size_t) std::min<uint64_t>(left, 65536);
+        drop.resize(take);
+        const long g = source_read(drop.data(), take);
+        if (g < 0) err = true; else if ((size_t) g < take) eos = true;
+        left -= take;
+      }
+      if (eos || err) break;
+      const long g = source_read(reinterpret_cast<sdb_complex *>(bytes + h * N * bps), N);
+      if (g < 0) err = true; else if ((size_t) g < N) eos = true; else ++got_hops;
+    }
+    if (err) return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+    if (got_hops) {
+      for (size_t h = got_hops; h < HB; ++h)
+        memset(bytes + h * N * bps, src.input_format == SDB_FORMAT_UNSIGNED8 && !src.read ? 0x80 : 0, N * bps);
+      if (sdb_engine_feed_host(eng.get(), buf.data(), N, N) || sdb_engine_sync(eng.get()))
+        return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+      psd.resize(HB * N);
+      if (sdb_engine_read_psd(eng.get(), psd.data(), psd.size())) return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+      for (size_t h = 0; h < got_hops; ++h) post_psd((int64_t) llround(fcs[h]), src.samp_rate, &psd[h * N], N, 0, 0, 0);
+      total_samples += got_hops * (N + buffering);
+    }
+    if (eos) return stop(SDB_ANALYZER_MESSAGE_TYPE_EOS);
+    return true;
+  }
+
+  // ---------------------------------------------------------------------------------------------------------
+  // SUSCAN_ANALYZER_MODE_CHANNEL: one block per step
+  // ---------------------------------------------------------------------------------------------------------
+  // one block into buf, or left in the decimator's device output (on_device)
+  bool read_block(bool &on_device)
+  {
+    if (replaying && hist_fill > 0) {
+      // suscan_analyzer_replay: the source is paused and the history ring is played back, oldest sample first
+      for (size_t i = 0; i < block; ++i) {
+        if (replay_pos == 0 && replay_wrapped) looped = 1;         // playing the ring for the second time
+        buf[i] = hist[(hist_start + replay_pos) % hist.size()];
+        if (++replay_pos >= hist_fill) { replay_pos = 0; replay_wrapped = true; }
+      }
+      return true;
+    }
+    long got;
+    if (dec) {
+      // SPEC L: block * decim source samples in their native format -> block float32 samples at `rate`.  Baseband
+      // filters and the history see the decimated samples on the host; otherwise the engine reads them in place.
+      const long g = source_read(raw.data(), block * decim);
+      got = g < 0 ? g : g / (long) decim;
+      if (got == (long) block) {
+        if (sdb_decimator_feed_host(dec.get(), raw.data(), raw.size(), block * decim) != (long) block)
+          return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+        bool host = !hist.empty();
+        { std::lock_guard<std::mutex> l(cmd_m); host = host || !bb_filters.empty(); }
+        if (!host) {
+          if (sdb_decimator_sync(dec.get())) return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+          on_device = true;
+        } else if (sdb_decimator_read(dec.get(), buf.data(), buf.size())) {
+          return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+        }
+      }
+    } else {
+      got = source_read(buf.data(), block);
+    }
+    if (got == (long) block && f32_src() && !hist.empty()) {       // suscan_analyzer_set_history_size: keep the tail
+      for (size_t i = 0; i < block; ++i) {
+        hist[(hist_start + hist_fill) % hist.size()] = buf[i];
+        if (hist_fill < hist.size()) ++hist_fill; else hist_start = (hist_start + 1) % hist.size();
+      }
+    }
+    if (got < 0) return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+    if ((size_t) got < block) return stop(SDB_ANALYZER_MESSAGE_TYPE_EOS);   // partial tail blocks are dropped
+    return true;
+  }
+
+  // baseband filters see (and may rewrite) every float32 block before the analyzer does, in registration order;
+  // with decimation the block and the offset are at the decimated rate
+  bool run_filters(bool &on_device)
+  {
+    if (!f32_src()) return true;
+    const std::vector<BbFilter> fl = [&] { std::lock_guard<std::mutex> l(cmd_m); return bb_filters; }();
+    if (on_device && !fl.empty()) {                  // a filter registered while the block was being read
+      if (sdb_decimator_read(dec.get(), buf.data(), buf.size())) return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+      on_device = false;
+    }
+    for (auto &f : fl) f.fn(f.priv, this, buf.data(), (uint64_t) block, total_samples / decim);
+    return true;
+  }
+
+  bool feed(bool on_device)
+  {
+    const int fed = on_device ? sdb_engine_feed_device(eng.get(), sdb_decimator_output_device(dec.get()), block, block)
+                              : sdb_engine_feed_host(eng.get(), buf.data(), block, block);
+    if (fed || sdb_engine_sync(eng.get())) return stop(SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR);
+    total_samples += block * decim;                   // source samples
+    total_samples_pub.store(total_samples);
+    return true;
+  }
+
+  void pace()
+  {
+    if (throttle > 0) {                                // suscan_analyzer_set_throttle_async: pace to `throttle` samples/s
+      const double due = (double) (total_samples - throttle_s0) / throttle;
+      const double now = std::chrono::duration<double>(std::chrono::steady_clock::now() - throttle_t0).count();
+      if (due > now) std::this_thread::sleep_for(std::chrono::duration<double>(due - now));
+    }
+    double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    measured_rate.store(el > 0 ? (double) total_samples / el : 0);
+  }
+
+  // PSD messages at psd_update_int cadence of SIGNAL time (coverage = N / (fs * interval))
+  void publish_psd()
+  {
+    const size_t N = (size_t) params.detector_params.window_size, frames = block / N;
+    psd.resize(frames * N);
+    if (sdb_engine_read_psd(eng.get(), psd.data(), psd.size())) return;
+    const double per_frame = (double) N / rate;
+    for (size_t f = 0; f < frames; ++f) {
+      psd_credit += per_frame;
+      if (psd_credit + 1e-12 >= params.psd_update_int) {
+        psd_credit = params.psd_update_int > 0 ? fmod(psd_credit, params.psd_update_int) : 0;
+        post_psd((int64_t) src.freq, rate, &psd[f * N], N,
+                 (double) (total_samples - block * decim + f * N * decim) / src.samp_rate, looped, (uint64_t) hist_fill);
+      }
+    }
+  }
+
+  void deliver_symbols(sdb_engine_t *e, const Insp &i, size_t cap)
+  {
+    if (!i.has_id || i.engine_handle < 0) return;
+    soft.resize(cap); hard.resize(cap);
+    long n = sdb_engine_read_symbols(e, 0, i.engine_handle, soft.data(), hard.data(), cap);
+    if (n > 0) deliver(i, soft.data(), hard.data(), (size_t) n, false);
+  }
+
+  // sample batches, keyed by the caller-chosen inspector_id
+  // sub-carrier inspectors: the parent's channel samples of this block through the child engine.  `subs` is in
+  // parent-before-child order (rebuild), so a nested parent's engine has been fed by the time it is read.
+  void publish_symbols()
+  {
+    for (auto &sb : subs) {
+      const Insp &p = insps[sb.parent];
+      sdb_engine_t *host = engine_of(p);
+      if (!p.open || p.engine_handle < 0 || !host) continue;
+      std::vector<sdb_complex> ch(block);
+      long nch = sdb_engine_read_channel(host, 0, p.engine_handle, ch.data(), ch.size());
+      if (nch <= 0) continue;
+      if (sdb_engine_feed_host(sb.eng.get(), ch.data(), (size_t) nch, (size_t) nch) || sdb_engine_sync(sb.eng.get())) continue;
+      for (auto &i : insps) if (i.open && i.parent == p.handle) deliver_symbols(sb.eng.get(), i, (size_t) nch);
+    }
+    for (auto &i : insps) if (i.open && i.parent < 0) deliver_symbols(eng.get(), i, block);
+  }
+
+  // kind=SPECTRUM / kind=ESTIMATOR inspector messages (one per block that filled a frame)
+  void publish_spectra()
+  {
+    for (auto &i : insps) {
+      sdb_engine_t *ie = engine_of(i);
+      if (!i.open || i.engine_handle < 0 || !i.spect_size || !ie) continue;
+      if (i.spectsrc_id) {
+        std::vector<float> sp(i.spect_size);
+        uint32_t emitted = 0;
+        if (sdb_engine_read_spectrum(ie, i.engine_handle, sp.data(), &emitted) == 0 && emitted) {
+          sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_SPECTRUM, i.handle, i.inspector_id,
+                                                        kClassNames[i.cls]);
+          m->spectsrc_id = i.spectsrc_id; m->spectrum_size = emitted; m->samp_rate = (uint64_t) i.fs;
+          m->fs = (float) rate; m->equiv_fs = i.fs;
+          m->spectrum_data = (float *) malloc(emitted * sizeof(float));
+          memcpy(m->spectrum_data, sp.data(), emitted * sizeof(float));
+          post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
+        }
+      }
+      for (int e = 0; e < SDB_ESTIMATOR_COUNT; ++e) {
+        if (!(i.est_mask & (1u << e))) continue;
+        float v = 0; int32_t ok = 0;
+        if (sdb_engine_read_estimate(ie, i.engine_handle, e, &v, &ok) == 0 && ok) {
+          sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_ESTIMATOR, i.handle, i.inspector_id,
+                                                        kClassNames[i.cls]);
+          m->estimator_id = (uint32_t) e; m->enabled = 1; m->value = v;
+          post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
+        }
+      }
+    }
+  }
+
+  // MESSAGE_TYPE_CHANNEL at channel_update_int cadence of signal time
+  void publish_channels()
+  {
+    if (!(params.channel_update_int > 0)) return;
+    chan_credit += (double) block / rate;
+    if (chan_credit + 1e-12 >= params.channel_update_int) {
+      chan_credit = fmod(chan_credit, params.channel_update_int);
+      std::vector<sdb_detected_channel> ch(256);
+      uint32_t total = 0;
+      long nc = sdb_engine_read_channels(eng.get(), 0, src.freq, ch.data(), ch.size(), &total);
+      if (nc >= 0) {
+        sdb_analyzer_channel_msg *m = (sdb_analyzer_channel_msg *) calloc(1, sizeof(*m));
+        m->channel_count = (uint32_t) nc;
+        m->channel_list = (sdb_detected_channel *) malloc(std::max<long>(1, nc) * sizeof(sdb_detected_channel));
+        memcpy(m->channel_list, ch.data(), (size_t) nc * sizeof(sdb_detected_channel));
+        post(SDB_ANALYZER_MESSAGE_TYPE_CHANNEL, m);
+      }
+    }
+  }
+
+  // re-plan, read, baseband filters, feed, pacing, then the block's messages
+  bool step()
+  {
+    const size_t N = (size_t) params.detector_params.window_size;
+    if (block % N) block = std::max<size_t>(N, (block / N) * N);     // after a PARAMS change
+    if (buf.size() != block) buf.resize(block);
+    if (decim > 1 && raw.size() < block * decim) {    // first block, or a PARAMS change that grew the block
+      dec.reset();
+      raw.resize(block * decim);
+      dec.reset(sdb_decimator_new(src.device, 1, decim, src.read ? SDB_FORMAT_FLOAT32 : src.input_format, raw.size()));
+      if (!dec) return init_failure();
+    }
+    if (plan_dirty && !rebuild()) return init_failure();
+    bool on_device = false;                      // the decimated block is only in the decimator's device output
+    if (!read_block(on_device) || !run_filters(on_device) || !feed(on_device)) return false;
+    pace();
+    publish_psd();
+    publish_symbols();
+    publish_spectra();
+    publish_channels();
+    return true;
   }
 
   void run()
   {
-    std::vector<sdb_complex> buf(block);
-    std::vector<float> psd;
-    std::vector<sdb_complex> soft;
-    std::vector<uint8_t> hard;
-    if (params.mode == SDB_ANALYZER_MODE_WIDE_SPECTRUM) {
-      sdb_source_info *si = (sdb_source_info *) calloc(1, sizeof(*si));
-      si->source_samp_rate = (uint64_t) src.samp_rate; si->effective_samp_rate = (uint64_t) src.samp_rate;
-      si->frequency = src.freq; si->seekable = 0;
-      post(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INFO, si);
-      run_wide();
-      return;
-    }
-    {
-      sdb_source_info *si = (sdb_source_info *) calloc(1, sizeof(*si));
-      si->source_samp_rate = (uint64_t) src.samp_rate; si->effective_samp_rate = (uint64_t) rate;
-      si->measured_samp_rate = 0; si->frequency = src.freq; si->seekable = src.read ? 0 : 1;
-      post(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INFO, si);
-    }
-    auto t0 = std::chrono::steady_clock::now();
-    uint32_t exit_type = SDB_WORKER_MSG_TYPE_HALT;
+    // the mode is the one the analyzer was created with: a later SET_PARAMS does not switch it
+    const bool wide = params.mode == SDB_ANALYZER_MODE_WIDE_SPECTRUM;
+    sdb_source_info *si = (sdb_source_info *) calloc(1, sizeof(*si));
+    si->source_samp_rate = (uint64_t) src.samp_rate; si->effective_samp_rate = (uint64_t) rate;
+    si->frequency = src.freq; si->seekable = !wide && !src.read;
+    post(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INFO, si);
+    if (wide) { hop_min = params.min_freq; hop_max = params.max_freq; }
+    t0 = std::chrono::steady_clock::now();
     for (;;) {
       { std::lock_guard<std::mutex> l(cmd_m); if (halt_req) break; }
       handle_cmds();
-      const size_t N = (size_t) params.detector_params.window_size;
-      if (block % N) block = std::max<size_t>(N, (block / N) * N);     // after a PARAMS change
-      if (buf.size() != block) buf.resize(block);
-      if (decim > 1 && raw.size() < block * decim) {    // first block, or a PARAMS change that grew the block
-        if (dec) sdb_decimator_destroy(dec);
-        raw.resize(block * decim);
-        dec = sdb_decimator_new(src.device, 1, decim, src.read ? SDB_FORMAT_FLOAT32 : src.input_format, raw.size());
-        if (!dec) {
-          post_status(SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INIT, SDB_ANALYZER_INIT_FAILURE, sdb_last_error());
-          exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
-        }
-      }
-      if (plan_dirty && !rebuild()) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
-      long got;
-      const bool f32_src = src.read || src.input_format == SDB_FORMAT_FLOAT32 || dec;
-      bool on_device = false;                      // the decimated block is only in the decimator's device output
-      if (replaying && hist_fill > 0) {
-        // suscan_analyzer_replay: the source is paused and the history ring is played back, oldest sample first
-        for (size_t i = 0; i < block; ++i) {
-          if (replay_pos == 0 && replay_wrapped) looped = 1;         // playing the ring for the second time
-          buf[i] = hist[(hist_start + replay_pos) % hist.size()];
-          if (++replay_pos >= hist_fill) { replay_pos = 0; replay_wrapped = true; }
-        }
-        got = (long) block;
-      } else {
-        if (dec) {
-          // SPEC L: block * decim source samples in their native format -> block float32 samples at `rate`.  Baseband
-          // filters and the history see the decimated samples on the host; otherwise the engine reads them in place.
-          const long g = source_read(raw.data(), block * decim);
-          got = g < 0 ? g : g / (long) decim;
-          if (got == (long) block) {
-            if (sdb_decimator_feed_host(dec, raw.data(), raw.size(), block * decim) != (long) block) {
-              exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
-            }
-            bool host = !hist.empty();
-            { std::lock_guard<std::mutex> l(cmd_m); host = host || !bb_filters.empty(); }
-            if (!host) {
-              if (sdb_decimator_sync(dec)) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
-              on_device = true;
-            } else if (sdb_decimator_read(dec, buf.data(), buf.size())) {
-              exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
-            }
-          }
-        } else {
-          got = source_read(buf.data(), block);
-        }
-        if (got == (long) block && f32_src && !hist.empty()) {       // suscan_analyzer_set_history_size: keep the tail
-          for (size_t i = 0; i < block; ++i) {
-            hist[(hist_start + hist_fill) % hist.size()] = buf[i];
-            if (hist_fill < hist.size()) ++hist_fill; else hist_start = (hist_start + 1) % hist.size();
-          }
-        }
-      }
-      if (got < 0) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
-      if ((size_t) got < block) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_EOS; break; }   // partial tail blocks are dropped
-      // baseband filters see (and may rewrite) every float32 block before the analyzer does, in registration order;
-      // with decimation the block and the offset are at the decimated rate
-      if (f32_src) {
-        std::vector<BbFilter> fl;
-        { std::lock_guard<std::mutex> l(cmd_m); fl = bb_filters; }
-        if (on_device && !fl.empty()) {                  // a filter registered while the block was being read
-          if (sdb_decimator_read(dec, buf.data(), buf.size())) { exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break; }
-          on_device = false;
-        }
-        for (auto &f : fl) f.fn(f.priv, this, buf.data(), (uint64_t) block, total_samples / decim);
-      }
-      const int fed = on_device ? sdb_engine_feed_device(eng, sdb_decimator_output_device(dec), block, block)
-                                : sdb_engine_feed_host(eng, buf.data(), block, block);
-      if (fed || sdb_engine_sync(eng)) {
-        exit_type = SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR; break;
-      }
-      total_samples += block * decim;                   // source samples
-      total_samples_pub.store(total_samples);
-      if (throttle > 0) {                                // suscan_analyzer_set_throttle_async: pace to `throttle` samples/s
-        const double due = (double) (total_samples - throttle_s0) / throttle;
-        const double now = std::chrono::duration<double>(std::chrono::steady_clock::now() - throttle_t0).count();
-        if (due > now) std::this_thread::sleep_for(std::chrono::duration<double>(due - now));
-      }
-      double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      measured_rate.store(el > 0 ? (double) total_samples / el : 0);
-      // PSD messages at psd_update_int cadence of SIGNAL time (coverage = N / (fs * interval))
-      const size_t frames = block / N;
-      psd.resize(frames * N);
-      if (sdb_engine_read_psd(eng, psd.data(), psd.size()) == 0) {
-        const double per_frame = (double) N / rate;
-        for (size_t f = 0; f < frames; ++f) {
-          psd_credit += per_frame;
-          if (psd_credit + 1e-12 >= params.psd_update_int) {
-            psd_credit = params.psd_update_int > 0 ? fmod(psd_credit, params.psd_update_int) : 0;
-            sdb_analyzer_psd_msg *m = (sdb_analyzer_psd_msg *) calloc(1, sizeof(*m));
-            m->fc = (int64_t) src.freq; m->samp_rate = (float) rate; m->measured_samp_rate = (float) measured_rate.load();
-            gettimeofday(&m->rt_time, nullptr);
-            double ts = (double) (total_samples - block * decim + f * N * decim) / src.samp_rate;
-            m->timestamp.tv_sec = (time_t) ts; m->timestamp.tv_usec = (suseconds_t) ((ts - floor(ts)) * 1e6);
-            m->looped = looped; m->history_size = (uint64_t) hist_fill;
-            m->psd_size = N;
-            m->psd_data = (float *) malloc(N * sizeof(float));
-            memcpy(m->psd_data, &psd[f * N], N * sizeof(float));
-            post(SDB_ANALYZER_MESSAGE_TYPE_PSD, m);
-          }
-        }
-      }
-      // sample batches, keyed by the caller-chosen inspector_id
-      // sub-carrier inspectors: the parent's channel samples of this block through the child engine.  `subs` is in
-      // parent-before-child order (rebuild), so a nested parent's engine has been fed by the time it is read.
-      for (auto &sb : subs) {
-        const Insp &p = insps[sb.parent];
-        sdb_engine_t *host = engine_of(p);
-        if (!p.open || p.engine_handle < 0 || !host) continue;
-        std::vector<sdb_complex> ch(block);
-        long nch = sdb_engine_read_channel(host, 0, p.engine_handle, ch.data(), ch.size());
-        if (nch <= 0) continue;
-        if (sdb_engine_feed_host(sb.eng, ch.data(), (size_t) nch, (size_t) nch) || sdb_engine_sync(sb.eng)) continue;
-        for (auto &i : insps) {
-          if (!i.open || i.parent != p.handle || !i.has_id || i.engine_handle < 0) continue;
-          soft.resize((size_t) nch); hard.resize((size_t) nch);
-          long n = sdb_engine_read_symbols(sb.eng, 0, i.engine_handle, soft.data(), hard.data(), (size_t) nch);
-          if (n <= 0) continue;
-          deliver(i, soft.data(), hard.data(), (size_t) n, false);
-        }
-      }
-      for (auto &i : insps) {
-        if (!i.open || !i.has_id || i.engine_handle < 0 || i.parent >= 0) continue;
-        size_t cap = block;
-        soft.resize(cap); hard.resize(cap);
-        long n = sdb_engine_read_symbols(eng, 0, i.engine_handle, soft.data(), hard.data(), cap);
-        if (n <= 0) continue;
-        deliver(i, soft.data(), hard.data(), (size_t) n, false);
-      }
-      // kind=SPECTRUM / kind=ESTIMATOR inspector messages (one per block that filled a frame)
-      for (auto &i : insps) {
-        sdb_engine_t *ie = engine_of(i);
-        if (!i.open || i.engine_handle < 0 || !i.spect_size || !ie) continue;
-        if (i.spectsrc_id) {
-          std::vector<float> sp(i.spect_size);
-          uint32_t emitted = 0;
-          if (sdb_engine_read_spectrum(ie, i.engine_handle, sp.data(), &emitted) == 0 && emitted) {
-            sdb_analyzer_inspector_msg *m = (sdb_analyzer_inspector_msg *) calloc(1, sizeof(*m));
-            m->kind = SDB_INSPECTOR_MSGKIND_SPECTRUM; m->handle = i.handle; m->inspector_id = i.inspector_id;
-            m->class_name = dupstr((const char *[]){ "psk", "fsk", "ask", "audio", "raw" }[i.cls]);
-            m->spectsrc_id = i.spectsrc_id; m->spectrum_size = emitted; m->samp_rate = (uint64_t) i.fs;
-            m->fs = (float) rate; m->equiv_fs = i.fs;
-            m->spectrum_data = (float *) malloc(emitted * sizeof(float));
-            memcpy(m->spectrum_data, sp.data(), emitted * sizeof(float));
-            post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
-          }
-        }
-        for (int e = 0; e < SDB_ESTIMATOR_COUNT; ++e) {
-          if (!(i.est_mask & (1u << e))) continue;
-          float v = 0; int32_t ok = 0;
-          if (sdb_engine_read_estimate(ie, i.engine_handle, e, &v, &ok) == 0 && ok) {
-            sdb_analyzer_inspector_msg *m = (sdb_analyzer_inspector_msg *) calloc(1, sizeof(*m));
-            m->kind = SDB_INSPECTOR_MSGKIND_ESTIMATOR; m->handle = i.handle; m->inspector_id = i.inspector_id;
-            m->class_name = dupstr((const char *[]){ "psk", "fsk", "ask", "audio", "raw" }[i.cls]);
-            m->estimator_id = (uint32_t) e; m->enabled = 1; m->value = v;
-            post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
-          }
-        }
-      }
-      // MESSAGE_TYPE_CHANNEL at channel_update_int cadence of signal time
-      if (params.channel_update_int > 0) {
-        chan_credit += (double) block / rate;
-        if (chan_credit + 1e-12 >= params.channel_update_int) {
-          chan_credit = fmod(chan_credit, params.channel_update_int);
-          std::vector<sdb_detected_channel> ch(256);
-          uint32_t total = 0;
-          long nc = sdb_engine_read_channels(eng, 0, src.freq, ch.data(), ch.size(), &total);
-          if (nc >= 0) {
-            sdb_analyzer_channel_msg *m = (sdb_analyzer_channel_msg *) calloc(1, sizeof(*m));
-            m->channel_count = (uint32_t) nc;
-            m->channel_list = (sdb_detected_channel *) malloc(std::max<long>(1, nc) * sizeof(sdb_detected_channel));
-            memcpy(m->channel_list, ch.data(), (size_t) nc * sizeof(sdb_detected_channel));
-            post(SDB_ANALYZER_MESSAGE_TYPE_CHANNEL, m);
-          }
-        }
-      }
+      if (!(wide ? sweep() : step())) break;
     }
     for (auto &i : insps)                                // what the watermark still holds back goes out with the end
       if (i.has_id && pending.count(i.handle)) deliver(i, nullptr, nullptr, 0, true);
-    drop_subs();
-    if (eng) { sdb_engine_destroy(eng); eng = nullptr; }
-    if (dec) { sdb_decimator_destroy(dec); dec = nullptr; }
+    subs.clear(); eng.reset(); dec.reset();              // released before the exit status is posted
     post_status(exit_type, 0, exit_type == SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR ? sdb_last_error() : nullptr);
   }
 };
@@ -1046,8 +1039,9 @@ extern "C" int sdb_analyzer_get_inspector_config(sdb_analyzer_t *a, int32_t hand
 {
   if (!a || !cfg) return -1;
   std::lock_guard<std::mutex> l(a->insp_m);
-  if (handle < 0 || handle >= (int32_t) a->insps.size() || !a->insps[handle].open) return -1;
-  *cfg = a->insps[handle].cfg;
+  const Insp *i = a->open_insp(handle);
+  if (!i) return -1;
+  *cfg = i->cfg;
   return 0;
 }
 extern "C" int sdb_analyzer_inspector_set_spectrum_async(sdb_analyzer_t *a, int32_t handle, uint32_t spectsrc_id,
