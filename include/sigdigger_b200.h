@@ -55,7 +55,12 @@ typedef struct {
   int32_t  device;          /* CUDA ordinal */
   uint32_t flags;
   int32_t  input_format;    /* SDB_FORMAT_*: layout of the IQ the feed calls receive */
+  /* Frame-averaged main PSD (SPEC A, oracle/SPEC_A.md): 0 or 1 = off; A in [2, SDB_PSD_AVERAGE_MAX] emits the mean of
+   * every A consecutive frames of each stream (the partial group carries across feeds; sdb_engine_read_psd_average).
+   * With averaging on, SDB_FLAG_PSD_SHIFT_DB applies to the means only and the per-frame PSD stays linear. */
+  uint32_t psd_average;
 } sdb_engine_params;
+#define SDB_PSD_AVERAGE_MAX 65536u
 
 /* SUSCAN_SOURCE_FORMAT_RAW_{FLOAT32, UNSIGNED8, SIGNED8, SIGNED16} (Default/SourceConfig/FileSourcePage.cpp:80-104):
  * interleaved I,Q pairs; 8/16-bit samples are converted inside the first load of the path (u8: (v-128)/128,
@@ -128,8 +133,9 @@ int sdb_inspector_config_default(sdb_inspector_config *cfg, int insp_class, floa
 /* freezes the channel plan and allocates device buffers; required before the first feed */
 int sdb_engine_commit(sdb_engine_t *e);
 /* Live re-plan: `dst` (committed, not yet fed) takes over the running state of `src` (same streams / window /
- * device): input history, and per channel with identical parameters the cross-fade tail, the LO phase and -- if the
- * inspector class and the sizes of its state lines are unchanged -- the loop state of every chain.  This is how an
+ * device): input history, the partial group of the frame-averaged PSD when psd_size, psd_window and psd_average match
+ * (otherwise `dst` starts an empty group), and per channel with identical parameters the cross-fade tail, the LO phase
+ * and -- if the inspector class and the sizes of its state lines are unchanged -- the loop state of every chain.  This is how an
  * analyzer opens, closes, retunes or reconfigures ONE inspector at a block boundary while the others keep running
  * (suscan_analyzer_open_ex_async / close_async / set_inspector_config_async / set_inspector_freq_overridable,
  * Suscan/Analyzer.cpp:459-526).  `src` is synchronised and left intact. */
@@ -158,6 +164,13 @@ int sdb_engine_join(sdb_engine_t *e);
 size_t       sdb_engine_psd_frames(const sdb_engine_t *e);
 const float *sdb_engine_psd_device(const sdb_engine_t *e);
 int          sdb_engine_read_psd(sdb_engine_t *e, float *dst, size_t cap_floats);
+/* Frame-averaged PSD of the last feed (sdb_engine_params.psd_average >= 2): [stream][mean][psd_size] float32, the means
+ * of the groups the feed completed, linear with DC at 0 unless SDB_FLAG_PSD_SHIFT_DB.  _frames: means per stream (0
+ * when averaging is off); _device: the engine's buffer, valid until the feed after next; read: blocking copy, fenced
+ * like sdb_engine_read_psd. */
+size_t       sdb_engine_psd_average_frames(const sdb_engine_t *e);
+const float *sdb_engine_psd_average_device(const sdb_engine_t *e);
+int          sdb_engine_read_psd_average(sdb_engine_t *e, float *dst, size_t cap_floats);
 /* channel-rate output of the channeliser (what on_data delivers, Tasks/LPFTask.cpp:28-42) */
 long         sdb_engine_read_channel(sdb_engine_t *e, uint32_t stream, int handle, sdb_complex *dst,
                                      size_t cap);
@@ -222,7 +235,8 @@ typedef struct {
   float    snr, S0, N0;             /* linear power: peak averaged level, noise floor, S0 / N0 */
   uint32_t bin_lo, bin_hi;          /* [lo, hi) in ascending-frequency bin order */
 } sdb_detected_channel;
-/* engine-integrated: enable before sdb_engine_commit(); needs a linear PSD (no SDB_FLAG_PSD_SHIFT_DB) */
+/* engine-integrated: enable before sdb_engine_commit(); needs a linear per-frame PSD (no SDB_FLAG_PSD_SHIFT_DB, unless
+ * psd_average >= 2 confines the flag to the means) */
 int  sdb_engine_set_channel_detector(sdb_engine_t *e, float alpha, float beta, float gamma, float snr,
                                      uint32_t min_bins);
 /* channels of one stream after the latest feed (ascending frequency); *total = channels found before the
@@ -254,8 +268,9 @@ void    *sdb_engine_stream(const sdb_engine_t *e);
 uint64_t sdb_engine_launch_count(const sdb_engine_t *e);
 /* average device time (ms) of the named kernel family over the launches since the last reset, measured
  * with CUDA events on the engine stream; families: "fft_cols", "fft_rows_psd", "fft_rows_chan",
- * "chan_ifft", "inspector".  A 65536-point plan's fused forward transform counts as "fft_cols"; its
- * "fft_rows_psd" / "fft_rows_chan" stay at zero launches */
+ * "chan_ifft", "inspector", "psd_average".  A 65536-point plan's fused forward transform counts as "fft_cols"; its
+ * "fft_rows_psd" / "fft_rows_chan" stay at zero launches; "psd_average" (the group means) records none while
+ * averaging is off */
 int      sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches);
 void     sdb_engine_timing(sdb_engine_t *e, int enable);
 /* inspector-kernel stage balance since the last reset: out[0..3] = busy SM cycles of the gain / carrier /
@@ -443,6 +458,10 @@ typedef struct {
   struct { uint64_t window_size; int32_t window; float alpha, beta, gamma, snr; } detector_params;
   float   channel_update_int, psd_update_int;       /* seconds */
   double  min_freq, max_freq;
+  /* Channel mode: non-zero posts, instead of one frame per psd_update_int, the mean of every
+   * A = clamp(llround(psd_update_int * rate / window_size), 1, SDB_PSD_AVERAGE_MAX) frames (SPEC A), time-stamped at
+   * its first sample; 0 = one frame per interval.  Wide-spectrum sweeps ignore it. */
+  int32_t psd_average;
 } sdb_analyzer_params;
 
 /* the part of suscan_source_config_t this path needs: a callback source (role of file / stdin / SoapySDR

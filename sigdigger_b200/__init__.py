@@ -26,7 +26,7 @@ ESTIMATOR = {"baud-fac": 0, "baud-nonlinear": 1}
 class EngineParams(C.Structure):
     _fields_ = [("n_streams", C.c_uint32), ("psd_size", C.c_uint32), ("psd_window", C.c_int32),
                 ("st_window_size", C.c_uint32), ("max_feed", C.c_uint32), ("device", C.c_int32),
-                ("flags", C.c_uint32), ("input_format", C.c_int32)]
+                ("flags", C.c_uint32), ("input_format", C.c_int32), ("psd_average", C.c_uint32)]
 
 
 FORMAT = {"f32": 0, "u8": 1, "s8": 2, "s16": 3}
@@ -271,6 +271,9 @@ _PROTOS = {
     "sdb_engine_psd_frames": (C.c_size_t, [C.c_void_p]),
     "sdb_engine_psd_device": (C.c_void_p, [C.c_void_p]),
     "sdb_engine_read_psd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "sdb_engine_psd_average_frames": (C.c_size_t, [C.c_void_p]),
+    "sdb_engine_psd_average_device": (C.c_void_p, [C.c_void_p]),
+    "sdb_engine_read_psd_average": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "sdb_engine_read_channel": (C.c_long, [C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t]),
     "sdb_engine_read_symbols": (C.c_long, [C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t]),
     "sdb_engine_read_all_symbols": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
@@ -499,11 +502,12 @@ class Engine:
     """Batch analyzer engine: main PSD + channeliser + inspectors over S streams on one GPU."""
 
     def __init__(self, n_streams=1, psd_size=65536, psd_window="blackmann_harris", st_window_size=0,
-                 max_feed=0, samp_rate=1.0, device=0, flags=0, input_format="f32"):
+                 max_feed=0, samp_rate=1.0, device=0, flags=0, input_format="f32", psd_average=0):
+        """psd_average: A >= 2 also emits the mean of every A PSD frames (SPEC A, read_psd_average); 0 or 1 = off."""
         L = load_library()
         self.input_format = FORMAT[input_format] if isinstance(input_format, str) else int(input_format)
         p = EngineParams(n_streams, psd_size, WINDOW[psd_window] if isinstance(psd_window, str) else psd_window,
-                         st_window_size, max_feed, device, flags, self.input_format)
+                         st_window_size, max_feed, device, flags, self.input_format, psd_average)
         self._L = L
         self.n_streams, self.psd_size, self.samp_rate = n_streams, psd_size, samp_rate
         self.st_window_size = st_window_size or psd_size
@@ -583,6 +587,22 @@ class Engine:
             out = np.empty((self.n_streams, f, self.psd_size), np.float32)
         _check(self._L.sdb_engine_read_psd(self._h, out.ctypes.data, out.size))
         return out
+
+    def read_psd_average(self, out=None):
+        """-> [n_streams, means, psd_size] float32: the group means the last feed completed (SPEC A)"""
+        m = self._L.sdb_engine_psd_average_frames(self._h)
+        if out is None:
+            out = np.empty((self.n_streams, m, self.psd_size), np.float32)
+        _check(self._L.sdb_engine_read_psd_average(self._h, out.ctypes.data, out.size))
+        return out
+
+    @property
+    def psd_average_frames(self):
+        return self._L.sdb_engine_psd_average_frames(self._h)
+
+    @property
+    def psd_average_device_ptr(self):
+        return self._L.sdb_engine_psd_average_device(self._h)
 
     # ---- channel detector (SPEC K; detector_params of Suscan/AnalyzerParams.cpp:27-66)
     def set_channel_detector(self, alpha=0.01, beta=0.01, gamma=0.5, snr=4.0, min_bins=2):

@@ -30,7 +30,8 @@ class DetectorParams(C.Structure):
 
 class AnalyzerParams(C.Structure):
     _fields_ = [("mode", C.c_int32), ("detector_params", DetectorParams), ("channel_update_int", C.c_float),
-                ("psd_update_int", C.c_float), ("min_freq", C.c_double), ("max_freq", C.c_double)]
+                ("psd_update_int", C.c_float), ("min_freq", C.c_double), ("max_freq", C.c_double),
+                ("psd_average", C.c_int32)]
 
 
 READ_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.c_void_p, C.c_size_t)
@@ -81,8 +82,10 @@ class StatusMsg(C.Structure):
 class Analyzer:
     def __init__(self, samp_rate, window_size=8192, window="hann", psd_update_int=0.04, data=None, read=None,
                  read_size=0, loop=False, freq=0.0, device=0, channel_update_int=0.0, alpha=0.25, beta=0.25,
-                 gamma=0.5, snr=8.0, wide=False, min_freq=0.0, max_freq=0.0, set_frequency=None, decimation=1):
-        """decimation: source decimation D (SPEC L); the analyzer then runs at samp_rate / D."""
+                 gamma=0.5, snr=8.0, wide=False, min_freq=0.0, max_freq=0.0, set_frequency=None, decimation=1,
+                 psd_average=0):
+        """decimation: source decimation D (SPEC L); the analyzer then runs at samp_rate / D.
+        psd_average: non-zero posts the mean of the frames of every psd_update_int instead of one frame (SPEC A)."""
         self._L = load_library()
         p = AnalyzerParams()
         p.mode = 1 if wide else 0                      # SDB_ANALYZER_MODE_{CHANNEL, WIDE_SPECTRUM}
@@ -93,6 +96,7 @@ class Analyzer:
         p.detector_params.gamma, p.detector_params.snr = gamma, snr
         p.psd_update_int = psd_update_int
         p.channel_update_int = channel_update_int
+        p.psd_average = psd_average
         self.params = p
         s = SourceConfig()
         s.samp_rate, s.freq, s.read_size, s.loop, s.device = samp_rate, freq, read_size, int(loop), device
@@ -198,6 +202,22 @@ class Analyzer:
     def estimator_cmd(self, handle, estimator_id, enabled=True, req_id=0):
         self._L.sdb_analyzer_inspector_estimator_cmd_async(self._h, handle, estimator_id, int(enabled), req_id)
 
+    def set_params(self, req_id=0, **changes):
+        """suscan_analyzer_set_params_async: the current params with `changes` (AnalyzerParams field names; the
+        detector's window_size / window as such)"""
+        p = AnalyzerParams()
+        C.memmove(C.byref(p), C.byref(self.params), C.sizeof(p))
+        for k, v in changes.items():
+            if k in ("window_size", "window"):
+                setattr(p.detector_params, k, WINDOW[v] if k == "window" and isinstance(v, str) else v)
+            elif hasattr(p, k):
+                setattr(p, k, v)
+            else:
+                raise KeyError(k)
+        if self._L.sdb_analyzer_set_params_async(self._h, C.byref(p), req_id):
+            raise SdbError("set_params_async rejected")
+        self.params = p
+
     def close_inspector(self, handle, req_id=0):
         self._L.sdb_analyzer_close_async(self._h, handle, req_id)
 
@@ -245,6 +265,11 @@ class Analyzer:
                 m = C.cast(ptr, C.POINTER(SourceInfo)).contents
                 out = dict(source_samp_rate=m.source_samp_rate, effective_samp_rate=m.effective_samp_rate,
                            frequency=m.frequency, seekable=m.seekable)
+            elif name == "PARAMS":
+                m = C.cast(ptr, C.POINTER(AnalyzerParams)).contents
+                out = dict(mode=m.mode, window_size=m.detector_params.window_size, window=m.detector_params.window,
+                           psd_update_int=m.psd_update_int, channel_update_int=m.channel_update_int,
+                           psd_average=m.psd_average)
             elif name in ("EOS", "READ_ERROR", "HALT", "SOURCE_INIT"):
                 m = C.cast(ptr, C.POINTER(StatusMsg)).contents
                 out = dict(code=m.code, err_msg=(m.err_msg or b"").decode())

@@ -149,6 +149,11 @@ struct sdb_analyzer {
   // geometry set by rebuild).
   std::mutex insp_m;
   double psd_credit = 0;
+  // frame-averaged PSD (params.psd_average, SPEC A): the A, window size and window function of the baseband engine,
+  // whether A was clamped, and the frames of the engine's current partial group (its carry survives a re-plan exactly
+  // when A, N and the window stay, see sdb_engine_migrate)
+  uint32_t avg_A = 0, avg_N = 0; int32_t avg_window = 0; bool avg_clamped = false;
+  uint64_t avg_frames = 0;
   // source-side options of the worker loop (Suscan/Analyzer.cpp:117-135, 229-244; SourceWidget.cpp:1156-1184)
   bool iq_reverse = false, dc_remove = false;
   double throttle = 0;                                  // samples / s, 0 = as fast as the source delivers
@@ -314,6 +319,18 @@ struct sdb_analyzer {
     ep.device = src.device;
     ep.flags = (iq_reverse ? SDB_FLAG_IQ_REVERSE : 0) | (dc_remove ? SDB_FLAG_DC_REMOVE : 0);
     ep.input_format = src.read || dec ? SDB_FORMAT_FLOAT32 : src.input_format;
+    // frames per averaged PSD: the whole frames of one psd_update_int (1 = every frame, averaging off)
+    uint32_t A = 0;
+    avg_clamped = false;
+    if (params.psd_average) {
+      const double want = (double) params.psd_update_int * rate / (double) ep.psd_size;
+      const long long r = want > 0 ? llround(std::min(want, 1e12)) : 0;
+      A = (uint32_t) std::min<long long>(std::max<long long>(r, 1), SDB_PSD_AVERAGE_MAX);
+      avg_clamped = (long long) A != r;
+    }
+    ep.psd_average = A;
+    if (!old || A != avg_A || ep.psd_size != avg_N || ep.psd_window != avg_window) avg_frames = 0;
+    avg_A = A; avg_N = ep.psd_size; avg_window = ep.psd_window;
     eng = plan_level(ep, rate, -1, old_handle, old.get());
     if (!eng) return false;
     // sub-carrier engines: one per inspector that has open children, parents before children (an inspector's handle
@@ -671,6 +688,29 @@ struct sdb_analyzer {
   void publish_psd()
   {
     const size_t N = (size_t) params.detector_params.window_size, frames = block / N;
+    if (avg_A >= 2) {
+      // the means the block completed, one per A frames; group j of the block starts j A - avg_frames frames after
+      // the block's first (earlier blocks hold its start when that is negative).  Unless A was clamped a mean lasts
+      // exactly the interval the credit is measured against, so every mean is posted.
+      const size_t means = sdb_engine_psd_average_frames(eng.get());
+      const uint64_t carried = avg_frames;
+      avg_frames = (avg_frames + frames) % avg_A;
+      psd.resize(means * N);
+      if (means && sdb_engine_read_psd_average(eng.get(), psd.data(), psd.size())) return;
+      const double per_mean = (double) avg_A * (double) N / rate;
+      const double interval = avg_clamped ? (double) params.psd_update_int : per_mean;
+      const int64_t block_start = (int64_t) (total_samples - block * decim);
+      for (size_t j = 0; j < means; ++j) {
+        psd_credit += per_mean;
+        if (psd_credit + 1e-12 >= interval) {
+          psd_credit = fmod(psd_credit, interval);
+          const int64_t first = (int64_t) (j * avg_A) - (int64_t) carried;
+          post_psd((int64_t) src.freq, rate, &psd[j * N], N,
+                   (double) (block_start + first * (int64_t) (N * decim)) / src.samp_rate, looped, (uint64_t) hist_fill);
+        }
+      }
+      return;
+    }
     psd.resize(frames * N);
     if (sdb_engine_read_psd(eng.get(), psd.data(), psd.size())) return;
     const double per_frame = (double) N / rate;

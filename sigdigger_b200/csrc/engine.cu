@@ -44,9 +44,9 @@ struct Channel {
 };
 
 struct TimedSpan { int family; Event a, b; };
-enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_COUNT };
+enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
-                                            "inspector" };
+                                            "inspector", "psd_average" };
 
 struct ChdetDeleter { void operator()(sdb_chdet *d) const { sdb_chdet_destroy(d); } };
 
@@ -54,6 +54,7 @@ struct ChdetDeleter { void operator()(sdb_chdet *d) const { sdb_chdet_destroy(d)
 // kernels of feed i (three copy/compute streams).  Each event guards its slot's buffers between the streams.
 struct Slot {
   float *psd = nullptr;                             // [S][frames][Np]
+  float *psd_avg = nullptr;                         // [S][means][Np], frame averaging only (SPEC A)
   // channel streams: the (latency-bound, 1-CTA-per-32-chains) inspector kernel of feed i runs on its own stream
   // while the FFT kernels of feed i+1 fill the other slot
   float2 *chan = nullptr;
@@ -108,11 +109,15 @@ struct Plan {
   // DC removal (SDB_FLAG_DC_REMOVE, SPEC R): per-stream estimate, the estimate the current block is corrected with,
   // run sums, and the corrected float32 copy of the block the rest of the path reads
   float2 *d_dc_state = nullptr, *d_dc_cur = nullptr, *d_xdc = nullptr; double2 *d_dc_part = nullptr;
+  // frame averaging (SPEC A): per-stream partial sums of the current group, and its frame count (the same in every
+  // stream: each feed has the same frames per stream)
+  float *d_avg_carry = nullptr;         // [S][Np]
+  unsigned avg_count = 0;
   // running state
   unsigned feed_index = 0, host_feeds = 0;
   bool first_feed = true;               // (engines without channels keep no history)
   uint64_t n_fed = 0;                   // samples fed so far
-  size_t last_frames = 0, last_hops = 0;
+  size_t last_frames = 0, last_hops = 0, last_means = 0;
 
   // the slot of the latest feed (slot 0 before the first)
   Slot &cur() { return slot[feed_index ? (feed_index - 1) & 1u : 0]; }
@@ -349,7 +354,8 @@ extern "C" int sdb_engine_set_channel_detector(sdb_engine_t *e, float alpha, flo
   if (!e) return fail("null argument");
   if (e->plan) return fail("engine already committed");
   if (!e->prm.psd_size) return fail("the channel detector needs the main PSD");
-  if (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) return fail("the channel detector needs a linear PSD");
+  if ((e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) && e->prm.psd_average < 2)
+    return fail("the channel detector needs a linear PSD");
   if (!(snr > 0.0f) || !(alpha >= 0.0f && alpha <= 1.0f) || !(gamma >= 0.0f && gamma <= 1.0f))
     return fail("detector parameters out of range");
   e->cd_enabled = true; e->cd_alpha = alpha; e->cd_gamma = gamma; e->cd_snr = snr; e->cd_min_bins = min_bins ? min_bins : 1;
@@ -604,6 +610,10 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
   if (max_feed == 0) return fail("max_feed must be > 0");
   if (max_feed % (W / 2)) return fail("max_feed must be a multiple of st_window_size / 2");
   if (Np && max_feed % Np) return fail("max_feed must be a multiple of psd_size");
+  const unsigned A = e->prm.psd_average;
+  if (A > SDB_PSD_AVERAGE_MAX)
+    return fail("psd_average must be at most " + std::to_string(SDB_PSD_AVERAGE_MAX) + ", got " + std::to_string(A));
+  if (A >= 2 && !Np) return fail("psd_average needs the main PSD (psd_size > 0)");
   // built here and handed to the engine at the end: every early return frees what was built so far
   auto plan = std::make_unique<Plan>();
   Plan &p = *plan;
@@ -622,6 +632,17 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
     for (Slot &sl : p.slot) {
       sl.psd = p.dalloc<float>((size_t) S * max_frames * Np);
       if (!sl.psd) return fail("out of device memory (psd)");
+    }
+    if (A >= 2) {
+      // a feed completes at most ceil(max_frames / A) groups (A - 1 carried frames + max_frames)
+      const size_t max_means = (max_frames + A - 1) / A;
+      for (Slot &sl : p.slot) {
+        sl.psd_avg = p.dalloc<float>((size_t) S * max_means * Np);
+        if (!sl.psd_avg) return fail("out of device memory (averaged psd)");
+      }
+      p.d_avg_carry = p.dalloc<float>((size_t) S * Np);
+      if (!p.d_avg_carry) return fail("out of device memory (averaged psd)");
+      CK(cudaMemset(p.d_avg_carry, 0, (size_t) S * Np * sizeof(float)));
     }
     if (e->cd_enabled) {
       p.chdet.reset(sdb_chdet_new(e->prm.device, Np, S, e->cd_alpha, e->cd_gamma, e->cd_snr, e->cd_min_bins));
@@ -857,10 +878,24 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     x = p.d_xdc; fmt = SDB_FMT_F32; stride = n;
   }
   SdbLaunchCtx ctx{ e->stream, &e->launches };
-  const int shift_db = (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) ? 1 : 0;
+  // with frame averaging the flag applies to the means: the transforms keep the per-frame PSD linear
+  const int means_db = (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) ? 1 : 0;
+  const int shift_db = p.d_avg_carry ? 0 : means_db;
   Slot &sl = p.slot[p.feed_index & 1u];     // result buffers of this feed
 
   const int frames = Np ? (int) (n / Np) : 0;
+  // SPEC A group means of this feed, on the stream of its PSD transforms, after the last of them
+  auto group_means = [&](const SdbLaunchCtx &lc) -> int {
+    if (!p.d_avg_carry) return 0;
+    const unsigned A = e->prm.psd_average, means = (p.avg_count + (unsigned) frames) / A;
+    e->span_begin(FAM_PSD_AVERAGE, lc.stream);
+    CK(sdb_launch_psd_group_mean(lc, sl.psd, (unsigned) frames, Np, S, A, p.avg_count, means, means_db,
+                                 p.d_avg_carry, sl.psd_avg));
+    e->span_end(lc.stream);
+    p.avg_count = (p.avg_count + (unsigned) frames) % A;
+    p.last_means = means;
+    return 0;
+  };
   const int H = K ? (int) (n / (W / 2)) : 0;
   const int first = (K && p.first_feed) ? 1 : 0;
   const int wps = K ? H - first : 0;
@@ -920,6 +955,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     }
     if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, p.psd_stream,
                                           &e->launches));
+    if (group_means(pctx)) return -1;
     CK(sl.psd_ready.record(p.psd_stream));
     CK(sl.psd_ready.wait_on(e->stream));          // the main stream stays the engine's timeline
   } else {
@@ -952,6 +988,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
       }
       if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, e->stream,
                                             &e->launches));
+      if (group_means(ctx)) return -1;
       CK(sl.psd_ready.record(e->stream));
     }
     // ---- channeliser forward transforms
@@ -1067,6 +1104,30 @@ extern "C" int sdb_engine_read_psd(sdb_engine_t *e, float *dst, size_t cap)
   if (!e || !dst) return fail("null argument");
   if (sdb_engine_read_psd_async(e, dst, cap)) return -1;
   CK(cudaStreamSynchronize(e->plan->d2h_stream));
+  return 0;
+}
+
+extern "C" size_t sdb_engine_psd_average_frames(const sdb_engine_t *e) { return e && e->plan ? e->plan->last_means : 0; }
+extern "C" const float *sdb_engine_psd_average_device(const sdb_engine_t *e)
+{
+  return e && e->plan ? e->plan->cur().psd_avg : nullptr;
+}
+
+extern "C" int sdb_engine_read_psd_average(sdb_engine_t *e, float *dst, size_t cap)
+{
+  if (!e || !dst) return fail("null argument");
+  if (!e->plan || !e->plan->d_avg_carry) return fail("PSD averaging not enabled");
+  Plan &p = *e->plan;
+  if (p.feed_index == 0) return fail("no PSD available");
+  const size_t n = (size_t) e->prm.n_streams * p.last_means * e->Np;
+  if (cap < n) return fail("destination too small");
+  if (n == 0) return 0;
+  Slot &sl = p.cur();
+  CK(cudaSetDevice(e->prm.device));
+  CK(sl.psd_ready.wait_on(p.d2h_stream));
+  CK(cudaMemcpyAsync(dst, sl.psd_avg, n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
+  CK(sl.psd_read.record(p.d2h_stream));
+  CK(cudaStreamSynchronize(p.d2h_stream));
   return 0;
 }
 
@@ -1252,6 +1313,12 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
     CK(cudaMemcpy(to.d_hist, from.d_hist, (size_t) S * (W / 2) * sizeof(float2), cudaMemcpyDeviceToDevice));
   if (to.d_dc_state && from.d_dc_state)
     CK(cudaMemcpy(to.d_dc_state, from.d_dc_state, S * sizeof(float2), cudaMemcpyDeviceToDevice));
+  // the partial SPEC A group, when both engines average the same frames the same way
+  if (to.d_avg_carry && from.d_avg_carry && dst->Np == src->Np && dst->prm.psd_window == src->prm.psd_window &&
+      dst->prm.psd_average == src->prm.psd_average) {
+    CK(cudaMemcpy(to.d_avg_carry, from.d_avg_carry, (size_t) S * dst->Np * sizeof(float), cudaMemcpyDeviceToDevice));
+    to.avg_count = from.avg_count;
+  }
   // an engine that had no channel so far kept no input history: its first window starts with this feed
   to.first_feed = from.d_hist ? from.first_feed : true;
   to.n_fed = from.n_fed;

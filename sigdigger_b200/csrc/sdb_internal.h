@@ -428,6 +428,10 @@ cudaError_t sdb_launch_spectsrc(const SdbLaunchCtx &c, const SdbSpectCfg *cfg_de
                                 int n_channels, int n_streams, int max_ns, const float2 *chan_in,
                                 size_t chan_stream_stride, uint32_t n_hops, float *spect, size_t spect_stream_stride,
                                 uint32_t *spect_size, float *est, int *est_valid);
+// sview_kernels.cu: frame-averaged main PSD (SPEC A); psd [S][frames][n] -> out [S][means][n], carry [S][n]
+cudaError_t sdb_launch_psd_group_mean(const SdbLaunchCtx &c, const float *psd, unsigned frames, unsigned n,
+                                      size_t n_streams, unsigned A, unsigned carried, unsigned means, int shift_db,
+                                      float *carry, float *out);
 // tasks_kernels.cu
 cudaError_t sdb_launch_dc_remove(cudaStream_t st, const void *x, int fmt, size_t stream_stride, size_t n, int n_streams,
                                  float alpha, float2 *state, float2 *cur, double2 *part, float2 *out);

@@ -440,6 +440,59 @@ static cudaError_t sdb_launch_psd_average(cudaStream_t s, const float *psd, size
   return cudaGetLastError();
 }
 
+// Frame-averaged main PSD (SPEC A, oracle/SPEC_A.md): per (stream, bin), the frames of the feed are added in order to
+// the carried partial sum (plain binary32 adds, this unit is built without contraction); every A-th frame of the
+// running count finishes a group, whose mean acc / A is one IEEE division.  psd is [S][frames][n], out [S][means][n]
+// (fft-shifted and in dB with shift_db, the expression of k_psd_shift_db), carry [S][n].  `carried` frames of the
+// current group precede this feed.  Threads of a warp own consecutive bins, so every load and store is coalesced; the
+// frame loop issues UNROLL independent loads before the in-order adds.
+#define SDB_MEAN_UNROLL 8
+__global__ void __launch_bounds__(256) k_psd_group_mean(const float *__restrict__ psd, unsigned frames, unsigned n,
+                                                         size_t n_streams, unsigned A, unsigned carried, unsigned means,
+                                                         int shift_db, float *__restrict__ carry,
+                                                         float *__restrict__ out)
+{
+  const size_t t = blockIdx.x * (size_t) blockDim.x + threadIdx.x;
+  if (t >= n_streams * n) return;
+  const size_t s = t / n;
+  const unsigned k = (unsigned) (t - s * n);
+  const float *__restrict__ x = psd + s * (size_t) frames * n + k;
+  float *__restrict__ o = out + s * (size_t) means * n + (shift_db ? ((k + (n >> 1)) & (n - 1)) : k);
+  const float fa = (float) A;
+  // the carry is only read when a group is open and only written when one stays open: feeds that end on a group
+  // boundary move no carry bytes
+  float acc = carried ? carry[t] : 0.0f;
+  unsigned cnt = carried;
+  for (unsigned f0 = 0; f0 < frames; f0 += SDB_MEAN_UNROLL) {
+    float v[SDB_MEAN_UNROLL];
+#pragma unroll
+    for (int u = 0; u < SDB_MEAN_UNROLL; ++u) v[u] = f0 + u < frames ? __ldg(x + (size_t) (f0 + u) * n) : 0.0f;
+#pragma unroll
+    for (int u = 0; u < SDB_MEAN_UNROLL; ++u) {
+      if (f0 + u < frames) {
+        acc = __fadd_rn(acc, v[u]);
+        if (++cnt == A) {
+          const float m = __fdiv_rn(acc, fa);
+          *o = shift_db ? 10.0f * d_log10f(m + 1e-8f) : m;
+          o += n; acc = 0.0f; cnt = 0;
+        }
+      }
+    }
+  }
+  if (cnt) carry[t] = acc;
+}
+
+cudaError_t sdb_launch_psd_group_mean(const SdbLaunchCtx &c, const float *psd, unsigned frames, unsigned n,
+                                      size_t n_streams, unsigned A, unsigned carried, unsigned means, int shift_db,
+                                      float *carry, float *out)
+{
+  if (frames == 0 || n_streams * n == 0) return cudaSuccess;
+  k_psd_group_mean<<<(unsigned) ((n_streams * n + 255) / 256), 256, 0, c.stream>>>(psd, frames, n, n_streams, A, carried,
+                                                                                   means, shift_db, carry, out);
+  if (c.launch_counter) ++*c.launch_counter;
+  return cudaGetLastError();
+}
+
 static cudaError_t sdb_launch_psd_shift_db(cudaStream_t s, const float *lin, float *db, size_t n_frames, unsigned n)
 {
   const size_t total = n_frames * n;
