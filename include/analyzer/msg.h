@@ -81,7 +81,7 @@ SUBOOL suscan_config_set_bool(suscan_config_t *cfg, const char *name, SUBOOL val
 SUBOOL suscan_config_set_string(suscan_config_t *cfg, const char *name, const char *value);
 SUBOOL suscan_config_desc_has_prefix(const suscan_config_desc_t *desc, const char *prefix);
 SUBOOL suscan_config_str_to_bool(const char *str, SUBOOL deflt);
-/* the bag of an inspector class ("psk", "fsk", "ask", "audio", "raw") with its default values for a channel rate */
+/* the bag of an inspector class ("psk", "fsk", "ask", "audio", "raw", "power") with its default values for a channel rate */
 suscan_config_t *suscan_inspector_config_new(const char *class_name, SUFLOAT equiv_fs);
 
 /* enum values of the config vocabulary (InspectorCtl/ClockRecovery.cpp:59-93, MfControl.cpp:56-78,

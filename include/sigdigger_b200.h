@@ -27,8 +27,10 @@ enum { SDB_WINDOW_NONE = 0, SDB_WINDOW_HAMMING, SDB_WINDOW_HANN, SDB_WINDOW_FLAT
        SDB_WINDOW_BLACKMANN_HARRIS };
 
 /* inspector classes: "psk" / "fsk" / "ask" (Default/Inspection/InspToolWidget.cpp:932,938,944),
- * "audio" (Default/Audio/AudioProcessor.cpp:153), "raw" (InspToolWidget.cpp:612) */
-enum { SDB_INSP_PSK = 0, SDB_INSP_FSK = 1, SDB_INSP_ASK = 2, SDB_INSP_AUDIO = 3, SDB_INSP_RAW = 4 };
+ * "audio" (Default/Audio/AudioProcessor.cpp:153), "raw" (InspToolWidget.cpp:612), "power" (InspToolWidget.cpp:950,
+ * the RMS tool: one mean channel power (re, 0) per power_integrate_samples channel samples, SPEC PW in
+ * oracle/SPEC_PW.md) */
+enum { SDB_INSP_PSK = 0, SDB_INSP_FSK = 1, SDB_INSP_ASK = 2, SDB_INSP_AUDIO = 3, SDB_INSP_RAW = 4, SDB_INSP_POWER = 5 };
 
 /* SigDigger's AudioDemod enum + 1 as it goes on the wire (include/SigDiggerHelpers.h:39-45,
  * Default/Audio/AudioProcessor.cpp:261) */
@@ -86,7 +88,8 @@ typedef struct {
  * (AskControl.cpp:53-77); mf.type, mf.roll-off (MfControl.cpp:56-78); clock.type, clock.baud,
  * clock.gain, clock.phase, clock.running (ClockRecovery.cpp:59-93); equalizer.type, equalizer.rate,
  * equalizer.locked (EqualizerControl.cpp:47-75); audio.* and agc.ts
- * (Default/Audio/AudioProcessor.cpp:257-265).  All under Default/GenericInspector/InspectorCtl/. */
+ * (Default/Audio/AudioProcessor.cpp:257-265).  All under Default/GenericInspector/InspectorCtl/, except
+ * power.integrate-samples (Default/RMSInspector/RMSInspector.cpp:404-416, 438-439). */
 typedef struct {
   int32_t  insp_class;
   float    fs;              /* filled by the engine: equivalent channel rate in Hz (= samp_rate / decimation) */
@@ -111,6 +114,9 @@ typedef struct {
   uint32_t eq_type;         /* equalizer.type: SUSCAN_INSPECTOR_EQUALIZER_{BYPASS=0, CMA=1} (EqualizerControl.cpp:56-75) */
   float    eq_rate;         /* equalizer.rate */
   int32_t  eq_locked;       /* equalizer.locked */
+  /* power.integrate-samples: channel samples per mean of the "power" class (0 is read as 1); the default is
+   * max(1, llround(0.1 fs)), a tenth of a second of channel samples */
+  uint64_t power_integrate_samples;
 } sdb_inspector_config;
 
 const char *sdb_last_error(void);
@@ -135,7 +141,8 @@ int sdb_engine_commit(sdb_engine_t *e);
 /* Live re-plan: `dst` (committed, not yet fed) takes over the running state of `src` (same streams / window /
  * device): input history, the partial group of the frame-averaged PSD when psd_size, psd_window and psd_average match
  * (otherwise `dst` starts an empty group), and per channel with identical parameters the cross-fade tail, the LO phase
- * and -- if the inspector class and the sizes of its state lines are unchanged -- the loop state of every chain.  This is how an
+ * and -- if the inspector class and the sizes of its state lines are unchanged -- the loop state of every chain; a power
+ * inspector that stays one with the same power_integrate_samples keeps its partial group (SPEC PW).  This is how an
  * analyzer opens, closes, retunes or reconfigures ONE inspector at a block boundary while the others keep running
  * (suscan_analyzer_open_ex_async / close_async / set_inspector_config_async / set_inspector_freq_overridable,
  * Suscan/Analyzer.cpp:459-526).  `src` is synchronised and left intact. */
@@ -268,9 +275,9 @@ void    *sdb_engine_stream(const sdb_engine_t *e);
 uint64_t sdb_engine_launch_count(const sdb_engine_t *e);
 /* average device time (ms) of the named kernel family over the launches since the last reset, measured
  * with CUDA events on the engine stream; families: "fft_cols", "fft_rows_psd", "fft_rows_chan",
- * "chan_ifft", "inspector", "psd_average".  A 65536-point plan's fused forward transform counts as "fft_cols"; its
- * "fft_rows_psd" / "fft_rows_chan" stay at zero launches; "psd_average" (the group means) records none while
- * averaging is off */
+ * "chan_ifft", "inspector", "psd_average", "power".  A 65536-point plan's fused forward transform counts as "fft_cols";
+ * its "fft_rows_psd" / "fft_rows_chan" stay at zero launches; "psd_average" (the group means) records none while
+ * averaging is off, "power" (the power inspectors' integration) none while no channel has a power inspector */
 int      sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches);
 void     sdb_engine_timing(sdb_engine_t *e, int enable);
 /* inspector-kernel stage balance since the last reset: out[0..3] = busy SM cycles of the gain / carrier /
@@ -741,6 +748,11 @@ int  sdb_tv_feed_transform(const sdb_complex *x, size_t n, int mode, float k, fl
  * cfg->fs must be the buffers' sample rate. */
 long sdb_task_inspector(const sdb_inspector_config *cfg, const sdb_complex *src, size_t n, size_t batch,
                         sdb_complex *soft, uint8_t *hard, uint32_t *counts, size_t cap);
+/* Offline power inspector (SPEC PW) over captured channel-rate buffers, what the RMS tab's raw mode computes over a
+ * capture: `batch` buffers of n samples, each integrated from an empty group with `integrate_samples` samples per
+ * mean (0 is read as 1) -> means [batch][cap] as (mean, 0), counts [batch]; cap must be >= n / integrate_samples */
+long sdb_task_power(const sdb_complex *src, size_t n, size_t batch, uint64_t integrate_samples, sdb_complex *means,
+                    uint32_t *counts, size_t cap);
 
 #ifdef __cplusplus
 }

@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsigdigger_b200.so")
 
 WINDOW = {"none": 0, "hamming": 1, "hann": 2, "flat_top": 3, "blackmann_harris": 4}
-INSP = {"psk": 0, "fsk": 1, "ask": 2, "audio": 3, "raw": 4}
+INSP = {"psk": 0, "fsk": 1, "ask": 2, "audio": 3, "raw": 4, "power": 5}
 AUDIO = {"disabled": 0, "am": 1, "fm": 2, "usb": 3, "lsb": 4}
 FLAG_PSD_SHIFT_DB = 1
 FLAG_IQ_REVERSE = 2
@@ -232,7 +232,8 @@ class InspectorConfig(C.Structure):
                 ("clock_running", C.c_int32), ("audio_cutoff", C.c_float), ("audio_volume", C.c_float),
                 ("audio_squelch_level", C.c_float), ("agc_ts", C.c_float),
                 ("audio_sample_rate", C.c_uint32), ("audio_demod", C.c_uint32), ("audio_squelch", C.c_int32),
-                ("eq_type", C.c_uint32), ("eq_rate", C.c_float), ("eq_locked", C.c_int32)]
+                ("eq_type", C.c_uint32), ("eq_rate", C.c_float), ("eq_locked", C.c_int32),
+                ("power_integrate_samples", C.c_uint64)]
 
 
 _lib = None
@@ -418,6 +419,8 @@ _PROTOS = {
     "sdb_tv_processor_read_frame": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_size_t]),
     "sdb_tv_processor_estimates": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sdb_tv_feed_transform": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_float, C.c_float, C.c_void_p]),
+    "sdb_task_power": (C.c_long, [C.c_void_p, C.c_size_t, C.c_size_t, C.c_uint64, C.c_void_p, C.c_void_p,
+                                  C.c_size_t]),
     "sdb_task_inspector": (C.c_long, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_size_t]),
 }
@@ -827,6 +830,21 @@ def inspector_run(cls, fs, x, **kw):
     _check(L.sdb_task_inspector(C.byref(cfg), x.ctypes.data, n, batch, soft.ctypes.data, hard.ctypes.data,
                                 counts.ctypes.data, cap))
     return [(soft[b, :counts[b]].copy(), hard[b, :counts[b]].copy()) for b in range(batch)]
+
+
+def task_power(x, integrate_samples):
+    """Offline power inspector (SPEC PW) over captured channel-rate buffers: x [n] or [batch, n] complex64 ->
+    one complex64 array of (mean, 0) samples per buffer, each buffer integrated from an empty group."""
+    L = load_library()
+    x = np.ascontiguousarray(x, dtype=np.complex64)
+    if x.ndim == 1:
+        x = x[None, :]
+    batch, n = x.shape
+    cap = max(1, n // max(1, integrate_samples))
+    means = np.empty((batch, cap), np.complex64)
+    counts = np.zeros(batch, np.uint32)
+    _check(L.sdb_task_power(x.ctypes.data, n, batch, integrate_samples, means.ctypes.data, counts.ctypes.data, cap))
+    return [means[b, :counts[b]].copy() for b in range(batch)]
 
 
 class SnrEstimator:

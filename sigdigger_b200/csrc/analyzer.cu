@@ -72,11 +72,11 @@ struct Insp {
 };
 
 // class names in SDB_INSP_* order, as requests and inspector messages carry them
-const char *const kClassNames[] = { "psk", "fsk", "ask", "audio", "raw" };
+const char *const kClassNames[] = { "psk", "fsk", "ask", "audio", "raw", "power" };
 
 int class_id(const std::string &c)
 {
-  for (int k = SDB_INSP_PSK; k <= SDB_INSP_RAW; ++k)
+  for (int k = SDB_INSP_PSK; k <= SDB_INSP_POWER; ++k)
     if (c == kClassNames[k]) return k;
   return -1;
 }

@@ -44,9 +44,13 @@ struct Channel {
 };
 
 struct TimedSpan { int family; Event a, b; };
-enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_COUNT };
+enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_POWER, FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
-                                            "inspector", "psd_average" };
+                                            "inspector", "psd_average", "power" };
+
+// SPEC PW: samples per mean of a power inspector (power.integrate-samples, 0 read as 1)
+static uint64_t power_m(const sdb_inspector_config &c) { return c.power_integrate_samples ? c.power_integrate_samples : 1; }
+static bool is_power(const Channel &c) { return c.has_insp && c.cfg.insp_class == SDB_INSP_POWER; }
 
 struct ChdetDeleter { void operator()(sdb_chdet *d) const { sdb_chdet_destroy(d); } };
 
@@ -100,6 +104,10 @@ struct Plan {
   int *d_chain_map = nullptr; int insp_ctas = 0; std::vector<int> h_chain_map;
   float *d_taps = nullptr;
   size_t sym_cap = 0;
+  // power inspectors (SPEC PW; power_kernels.cu): one integrator per (power channel, stream), channel-major, and the
+  // partial group of every [stream][channel] (entries of other classes stay unused).  No power channel: both empty.
+  DevBuf<SdbPowerChain> d_power; int n_power = 0;
+  DevBuf<SdbPowerCarry> power_carry;
   // channel detector on the main PSD (SPEC K; chdet_kernels.cu)
   std::unique_ptr<sdb_chdet, ChdetDeleter> chdet;
   // inspector spectrum sources / estimators (SPEC U)
@@ -298,6 +306,9 @@ extern "C" int sdb_inspector_config_default(sdb_inspector_config *c, int insp_cl
   c->audio_cutoff = 5000.0f; c->audio_volume = 1.0f; c->audio_sample_rate = 44100;
   c->audio_demod = SDB_AUDIO_FM; c->agc_ts = 0.1f;
   c->eq_type = 0; c->eq_rate = 1e-3f; c->eq_locked = 0;
+  // a tenth of a second of channel samples (the upstream default is not known)
+  const double m = 0.1 * (double) fs;
+  c->power_integrate_samples = m > 1.0 ? (uint64_t) llround(m) : 1;
   return 0;
 }
 
@@ -340,7 +351,7 @@ extern "C" int sdb_engine_set_inspector(sdb_engine_t *e, int handle, const sdb_i
   if (!e || !cfg) return fail("null argument");
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");   // WRONG_HANDLE
   if (e->plan) return fail("engine already committed");
-  if (cfg->insp_class < SDB_INSP_PSK || cfg->insp_class > SDB_INSP_RAW) return fail("wrong kind");
+  if (cfg->insp_class < SDB_INSP_PSK || cfg->insp_class > SDB_INSP_POWER) return fail("wrong kind");
   Channel &c = e->channels[handle];
   c.cfg = *cfg; c.has_insp = true;
   c.cfg.fs = (float) (e->samp_rate * (double) c.size / (double) e->W);
@@ -456,13 +467,14 @@ extern "C" int sdb_engine_read_estimate(sdb_engine_t *e, int handle, int estimat
   return 0;
 }
 
-// sdb_inspector_config -> SdbChainCfg (SPEC X; same derivations as the inspector constructors)
+// sdb_inspector_config -> SdbChainCfg (SPEC X; same derivations as the inspector constructors).  A power inspector
+// keeps only its class: it has no chain (sdb_build_chain_map leaves it out).
 static bool build_chain_cfg(const Channel &ch, SdbChainCfg &c, std::vector<float> &taps_pool)
 {
   const sdb_inspector_config &g = ch.cfg;
   memset(&c, 0, sizeof(c));
   c.cls = ch.has_insp ? g.insp_class : SDB_INSP_RAW;
-  if (c.cls == SDB_INSP_RAW) return true;
+  if (c.cls == SDB_INSP_RAW || c.cls == SDB_INSP_POWER) return true;
   const float fs = g.fs;
   float bnor = g.baud / fs;
   if (bnor > 1.0f) bnor = 1.0f;
@@ -836,6 +848,20 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       }
       CK(cudaMemcpy(p.d_pool, hp.data(), pool_floats * sizeof(float), cudaMemcpyHostToDevice));
     }
+    // ---- power inspectors (SPEC PW): their groups start empty
+    std::vector<SdbPowerChain> pw;
+    for (int k = 0; k < K; ++k)
+      if (is_power(e->channels[k]))
+        for (unsigned s = 0; s < S; ++s)
+          pw.push_back(SdbPowerChain{ (size_t) s * p.chan_stride + p.h_chans[k].out_off, e->channels[k].halfsz,
+                                      s * (uint32_t) K + (uint32_t) k, power_m(e->channels[k].cfg) });
+    if (!pw.empty()) {
+      if (p.d_power.alloc(pw.size()) != cudaSuccess || p.power_carry.alloc(chains) != cudaSuccess)
+        return fail("out of device memory (power inspectors)");
+      p.n_power = (int) pw.size();
+      CK(cudaMemcpy(p.d_power, pw.data(), pw.size() * sizeof(SdbPowerChain), cudaMemcpyHostToDevice));
+      CK(cudaMemset(p.power_carry, 0, chains * sizeof(SdbPowerCarry)));
+    }
   }
   if (e->prm.flags & SDB_FLAG_DC_REMOVE) {
     p.d_dc_state = p.dalloc<float2>(S); p.d_dc_cur = p.dalloc<float2>(S);
@@ -1018,12 +1044,20 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
         CK(sdb_launch_spectsrc(ictx, p.d_spectcfg, p.d_chans, K, (int) S, p.spect_max_ns, sl.chan,
                                p.chan_stride, (uint32_t) wps, p.d_spect, p.spect_stride, p.d_spect_size,
                                p.d_est, p.d_est_valid));
-      e->span_begin(FAM_INSPECTOR, ictx.stream);
-      CK(sdb_launch_inspectors_n(ictx, p.d_cfg, K, (int) S, p.d_chain_map, p.insp_ctas, p.d_state, p.d_pool,
-                                 p.pool_stride, p.d_taps,
-                                 p.d_chans, sl.chan, p.chan_stride, (uint32_t) wps, sl.soft, sl.hard,
-                                 sl.counts, p.sym_cap, 0, sdb_insp_dyn(p.h_cfg.data(), K)));
-      e->span_end(ictx.stream);
+      if (p.insp_ctas > 0) {                      // (every channel a power inspector: no chain)
+        e->span_begin(FAM_INSPECTOR, ictx.stream);
+        CK(sdb_launch_inspectors_n(ictx, p.d_cfg, K, (int) S, p.d_chain_map, p.insp_ctas, p.d_state, p.d_pool,
+                                   p.pool_stride, p.d_taps,
+                                   p.d_chans, sl.chan, p.chan_stride, (uint32_t) wps, sl.soft, sl.hard,
+                                   sl.counts, p.sym_cap, 0, sdb_insp_dyn(p.h_cfg.data(), K)));
+        e->span_end(ictx.stream);
+      }
+      if (p.n_power) {
+        e->span_begin(FAM_POWER, ictx.stream);
+        CK(sdb_launch_power_integrate(ictx, p.d_power, p.n_power, sl.chan, (uint32_t) wps, p.power_carry, sl.soft,
+                                      sl.hard, sl.counts, p.sym_cap));
+        e->span_end(ictx.stream);
+      }
       CK(sl.insp.record(ictx.stream));
     } else {
       CK(sl.sym_read.wait_on(p.insp_stream));
@@ -1340,6 +1374,13 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
                       sizeof(float), S, cudaMemcpyDeviceToDevice));
     }
     if (!cn.has_insp || !co.has_insp) continue;
+    if (is_power(cn) || is_power(co)) {
+      // SPEC PW: the partial group goes on while the inspector stays a power inspector with the same M
+      if (is_power(cn) && is_power(co) && power_m(cn.cfg) == power_m(co.cfg))
+        CK(cudaMemcpy2D(to.power_carry + kn, (size_t) Kn * sizeof(SdbPowerCarry), from.power_carry + ko,
+                        (size_t) Ko * sizeof(SdbPowerCarry), sizeof(SdbPowerCarry), S, cudaMemcpyDeviceToDevice));
+      continue;
+    }
     const SdbChainCfg &a = to.h_cfg[kn], &b = from.h_cfg[ko];
     if (a.cls != b.cls || a.have_agc != b.have_agc || a.dl_size != b.dl_size || a.mh_size != b.mh_size ||
         a.have_mf != b.have_mf || a.mf_n != b.mf_n || a.af_n != b.af_n || a.alpf_n != b.alpf_n ||
@@ -1415,6 +1456,7 @@ extern "C" long sdb_task_inspector(const sdb_inspector_config *cfg, const sdb_co
                                    size_t batch, sdb_complex *soft, uint8_t *hard, uint32_t *counts, size_t cap)
 {
   if (!cfg || !src || !counts || n == 0 || batch == 0) return fail("invalid argument");
+  if (cfg->insp_class == SDB_INSP_POWER) return fail("invalid inspector configuration: the power class has no chain");
   if (sdb_device_count() <= 0) return fail("no CUDA device: sigdigger_b200 has no CPU fallback");
   Channel ch; memset(&ch.p, 0, sizeof(ch.p));
   ch.center = 0; ch.size = 2; ch.width = 2; ch.halfw = 1; ch.halfsz = 1; ch.has_insp = true; ch.cfg = *cfg;

@@ -355,9 +355,11 @@ static inline SdbInspDyn sdb_insp_dyn(const SdbChainCfg *cfgs, int n)
 #ifdef __cplusplus
 #include <vector>
 #include <algorithm>
+#include "../../include/sigdigger_b200.h"
 // CTA slot -> chain (channel-major index k * S + s) or -1.  A CTA holds chains of ONE inspector class so that its
 // role warps do not diverge (a single source with a psk / fsk / ask mix would otherwise execute all three carrier
-// stages in every warp); the classes with the longest recurrences come first so that their CTAs start first.
+// stages in every warp); the classes with the longest recurrences come first so that their CTAs start first.  Power
+// inspectors have no chain here: k_power_integrate serves them.
 static inline int sdb_build_chain_map(const SdbChainCfg *cfgs, int K, int S, std::vector<int> &map)
 {
   auto cost = [&](const SdbChainCfg &c) {          // rough per-sample cost order of the carrier stage
@@ -377,6 +379,7 @@ static inline int sdb_build_chain_map(const SdbChainCfg *cfgs, int K, int S, std
   int prev_key = -1;
   for (int idx = 0; idx < K; ++idx) {
     const int k = order[idx];
+    if (cfgs[k].cls == SDB_INSP_POWER) continue;   // served by k_power_integrate
     const int key = cost(cfgs[k]) * 8 + cfgs[k].cls;
     if (key != prev_key) while (map.size() % 32) map.push_back(-1);
     prev_key = key;
@@ -432,6 +435,18 @@ cudaError_t sdb_launch_spectsrc(const SdbLaunchCtx &c, const SdbSpectCfg *cfg_de
 cudaError_t sdb_launch_psd_group_mean(const SdbLaunchCtx &c, const float *psd, unsigned frames, unsigned n,
                                       size_t n_streams, unsigned A, unsigned carried, unsigned means, int shift_db,
                                       float *carry, float *out);
+// power_kernels.cu: the power inspector (SPEC PW).  One entry per (power channel, stream); the carry is indexed by
+// `out` like the symbol rows, [S][K] over every channel.
+struct SdbPowerChain {
+  size_t   in_off;          // offset (complex samples) of the chain's input in a slot's channel block: s * stride + out_off
+  uint32_t halfsz;          // channel samples per hop
+  uint32_t out;             // output row s * K + k of soft / hard / counts, and carry entry
+  unsigned long long M;     // samples per mean (>= 1)
+};
+struct SdbPowerCarry { double acc, c; unsigned long long n; };   // Kahan sum, its compensation, samples in the group
+cudaError_t sdb_launch_power_integrate(const SdbLaunchCtx &c, const SdbPowerChain *chains, int n_chains,
+                                       const float2 *chan_in, uint32_t n_hops, SdbPowerCarry *carry, float2 *soft,
+                                       uint8_t *hard, uint32_t *sym_counts, size_t sym_cap);
 // tasks_kernels.cu
 cudaError_t sdb_launch_dc_remove(cudaStream_t st, const void *x, int fmt, size_t stream_stride, size_t n, int n_streams,
                                  float alpha, float2 *state, float2 *cur, double2 *part, float2 *out);

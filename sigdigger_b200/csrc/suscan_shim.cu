@@ -125,6 +125,8 @@ const KeyDef kAudio[] = { { "audio.volume", 'f', "Audio gain" }, { "audio.cutoff
                           { "audio.sample-rate", 'i', "Audio sample rate" }, { "audio.demodulator", 'i', "Analog demodulator to use" },
                           { "audio.squelch", 'b', "Enable squelch" }, { "audio.squelch-level", 'f', "Squelch level" },
                           { "agc.ts", 'f', "AGC time scale" } };
+// the RMS tool (Default/RMSInspector/RMSInspector.cpp:404-416, 438-439): Suscan::Config::set(name, uint64_t)
+const KeyDef kPower[] = { { "power.integrate-samples", 'i', "Samples per integrated power reading" } };
 template <size_t N> void add(std::vector<KeyDef> &v, const KeyDef (&k)[N]) { v.insert(v.end(), k, k + N); }
 
 std::vector<KeyDef> keys_of(int cls)
@@ -135,6 +137,7 @@ std::vector<KeyDef> keys_of(int cls)
     case SDB_INSP_FSK: add(v, kGain); add(v, kFsk); add(v, kMf); add(v, kClock); break;
     case SDB_INSP_ASK: add(v, kGain); add(v, kAsk); add(v, kMf); add(v, kClock); break;
     case SDB_INSP_AUDIO: add(v, kGain); add(v, kAudio); break;
+    case SDB_INSP_POWER: add(v, kPower); break;
     default: break;
   }
   return v;
@@ -147,16 +150,18 @@ int class_of(const char *n)
   if (!strcmp(n, "ask")) return SDB_INSP_ASK;
   if (!strcmp(n, "audio")) return SDB_INSP_AUDIO;
   if (!strcmp(n, "raw")) return SDB_INSP_RAW;
+  if (!strcmp(n, "power")) return SDB_INSP_POWER;
   return -1;
 }
-const char *kClassNames[] = { "psk", "fsk", "ask", "audio", "raw" };
+const char *kClassNames[] = { "psk", "fsk", "ask", "audio", "raw", "power" };
+constexpr int kClasses = sizeof(kClassNames) / sizeof(kClassNames[0]);
 
 // one immutable descriptor per class, built on first use
 const suscan_config_desc_t *desc_of(int cls)
 {
   static std::mutex m;
-  static suscan_config_desc_t *descs[5] = { nullptr, nullptr, nullptr, nullptr, nullptr };
-  if (cls < 0 || cls > 4) return nullptr;
+  static suscan_config_desc_t *descs[kClasses] = {};
+  if (cls < 0 || cls >= kClasses) return nullptr;
   std::lock_guard<std::mutex> l(m);
   if (!descs[cls]) {
     auto keys = keys_of(cls);
@@ -283,6 +288,7 @@ void bag_from_cfg(suscan_config_t *b, const sdb_inspector_config &c)
   suscan_config_set_bool(b, "audio.squelch", c.audio_squelch);
   suscan_config_set_float(b, "audio.squelch-level", c.audio_squelch_level);
   suscan_config_set_float(b, "agc.ts", c.agc_ts);
+  suscan_config_set_integer(b, "power.integrate-samples", c.power_integrate_samples);
 }
 void cfg_from_bag(sdb_inspector_config &c, const suscan_config_t *b)
 {
@@ -302,6 +308,7 @@ void cfg_from_bag(sdb_inspector_config &c, const suscan_config_t *b)
   F("audio.volume", c.audio_volume); F("audio.cutoff", c.audio_cutoff); I("audio.sample-rate", c.audio_sample_rate);
   I("audio.demodulator", c.audio_demod); B("audio.squelch", c.audio_squelch); F("audio.squelch-level", c.audio_squelch_level);
   F("agc.ts", c.agc_ts);
+  if (auto *v = suscan_config_get_value(b, "power.integrate-samples")) c.power_integrate_samples = v->as_int;
 }
 }  // namespace
 
