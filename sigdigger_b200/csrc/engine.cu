@@ -236,11 +236,16 @@ static bool make_plan(Plan &pl, unsigned N, bool psd, SdbFourStep *fs)
 
 static bool uses_scratch(const SdbFourStep &fs) { return fs.path == SDB_FFT_F5 || fs.path == SDB_FFT_STOCKHAM; }
 
-// Windows per chunk of the four-step scratch, for the largest scratch transform `big` of the engine
+// Windows per chunk of the four-step scratch, for the largest scratch transform `big` of the engine.  Both passes of
+// both two-kernel paths put the window of the chunk on grid.y, so a chunk holds at most the device's grid.y limit
+// (65535 on an H100): 64 MB of 64- or 128-point channeliser windows would otherwise be 131072 or 65536 of them.
 static size_t scratch_chunk_windows(const SdbFourStep &big, int device)
 {
   const size_t window_bytes = (size_t) big.N * sizeof(float2);
   size_t cw = std::max<size_t>(1, ((size_t) 64 << 20) / window_bytes);
+  int max_grid_y = 0;
+  if (cudaDeviceGetAttribute(&max_grid_y, cudaDevAttrMaxGridDimY, device) == cudaSuccess && max_grid_y > 0)
+    cw = std::min(cw, (size_t) max_grid_y);
   if (big.path != SDB_FFT_F5) return cw;
   // SPEC F.5 path: 512 KB of windows per SM is whole waves of both passes (two 32768-point windows: 32 k_cols16T
   // CTAs at 8 per SM, 8 k_rows256 CTAs at 2 per SM).  On an H100 that is 69 MB, more than its 50 MB L2 can set

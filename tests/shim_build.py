@@ -3,9 +3,20 @@ libraries; shared by the CPU and GPU shim tests."""
 import ctypes as C
 import os
 import subprocess
+import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _lib = None
+_build_dir = None
+
+
+def build_dir():
+    """A private directory, removed at exit, for the shared objects the tests compile: the repository tree they run
+    from may be read-only."""
+    global _build_dir
+    if _build_dir is None:
+        _build_dir = tempfile.TemporaryDirectory(prefix="sdb-shim-tests-")
+    return _build_dir.name
 
 
 def reference_tu():
@@ -13,8 +24,7 @@ def reference_tu():
     if _lib is None:
         import sigdigger_b200
         sigdigger_b200.load_library()          # fails loudly if the native library was not built
-        so = os.path.join(ROOT, "tests", "shim", "_build", "libreftu.so")
-        os.makedirs(os.path.dirname(so), exist_ok=True)
+        so = os.path.join(build_dir(), "libreftu.so")
         libdir = os.path.join(ROOT, "sigdigger_b200")
         subprocess.run(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"),
                         os.path.join(ROOT, "tests", "shim", "reference_tu.cpp"), "-o", so, "-L", libdir, "-lsuscan",

@@ -5,7 +5,7 @@ bit-identical to the CPU oracle, within tolerance of the float64 statement of SP
 Inverse-side kernels by channel size (sdb_launch_chan_ifft_group): 4 ... 256 k_chan_ifft<1> (CTAs of at least one
 warp, so channels below 128 points leave threads idle), 512 ... 4096 k_chan_ifft16 (P = 8 / 4 / 2 / 1 hops per round,
 the last round of a feed partial), 8192 k_chan_ifft<2>, 16384 k_chan_ifft<4>.  Forward side by window: <= 4096 and
-131072 / 262144 the generic four-step, 8192 / 16384 / 32768 SPEC F.5 (bins compacted through the ka mask), 65536 the
+131072 ... 1048576 the generic four-step, 8192 / 16384 / 32768 SPEC F.5 (bins compacted through the ka mask), 65536 the
 fused cluster kernel."""
 import numpy as np
 import pytest
@@ -67,7 +67,7 @@ def _sized(W, sizes, precise=()):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("W", [64, 256, 1024, 4096, 8192, 16384, 32768, 65536, 131072, 262144])
+@pytest.mark.parametrize("W", [64, 256, 1024, 4096, 8192, 16384, 32768, 65536, 131072, 262144, 524288, 1048576])
 def test_band_edges_every_window(sdb, oracle, W):
     """DC, centres wrapping to 0, channels straddling DC from each side, full band (W <= 16384), minimum width,
     odd widths, overlapping channels, `precise` with both residual signs and a wrapped centre.  The first feed is
@@ -148,3 +148,49 @@ def test_size_limit(sdb, oracle):
     infos = [e.channel_info(h)]
     e.close()
     _check(oracle, x, W, chans, got, infos)
+
+
+# the windows of one feed counted here are those of its single stream; each case names the count and the PSD size
+LIMIT_CASES = [(128, 65535, 0), (128, 65535, 4096), (128, 65536, 0), (128, 65536, 4096), (64, 65536, 0),
+               (64, 65536, 4096), (64, 131072, 0), (64, 131072, 4096), (64, 131073, 0), (64, 131071, 4096)]
+
+
+def _limit_feeds(W, windows, psd_size):
+    """Feeds (samples) whose first or second one holds exactly `windows` forward transforms.  The first feed also
+    primes the first half window; with a 4096-point PSD every feed is a multiple of 4096 samples, so a count arrives
+    in the first feed (4096 k / hop - 1 windows) or in the second (4096 k / hop)."""
+    hop = W // 2
+    unit = max(hop, psd_size)
+    if (windows + 1) * hop % unit == 0:
+        return [(windows + 1) * hop, unit]
+    assert windows * hop % unit == 0, (W, windows, psd_size)
+    return [unit, windows * hop]
+
+
+@pytest.mark.parametrize("W,windows,psd_size", LIMIT_CASES)
+def test_small_window_feeds_past_the_grid_y_limit(sdb, oracle, W, windows, psd_size):
+    """64- and 128-point windows run on the generic four-step, whose scratch chunk is sized in bytes (64 MB: 131072
+    or 65536 such windows) while both of its kernels put the window on grid.y, limited to 65535.  Feeds of 65535,
+    65536, 131071, 131072 and 131073 windows, with no PSD and next to a 4096-point PSD (which takes the small-PSD path,
+    so the channeliser owns the scratch): every channel bit-identical to the oracle and within tolerance of st_f64."""
+    chans = [st.edge_channels(W)[i] for i in (0, 3, 11)]           # plain, straddling DC, `precise`
+    feeds = _limit_feeds(W, windows, psd_size)
+    x = st.signal(sum(feeds), chans, seed=windows % 61)[None, :]
+    e = sdb.Engine(n_streams=1, psd_size=psd_size, psd_window="hann", st_window_size=W, max_feed=max(feeds))
+    hs = [e.open_channel(c["f0"], c["bw"], c["guard"], c.get("precise", False)) for c in chans]
+    e.commit()
+    acc, off, psd = [[] for _ in hs], 0, []
+    for m in feeds:
+        e.feed(x[:, off:off + m])
+        off += m
+        for i, h in enumerate(hs):
+            acc[i].append(e.read_channel(0, h))
+        if psd_size:
+            psd.append(e.read_psd()[0].copy())
+    infos = [e.channel_info(h) for h in hs]
+    e.close()
+    assert windows in (feeds[0] // (W // 2) - 1, feeds[1] // (W // 2))
+    _check(oracle, x, W, chans, [[np.concatenate(a) for a in acc]], infos)
+    if psd_size:
+        ref = oracle.psd_frames(x[0], psd_size, "hann")
+        assert np.array_equal(np.concatenate(psd).view(np.uint32), ref.view(np.uint32))

@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 import power_oracle as P
+import shim_build as SB
 from sigdigger_b200 import synth
 
 pytestmark = pytest.mark.gpu
@@ -296,8 +297,7 @@ def test_shim_power_session(sdb):
     """Through libsuscan.so: open_async("power"), a "power" bag with power.integrate-samples set by
     suscan_config_set_integer, set_inspector_config_async; the SAMPLES' real parts equal the oracle over the channel
     samples from the block the configuration went live."""
-    so = os.path.join(ROOT, "tests", "shim", "_build", "libpowertu.so")
-    os.makedirs(os.path.dirname(so), exist_ok=True)
+    so = os.path.join(SB.build_dir(), "libpowertu.so")
     libdir = os.path.join(ROOT, "sigdigger_b200")
     subprocess.run(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"),
                     os.path.join(ROOT, "tests", "shim", "power_tu.cpp"), "-o", so, "-L", libdir, "-lsuscan",

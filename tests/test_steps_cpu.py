@@ -13,10 +13,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.mark.skipif(shutil.which("nvcc") is None, reason="needs nvcc to compile the host-side check")
-def test_select_forms_equal_statement_forms():
+def test_select_forms_equal_statement_forms(tmp_path):
     src = os.path.join(HERE, "shim", "steps_equiv.cu")
-    out = os.path.join(HERE, "shim", "_build", "steps_equiv")
-    os.makedirs(os.path.dirname(out), exist_ok=True)
+    out = str(tmp_path / "steps_equiv")                   # the repository tree may be read-only
     r = subprocess.run(["nvcc", "-O2", "-fmad=false", "-Xcompiler", "-ffp-contract=off",
                         "-I" + os.path.join(HERE, "..", "include"), "-o", out, src], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr[-2000:]
