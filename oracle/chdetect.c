@@ -38,6 +38,7 @@ unsigned sdo_chdet_feed(sdo_chdet *d, const float *psd, unsigned frames, sdo_cha
   const unsigned n = d->n, half = n / 2;
   unsigned f, k, count = 0, i, raw = 0;
   float n0_inst, thr;
+  if (frames == 0) return 0;                   /* K.2: a feed without frames changes nothing */
   for (f = 0; f < frames; ++f) {
     const float *p = psd + (size_t) f * n;
     if (!d->primed) { memcpy(d->avg, p, n * sizeof(float)); d->primed = 1; }
