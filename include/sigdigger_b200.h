@@ -61,8 +61,14 @@ typedef struct {
    * every A consecutive frames of each stream (the partial group carries across feeds; sdb_engine_read_psd_average).
    * With averaging on, SDB_FLAG_PSD_SHIFT_DB applies to the means only and the per-frame PSD stays linear. */
   uint32_t psd_average;
+  /* Peak detectors of the main PSD (SPEC PK, oracle/SPEC_PK.md): 0 or 1 = off; P in [2, SDB_PSD_PEAK_MAX] emits the
+   * per-bin maximum and minimum of every P consecutive frames of each stream (the partial group carries across feeds;
+   * sdb_engine_read_psd_peak).  With peak detection on, SDB_FLAG_PSD_SHIFT_DB applies to the extremes (and to the means
+   * when averaging is on as well) and the per-frame PSD stays linear. */
+  uint32_t psd_peak;
 } sdb_engine_params;
 #define SDB_PSD_AVERAGE_MAX 65536u
+#define SDB_PSD_PEAK_MAX 65536u
 
 /* SUSCAN_SOURCE_FORMAT_RAW_{FLOAT32, UNSIGNED8, SIGNED8, SIGNED16} (Default/SourceConfig/FileSourcePage.cpp:80-104):
  * interleaved I,Q pairs; 8/16-bit samples are converted inside the first load of the path (u8: (v-128)/128,
@@ -140,7 +146,8 @@ int sdb_inspector_config_default(sdb_inspector_config *cfg, int insp_class, floa
 int sdb_engine_commit(sdb_engine_t *e);
 /* Live re-plan: `dst` (committed, not yet fed) takes over the running state of `src` (same streams / window /
  * device): input history, the partial group of the frame-averaged PSD when psd_size, psd_window and psd_average match
- * (otherwise `dst` starts an empty group), and per channel with identical parameters the cross-fade tail, the LO phase
+ * (otherwise `dst` starts an empty group), the partial group of the peak detectors when psd_size, psd_window and
+ * psd_peak match (likewise), and per channel with identical parameters the cross-fade tail, the LO phase
  * and -- if the inspector class and the sizes of its state lines are unchanged -- the loop state of every chain; a power
  * inspector that stays one with the same power_integrate_samples keeps its partial group (SPEC PW).  This is how an
  * analyzer opens, closes, retunes or reconfigures ONE inspector at a block boundary while the others keep running
@@ -178,6 +185,14 @@ int          sdb_engine_read_psd(sdb_engine_t *e, float *dst, size_t cap_floats)
 size_t       sdb_engine_psd_average_frames(const sdb_engine_t *e);
 const float *sdb_engine_psd_average_device(const sdb_engine_t *e);
 int          sdb_engine_read_psd_average(sdb_engine_t *e, float *dst, size_t cap_floats);
+/* Peak detectors of the last feed (sdb_engine_params.psd_peak >= 2): two [stream][group][psd_size] float32 arrays, the
+ * per-bin maxima and minima of the groups the feed completed, linear with DC at 0 unless SDB_FLAG_PSD_SHIFT_DB.
+ * _groups: groups per stream (0 when peak detection is off); _device: the engine's buffer of the maxima (which = 0) or
+ * the minima (which = 1), valid until the feed after next; read: blocking copy of both, fenced like sdb_engine_read_psd,
+ * either destination may be NULL and cap_floats applies to each. */
+size_t       sdb_engine_psd_peak_groups(const sdb_engine_t *e);
+const float *sdb_engine_psd_peak_device(const sdb_engine_t *e, int which);
+int          sdb_engine_read_psd_peak(sdb_engine_t *e, float *max_dst, float *min_dst, size_t cap_floats);
 /* channel-rate output of the channeliser (what on_data delivers, Tasks/LPFTask.cpp:28-42) */
 long         sdb_engine_read_channel(sdb_engine_t *e, uint32_t stream, int handle, sdb_complex *dst,
                                      size_t cap);
@@ -243,7 +258,7 @@ typedef struct {
   uint32_t bin_lo, bin_hi;          /* [lo, hi) in ascending-frequency bin order */
 } sdb_detected_channel;
 /* engine-integrated: enable before sdb_engine_commit(); needs a linear per-frame PSD (no SDB_FLAG_PSD_SHIFT_DB, unless
- * psd_average >= 2 confines the flag to the means) */
+ * psd_average >= 2 or psd_peak >= 2 confines the flag to the group outputs) */
 int  sdb_engine_set_channel_detector(sdb_engine_t *e, float alpha, float beta, float gamma, float snr,
                                      uint32_t min_bins);
 /* channels of one stream after the latest feed (ascending frequency); *total = channels found before the
@@ -275,9 +290,10 @@ void    *sdb_engine_stream(const sdb_engine_t *e);
 uint64_t sdb_engine_launch_count(const sdb_engine_t *e);
 /* average device time (ms) of the named kernel family over the launches since the last reset, measured
  * with CUDA events on the engine stream; families: "fft_cols", "fft_rows_psd", "fft_rows_chan",
- * "chan_ifft", "inspector", "psd_average", "power".  A 65536-point plan's fused forward transform counts as "fft_cols";
- * its "fft_rows_psd" / "fft_rows_chan" stay at zero launches; "psd_average" (the group means) records none while
- * averaging is off, "power" (the power inspectors' integration) none while no channel has a power inspector */
+ * "chan_ifft", "inspector", "psd_average", "power", "psd_peak".  A 65536-point plan's fused forward transform counts as
+ * "fft_cols"; its "fft_rows_psd" / "fft_rows_chan" stay at zero launches; "psd_average" (the group means) records none
+ * while averaging is off, "power" (the power inspectors' integration) none while no channel has a power inspector,
+ * "psd_peak" (the group extremes) none while peak detection is off */
 int      sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches);
 void     sdb_engine_timing(sdb_engine_t *e, int enable);
 /* inspector-kernel stage balance since the last reset: out[0..3] = busy SM cycles of the gain / carrier /
@@ -469,7 +485,14 @@ typedef struct {
    * A = clamp(llround(psd_update_int * rate / window_size), 1, SDB_PSD_AVERAGE_MAX) frames (SPEC A), time-stamped at
    * its first sample; 0 = one frame per interval.  Wide-spectrum sweeps ignore it. */
   int32_t psd_average;
+  /* Channel mode: SDB_PSD_DETECTOR_POS_PEAK / _NEG_PEAK post, instead, the per-bin maximum / minimum of every
+   * P = clamp(llround(psd_update_int * rate / window_size), 1, SDB_PSD_PEAK_MAX) frames (SPEC PK), time-stamped at the
+   * first sample of the group; a detector takes precedence over psd_average.  SDB_PSD_DETECTOR_DEFAULT = one frame per
+   * interval, or the mean with psd_average.  sdb_analyzer_new and _set_params_async refuse other values; wide-spectrum
+   * sweeps ignore it. */
+  int32_t psd_detector;
 } sdb_analyzer_params;
+enum { SDB_PSD_DETECTOR_DEFAULT = 0, SDB_PSD_DETECTOR_POS_PEAK = 1, SDB_PSD_DETECTOR_NEG_PEAK = 2 };
 
 /* the part of suscan_source_config_t this path needs: a callback source (role of file / stdin / SoapySDR
  * back-ends) or an in-memory capture */

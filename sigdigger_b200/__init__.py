@@ -26,7 +26,8 @@ ESTIMATOR = {"baud-fac": 0, "baud-nonlinear": 1}
 class EngineParams(C.Structure):
     _fields_ = [("n_streams", C.c_uint32), ("psd_size", C.c_uint32), ("psd_window", C.c_int32),
                 ("st_window_size", C.c_uint32), ("max_feed", C.c_uint32), ("device", C.c_int32),
-                ("flags", C.c_uint32), ("input_format", C.c_int32), ("psd_average", C.c_uint32)]
+                ("flags", C.c_uint32), ("input_format", C.c_int32), ("psd_average", C.c_uint32),
+                ("psd_peak", C.c_uint32)]
 
 
 FORMAT = {"f32": 0, "u8": 1, "s8": 2, "s16": 3}
@@ -275,6 +276,9 @@ _PROTOS = {
     "sdb_engine_psd_average_frames": (C.c_size_t, [C.c_void_p]),
     "sdb_engine_psd_average_device": (C.c_void_p, [C.c_void_p]),
     "sdb_engine_read_psd_average": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "sdb_engine_psd_peak_groups": (C.c_size_t, [C.c_void_p]),
+    "sdb_engine_psd_peak_device": (C.c_void_p, [C.c_void_p, C.c_int]),
+    "sdb_engine_read_psd_peak": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "sdb_engine_read_channel": (C.c_long, [C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t]),
     "sdb_engine_read_symbols": (C.c_long, [C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t]),
     "sdb_engine_read_all_symbols": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
@@ -505,12 +509,13 @@ class Engine:
     """Batch analyzer engine: main PSD + channeliser + inspectors over S streams on one GPU."""
 
     def __init__(self, n_streams=1, psd_size=65536, psd_window="blackmann_harris", st_window_size=0,
-                 max_feed=0, samp_rate=1.0, device=0, flags=0, input_format="f32", psd_average=0):
-        """psd_average: A >= 2 also emits the mean of every A PSD frames (SPEC A, read_psd_average); 0 or 1 = off."""
+                 max_feed=0, samp_rate=1.0, device=0, flags=0, input_format="f32", psd_average=0, psd_peak=0):
+        """psd_average: A >= 2 also emits the mean of every A PSD frames (SPEC A, read_psd_average); 0 or 1 = off.
+        psd_peak: P >= 2 also emits the per-bin maximum and minimum of every P PSD frames (SPEC PK, read_psd_peak)."""
         L = load_library()
         self.input_format = FORMAT[input_format] if isinstance(input_format, str) else int(input_format)
         p = EngineParams(n_streams, psd_size, WINDOW[psd_window] if isinstance(psd_window, str) else psd_window,
-                         st_window_size, max_feed, device, flags, self.input_format, psd_average)
+                         st_window_size, max_feed, device, flags, self.input_format, psd_average, psd_peak)
         self._L = L
         self.n_streams, self.psd_size, self.samp_rate = n_streams, psd_size, samp_rate
         self.st_window_size = st_window_size or psd_size
@@ -606,6 +611,23 @@ class Engine:
     @property
     def psd_average_device_ptr(self):
         return self._L.sdb_engine_psd_average_device(self._h)
+
+    def read_psd_peak(self):
+        """-> (max, min), each [n_streams, groups, psd_size] float32: the group extremes the last feed completed
+        (SPEC PK)"""
+        g = self._L.sdb_engine_psd_peak_groups(self._h)
+        mx = np.empty((self.n_streams, g, self.psd_size), np.float32)
+        mn = np.empty_like(mx)
+        _check(self._L.sdb_engine_read_psd_peak(self._h, mx.ctypes.data, mn.ctypes.data, mx.size))
+        return mx, mn
+
+    def psd_peak_groups(self):
+        """groups per stream the last feed completed (0 when peak detection is off)"""
+        return self._L.sdb_engine_psd_peak_groups(self._h)
+
+    def psd_peak_device_ptr(self, which):
+        """device address of the maxima (which = 0) or the minima (which = 1) of the last feed"""
+        return self._L.sdb_engine_psd_peak_device(self._h, which)
 
     # ---- channel detector (SPEC K; detector_params of Suscan/AnalyzerParams.cpp:27-66)
     def set_channel_detector(self, alpha=0.01, beta=0.01, gamma=0.5, snr=4.0, min_bins=2):

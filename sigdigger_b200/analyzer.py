@@ -11,6 +11,8 @@ from . import INSP, WINDOW, InspectorConfig, SdbError, last_error, load_library
 MSG = {"SOURCE_INFO": 0, "SOURCE_INIT": 1, "CHANNEL": 2, "EOS": 3, "READ_ERROR": 4, "INTERNAL": 5, "SAMPLES": 6,
        "INSPECTOR": 7, "PSD": 8, "PARAMS": 9, "HALT": 0xffffffff, "TIMEOUT": 0xfffffffe}
 MSG_NAME = {v: k for k, v in MSG.items()}
+# sdb_analyzer_params.psd_detector (SPEC PK): which spectrum a PSD message carries
+PSD_DETECTOR = {"default": 0, "pos_peak": 1, "neg_peak": 2}
 KIND = {0: "OPEN", 1: "SET_ID", 2: "GET_CONFIG", 3: "SET_CONFIG", 4: "ESTIMATOR", 5: "SPECTRUM", 6: "CLOSE",
         7: "INVALID_CHANNEL", 8: "WRONG_HANDLE", 9: "WRONG_OBJECT", 10: "WRONG_KIND"}
 
@@ -31,7 +33,7 @@ class DetectorParams(C.Structure):
 class AnalyzerParams(C.Structure):
     _fields_ = [("mode", C.c_int32), ("detector_params", DetectorParams), ("channel_update_int", C.c_float),
                 ("psd_update_int", C.c_float), ("min_freq", C.c_double), ("max_freq", C.c_double),
-                ("psd_average", C.c_int32)]
+                ("psd_average", C.c_int32), ("psd_detector", C.c_int32)]
 
 
 READ_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.c_void_p, C.c_size_t)
@@ -83,9 +85,11 @@ class Analyzer:
     def __init__(self, samp_rate, window_size=8192, window="hann", psd_update_int=0.04, data=None, read=None,
                  read_size=0, loop=False, freq=0.0, device=0, channel_update_int=0.0, alpha=0.25, beta=0.25,
                  gamma=0.5, snr=8.0, wide=False, min_freq=0.0, max_freq=0.0, set_frequency=None, decimation=1,
-                 psd_average=0):
+                 psd_average=0, psd_detector=0):
         """decimation: source decimation D (SPEC L); the analyzer then runs at samp_rate / D.
-        psd_average: non-zero posts the mean of the frames of every psd_update_int instead of one frame (SPEC A)."""
+        psd_average: non-zero posts the mean of the frames of every psd_update_int instead of one frame (SPEC A).
+        psd_detector: "pos_peak" / "neg_peak" (or PSD_DETECTOR's numbers) post the per-bin maximum / minimum of those
+        frames instead (SPEC PK); 0 or "default" leaves the choice to psd_average."""
         self._L = load_library()
         p = AnalyzerParams()
         p.mode = 1 if wide else 0                      # SDB_ANALYZER_MODE_{CHANNEL, WIDE_SPECTRUM}
@@ -97,6 +101,7 @@ class Analyzer:
         p.psd_update_int = psd_update_int
         p.channel_update_int = channel_update_int
         p.psd_average = psd_average
+        p.psd_detector = PSD_DETECTOR[psd_detector] if isinstance(psd_detector, str) else psd_detector
         self.params = p
         s = SourceConfig()
         s.samp_rate, s.freq, s.read_size, s.loop, s.device = samp_rate, freq, read_size, int(loop), device
@@ -210,6 +215,8 @@ class Analyzer:
         for k, v in changes.items():
             if k in ("window_size", "window"):
                 setattr(p.detector_params, k, WINDOW[v] if k == "window" and isinstance(v, str) else v)
+            elif k == "psd_detector":
+                p.psd_detector = PSD_DETECTOR[v] if isinstance(v, str) else v
             elif hasattr(p, k):
                 setattr(p, k, v)
             else:
@@ -269,7 +276,7 @@ class Analyzer:
                 m = C.cast(ptr, C.POINTER(AnalyzerParams)).contents
                 out = dict(mode=m.mode, window_size=m.detector_params.window_size, window=m.detector_params.window,
                            psd_update_int=m.psd_update_int, channel_update_int=m.channel_update_int,
-                           psd_average=m.psd_average)
+                           psd_average=m.psd_average, psd_detector=m.psd_detector)
             elif name in ("EOS", "READ_ERROR", "HALT", "SOURCE_INIT"):
                 m = C.cast(ptr, C.POINTER(StatusMsg)).contents
                 out = dict(code=m.code, err_msg=(m.err_msg or b"").decode())

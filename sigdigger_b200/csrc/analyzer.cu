@@ -154,6 +154,9 @@ struct sdb_analyzer {
   // when A, N and the window stay, see sdb_engine_migrate)
   uint32_t avg_A = 0, avg_N = 0; int32_t avg_window = 0; bool avg_clamped = false;
   uint64_t avg_frames = 0;
+  // peak detectors (params.psd_detector, SPEC PK), kept the same way; pk_neg: post the minima instead of the maxima
+  uint32_t pk_P = 0, pk_N = 0; int32_t pk_window = 0; bool pk_clamped = false, pk_neg = false;
+  uint64_t pk_frames = 0;
   // source-side options of the worker loop (Suscan/Analyzer.cpp:117-135, 229-244; SourceWidget.cpp:1156-1184)
   bool iq_reverse = false, dc_remove = false;
   double throttle = 0;                                  // samples / s, 0 = as fast as the source delivers
@@ -319,16 +322,25 @@ struct sdb_analyzer {
     ep.device = src.device;
     ep.flags = (iq_reverse ? SDB_FLAG_IQ_REVERSE : 0) | (dc_remove ? SDB_FLAG_DC_REMOVE : 0);
     ep.input_format = src.read || dec ? SDB_FORMAT_FLOAT32 : src.input_format;
-    // frames per averaged PSD: the whole frames of one psd_update_int (1 = every frame, averaging off)
-    uint32_t A = 0;
-    avg_clamped = false;
-    if (params.psd_average) {
+    // the whole frames of one psd_update_int, clamped to [1, max]; *clamped says whether the clamp changed them
+    auto interval_frames = [&](uint32_t max, bool *clamped) {
       const double want = (double) params.psd_update_int * rate / (double) ep.psd_size;
       const long long r = want > 0 ? llround(std::min(want, 1e12)) : 0;
-      A = (uint32_t) std::min<long long>(std::max<long long>(r, 1), SDB_PSD_AVERAGE_MAX);
-      avg_clamped = (long long) A != r;
-    }
+      const uint32_t f = (uint32_t) std::min<long long>(std::max<long long>(r, 1), max);
+      *clamped = (long long) f != r;
+      return f;
+    };
+    // a peak detector takes precedence over averaging (SPEC PK.5)
+    const bool peaks = params.psd_detector != SDB_PSD_DETECTOR_DEFAULT;
+    // frames per averaged PSD (1 = every frame, averaging off) and per peak group (1 = every frame, its own extreme)
+    avg_clamped = pk_clamped = false;
+    const uint32_t A = params.psd_average && !peaks ? interval_frames(SDB_PSD_AVERAGE_MAX, &avg_clamped) : 0;
+    const uint32_t P = peaks ? interval_frames(SDB_PSD_PEAK_MAX, &pk_clamped) : 0;
     ep.psd_average = A;
+    ep.psd_peak = P;
+    pk_neg = params.psd_detector == SDB_PSD_DETECTOR_NEG_PEAK;
+    if (!old || P != pk_P || ep.psd_size != pk_N || ep.psd_window != pk_window) pk_frames = 0;
+    pk_P = P; pk_N = ep.psd_size; pk_window = ep.psd_window;
     if (!old || A != avg_A || ep.psd_size != avg_N || ep.psd_window != avg_window) avg_frames = 0;
     avg_A = A; avg_N = ep.psd_size; avg_window = ep.psd_window;
     eng = plan_level(ep, rate, -1, old_handle, old.get());
@@ -684,27 +696,35 @@ struct sdb_analyzer {
     measured_rate.store(el > 0 ? (double) total_samples / el : 0);
   }
 
-  // PSD messages at psd_update_int cadence of SIGNAL time (coverage = N / (fs * interval))
-  void publish_psd()
+  // PSD messages at psd_update_int cadence of SIGNAL time (coverage = N / (fs * interval)).  Internal to the library:
+  // hidden, so that the compiler's choice not to inline it adds no export.
+  __attribute__((visibility("hidden"))) void publish_psd()
   {
     const size_t N = (size_t) params.detector_params.window_size, frames = block / N;
-    if (avg_A >= 2) {
-      // the means the block completed, one per A frames; group j of the block starts j A - avg_frames frames after
-      // the block's first (earlier blocks hold its start when that is negative).  Unless A was clamped a mean lasts
-      // exactly the interval the credit is measured against, so every mean is posted.
-      const size_t means = sdb_engine_psd_average_frames(eng.get());
-      const uint64_t carried = avg_frames;
-      avg_frames = (avg_frames + frames) % avg_A;
-      psd.resize(means * N);
-      if (means && sdb_engine_read_psd_average(eng.get(), psd.data(), psd.size())) return;
-      const double per_mean = (double) avg_A * (double) N / rate;
-      const double interval = avg_clamped ? (double) params.psd_update_int : per_mean;
+    // the extremes (SPEC PK) or the means (SPEC A) of the groups the block completed, G frames each
+    const bool peaks = pk_P >= 2;
+    if (peaks || avg_A >= 2) {
+      const uint32_t G = peaks ? pk_P : avg_A;
+      uint64_t &open = peaks ? pk_frames : avg_frames;
+      const size_t groups = peaks ? sdb_engine_psd_peak_groups(eng.get()) : sdb_engine_psd_average_frames(eng.get());
+      // group j of the block starts j G - carried frames after the block's first (earlier blocks hold its start when
+      // that is negative).  Unless G was clamped a group lasts exactly the interval the credit is measured against, so
+      // every group is posted.
+      const uint64_t carried = open;
+      open = (open + frames) % G;
+      psd.resize(groups * N);
+      if (groups && (peaks ? sdb_engine_read_psd_peak(eng.get(), pk_neg ? nullptr : psd.data(),
+                                                      pk_neg ? psd.data() : nullptr, psd.size())
+                           : sdb_engine_read_psd_average(eng.get(), psd.data(), psd.size())))
+        return;
+      const double per_group = (double) G * (double) N / rate;
+      const double interval = (peaks ? pk_clamped : avg_clamped) ? (double) params.psd_update_int : per_group;
       const int64_t block_start = (int64_t) (total_samples - block * decim);
-      for (size_t j = 0; j < means; ++j) {
-        psd_credit += per_mean;
+      for (size_t j = 0; j < groups; ++j) {
+        psd_credit += per_group;
         if (psd_credit + 1e-12 >= interval) {
           psd_credit = fmod(psd_credit, interval);
-          const int64_t first = (int64_t) (j * avg_A) - (int64_t) carried;
+          const int64_t first = (int64_t) (j * G) - (int64_t) carried;
           post_psd((int64_t) src.freq, rate, &psd[j * N], N,
                    (double) (block_start + first * (int64_t) (N * decim)) / src.samp_rate, looped, (uint64_t) hist_fill);
         }
@@ -854,6 +874,11 @@ extern "C" sdb_analyzer_t *sdb_analyzer_new(const sdb_analyzer_params *params, c
   const uint64_t N = params->detector_params.window_size;
   if (N < 16 || (N & (N - 1)) || !(src->samp_rate > 0) || (!src->read && !src->data)) return nullptr;
   if (src->input_format < SDB_FORMAT_FLOAT32 || src->input_format > SDB_FORMAT_SIGNED16) return nullptr;
+  if (params->psd_detector < SDB_PSD_DETECTOR_DEFAULT || params->psd_detector > SDB_PSD_DETECTOR_NEG_PEAK) {
+    fail("psd_detector must be SDB_PSD_DETECTOR_DEFAULT, _POS_PEAK or _NEG_PEAK, got " +
+         std::to_string(params->psd_detector));
+    return nullptr;
+  }
   const uint32_t D = src->decimation ? src->decimation : 1;
   if (D > SDB_DECIMATION_MAX) {
     fail("source decimation must be at most " + std::to_string(SDB_DECIMATION_MAX) + ", got " + std::to_string(D));
@@ -1101,6 +1126,7 @@ extern "C" int sdb_analyzer_set_params_async(sdb_analyzer_t *a, const sdb_analyz
   if (!p) return -1;
   const uint64_t N = p->detector_params.window_size;
   if (N < 16 || (N & (N - 1))) return -1;
+  if (p->psd_detector < SDB_PSD_DETECTOR_DEFAULT || p->psd_detector > SDB_PSD_DETECTOR_NEG_PEAK) return -1;
   Cmd c; c.kind = Cmd::SET_PARAMS; c.req_id = req_id; c.params = *p;
   return push_cmd(a, std::move(c));
 }

@@ -44,9 +44,10 @@ struct Channel {
 };
 
 struct TimedSpan { int family; Event a, b; };
-enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_POWER, FAM_COUNT };
+enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_POWER, FAM_PSD_PEAK,
+       FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
-                                            "inspector", "psd_average", "power" };
+                                            "inspector", "psd_average", "power", "psd_peak" };
 
 // SPEC PW: samples per mean of a power inspector (power.integrate-samples, 0 read as 1)
 static uint64_t power_m(const sdb_inspector_config &c) { return c.power_integrate_samples ? c.power_integrate_samples : 1; }
@@ -59,6 +60,7 @@ struct ChdetDeleter { void operator()(sdb_chdet *d) const { sdb_chdet_destroy(d)
 struct Slot {
   float *psd = nullptr;                             // [S][frames][Np]
   float *psd_avg = nullptr;                         // [S][means][Np], frame averaging only (SPEC A)
+  float *psd_max = nullptr, *psd_min = nullptr;     // [S][groups][Np] each, peak detection only (SPEC PK)
   // channel streams: the (latency-bound, 1-CTA-per-32-chains) inspector kernel of feed i runs on its own stream
   // while the FFT kernels of feed i+1 fill the other slot
   float2 *chan = nullptr;
@@ -121,11 +123,14 @@ struct Plan {
   // stream: each feed has the same frames per stream)
   float *d_avg_carry = nullptr;         // [S][Np]
   unsigned avg_count = 0;
+  // peak detection (SPEC PK): per-stream partial maxima and minima of the current group, and its frame count
+  float *d_peak_max = nullptr, *d_peak_min = nullptr;   // [S][Np] each
+  unsigned peak_count = 0;
   // running state
   unsigned feed_index = 0, host_feeds = 0;
   bool first_feed = true;               // (engines without channels keep no history)
   uint64_t n_fed = 0;                   // samples fed so far
-  size_t last_frames = 0, last_hops = 0, last_means = 0;
+  size_t last_frames = 0, last_hops = 0, last_means = 0, last_peaks = 0;
 
   // the slot of the latest feed (slot 0 before the first)
   Slot &cur() { return slot[feed_index ? (feed_index - 1) & 1u : 0]; }
@@ -370,7 +375,7 @@ extern "C" int sdb_engine_set_channel_detector(sdb_engine_t *e, float alpha, flo
   if (!e) return fail("null argument");
   if (e->plan) return fail("engine already committed");
   if (!e->prm.psd_size) return fail("the channel detector needs the main PSD");
-  if ((e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) && e->prm.psd_average < 2)
+  if ((e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) && e->prm.psd_average < 2 && e->prm.psd_peak < 2)
     return fail("the channel detector needs a linear PSD");
   if (!(snr > 0.0f) || !(alpha >= 0.0f && alpha <= 1.0f) || !(gamma >= 0.0f && gamma <= 1.0f))
     return fail("detector parameters out of range");
@@ -616,6 +621,15 @@ static void pin_scratch(const sdb_engine *e, Plan &p, const SdbFourStep &big)
   }
 }
 
+// the group size of the frame-averaged PSD (SPEC A.1) or of the peak detectors (SPEC PK.1): 0 or 1 = off, at most
+// `max`, and only with a main PSD
+static int check_group_size(const char *name, unsigned v, unsigned max, unsigned Np)
+{
+  if (v > max) return fail(std::string(name) + " must be at most " + std::to_string(max) + ", got " + std::to_string(v));
+  if (v >= 2 && !Np) return fail(std::string(name) + " needs the main PSD (psd_size > 0)");
+  return 0;
+}
+
 extern "C" int sdb_engine_commit(sdb_engine_t *e)
 {
   if (!e) return fail("null engine");
@@ -627,10 +641,9 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
   if (max_feed == 0) return fail("max_feed must be > 0");
   if (max_feed % (W / 2)) return fail("max_feed must be a multiple of st_window_size / 2");
   if (Np && max_feed % Np) return fail("max_feed must be a multiple of psd_size");
-  const unsigned A = e->prm.psd_average;
-  if (A > SDB_PSD_AVERAGE_MAX)
-    return fail("psd_average must be at most " + std::to_string(SDB_PSD_AVERAGE_MAX) + ", got " + std::to_string(A));
-  if (A >= 2 && !Np) return fail("psd_average needs the main PSD (psd_size > 0)");
+  const unsigned A = e->prm.psd_average, P = e->prm.psd_peak;
+  if (check_group_size("psd_average", A, SDB_PSD_AVERAGE_MAX, Np) || check_group_size("psd_peak", P, SDB_PSD_PEAK_MAX, Np))
+    return -1;
   // built here and handed to the engine at the end: every early return frees what was built so far
   auto plan = std::make_unique<Plan>();
   Plan &p = *plan;
@@ -660,6 +673,18 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       p.d_avg_carry = p.dalloc<float>((size_t) S * Np);
       if (!p.d_avg_carry) return fail("out of device memory (averaged psd)");
       CK(cudaMemset(p.d_avg_carry, 0, (size_t) S * Np * sizeof(float)));
+    }
+    if (P >= 2) {
+      // as for the means: at most ceil(max_frames / P) groups a feed, each written to both outputs
+      const size_t max_groups = (max_frames + P - 1) / P;
+      for (Slot &sl : p.slot) {
+        sl.psd_max = p.dalloc<float>((size_t) S * max_groups * Np);
+        sl.psd_min = p.dalloc<float>((size_t) S * max_groups * Np);
+        if (!sl.psd_max || !sl.psd_min) return fail("out of device memory (psd peaks)");
+      }
+      p.d_peak_max = p.dalloc<float>((size_t) S * Np);
+      p.d_peak_min = p.dalloc<float>((size_t) S * Np);
+      if (!p.d_peak_max || !p.d_peak_min) return fail("out of device memory (psd peaks)");
     }
     if (e->cd_enabled) {
       p.chdet.reset(sdb_chdet_new(e->prm.device, Np, S, e->cd_alpha, e->cd_gamma, e->cd_snr, e->cd_min_bins));
@@ -909,9 +934,10 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     x = p.d_xdc; fmt = SDB_FMT_F32; stride = n;
   }
   SdbLaunchCtx ctx{ e->stream, &e->launches };
-  // with frame averaging the flag applies to the means: the transforms keep the per-frame PSD linear
-  const int means_db = (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) ? 1 : 0;
-  const int shift_db = p.d_avg_carry ? 0 : means_db;
+  // with frame averaging or peak detection the flag applies to their group outputs: the transforms keep the per-frame
+  // PSD linear
+  const int groups_db = (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) ? 1 : 0;
+  const int shift_db = p.d_avg_carry || p.d_peak_max ? 0 : groups_db;
   Slot &sl = p.slot[p.feed_index & 1u];     // result buffers of this feed
 
   const int frames = Np ? (int) (n / Np) : 0;
@@ -920,11 +946,23 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     if (!p.d_avg_carry) return 0;
     const unsigned A = e->prm.psd_average, means = (p.avg_count + (unsigned) frames) / A;
     e->span_begin(FAM_PSD_AVERAGE, lc.stream);
-    CK(sdb_launch_psd_group_mean(lc, sl.psd, (unsigned) frames, Np, S, A, p.avg_count, means, means_db,
+    CK(sdb_launch_psd_group_mean(lc, sl.psd, (unsigned) frames, Np, S, A, p.avg_count, means, groups_db,
                                  p.d_avg_carry, sl.psd_avg));
     e->span_end(lc.stream);
     p.avg_count = (p.avg_count + (unsigned) frames) % A;
     p.last_means = means;
+    return 0;
+  };
+  // SPEC PK group extremes of this feed, on the same stream, after the means
+  auto group_peaks = [&](const SdbLaunchCtx &lc) -> int {
+    if (!p.d_peak_max) return 0;
+    const unsigned P = e->prm.psd_peak, groups = (p.peak_count + (unsigned) frames) / P;
+    e->span_begin(FAM_PSD_PEAK, lc.stream);
+    CK(sdb_launch_psd_group_peak(lc, sl.psd, (unsigned) frames, Np, S, P, p.peak_count, groups, groups_db,
+                                 p.d_peak_max, p.d_peak_min, sl.psd_max, sl.psd_min));
+    e->span_end(lc.stream);
+    p.peak_count = (p.peak_count + (unsigned) frames) % P;
+    p.last_peaks = groups;
     return 0;
   };
   const int H = K ? (int) (n / (W / 2)) : 0;
@@ -986,7 +1024,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     }
     if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, p.psd_stream,
                                           &e->launches));
-    if (group_means(pctx)) return -1;
+    if (group_means(pctx) || group_peaks(pctx)) return -1;
     CK(sl.psd_ready.record(p.psd_stream));
     CK(sl.psd_ready.wait_on(e->stream));          // the main stream stays the engine's timeline
   } else {
@@ -1019,7 +1057,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
       }
       if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, e->stream,
                                             &e->launches));
-      if (group_means(ctx)) return -1;
+      if (group_means(ctx) || group_peaks(ctx)) return -1;
       CK(sl.psd_ready.record(e->stream));
     }
     // ---- channeliser forward transforms
@@ -1165,6 +1203,32 @@ extern "C" int sdb_engine_read_psd_average(sdb_engine_t *e, float *dst, size_t c
   CK(cudaSetDevice(e->prm.device));
   CK(sl.psd_ready.wait_on(p.d2h_stream));
   CK(cudaMemcpyAsync(dst, sl.psd_avg, n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
+  CK(sl.psd_read.record(p.d2h_stream));
+  CK(cudaStreamSynchronize(p.d2h_stream));
+  return 0;
+}
+
+extern "C" size_t sdb_engine_psd_peak_groups(const sdb_engine_t *e) { return e && e->plan ? e->plan->last_peaks : 0; }
+extern "C" const float *sdb_engine_psd_peak_device(const sdb_engine_t *e, int which)
+{
+  if (!e || !e->plan || (which != 0 && which != 1)) return nullptr;
+  return which ? e->plan->cur().psd_min : e->plan->cur().psd_max;
+}
+
+extern "C" int sdb_engine_read_psd_peak(sdb_engine_t *e, float *max_dst, float *min_dst, size_t cap)
+{
+  if (!e) return fail("null argument");
+  if (!e->plan || !e->plan->d_peak_max) return fail("PSD peak detection not enabled");
+  Plan &p = *e->plan;
+  if (p.feed_index == 0) return fail("no PSD available");
+  const size_t n = (size_t) e->prm.n_streams * p.last_peaks * e->Np;
+  if (cap < n) return fail("destination too small");
+  if (n == 0 || (!max_dst && !min_dst)) return 0;
+  Slot &sl = p.cur();
+  CK(cudaSetDevice(e->prm.device));
+  CK(sl.psd_ready.wait_on(p.d2h_stream));
+  if (max_dst) CK(cudaMemcpyAsync(max_dst, sl.psd_max, n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
+  if (min_dst) CK(cudaMemcpyAsync(min_dst, sl.psd_min, n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
   CK(sl.psd_read.record(p.d2h_stream));
   CK(cudaStreamSynchronize(p.d2h_stream));
   return 0;
@@ -1357,6 +1421,13 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
       dst->prm.psd_average == src->prm.psd_average) {
     CK(cudaMemcpy(to.d_avg_carry, from.d_avg_carry, (size_t) S * dst->Np * sizeof(float), cudaMemcpyDeviceToDevice));
     to.avg_count = from.avg_count;
+  }
+  // the partial SPEC PK group, under the same condition
+  if (to.d_peak_max && from.d_peak_max && dst->Np == src->Np && dst->prm.psd_window == src->prm.psd_window &&
+      dst->prm.psd_peak == src->prm.psd_peak) {
+    CK(cudaMemcpy(to.d_peak_max, from.d_peak_max, (size_t) S * dst->Np * sizeof(float), cudaMemcpyDeviceToDevice));
+    CK(cudaMemcpy(to.d_peak_min, from.d_peak_min, (size_t) S * dst->Np * sizeof(float), cudaMemcpyDeviceToDevice));
+    to.peak_count = from.peak_count;
   }
   // an engine that had no channel so far kept no input history: its first window starts with this feed
   to.first_feed = from.d_hist ? from.first_feed : true;

@@ -435,6 +435,12 @@ cudaError_t sdb_launch_spectsrc(const SdbLaunchCtx &c, const SdbSpectCfg *cfg_de
 cudaError_t sdb_launch_psd_group_mean(const SdbLaunchCtx &c, const float *psd, unsigned frames, unsigned n,
                                       size_t n_streams, unsigned A, unsigned carried, unsigned means, int shift_db,
                                       float *carry, float *out);
+// sview_kernels.cu: peak detectors of the main PSD (SPEC PK); psd [S][frames][n] -> out_max, out_min [S][groups][n],
+// carry_max, carry_min [S][n]; n a power of two >= 16.  Internal to the library: not exported.
+__attribute__((visibility("hidden")))
+cudaError_t sdb_launch_psd_group_peak(const SdbLaunchCtx &c, const float *psd, unsigned frames, unsigned n,
+                                      size_t n_streams, unsigned P, unsigned carried, unsigned groups, int shift_db,
+                                      float *carry_max, float *carry_min, float *out_max, float *out_min);
 // power_kernels.cu: the power inspector (SPEC PW).  One entry per (power channel, stream); the carry is indexed by
 // `out` like the symbol rows, [S][K] over every channel.
 struct SdbPowerChain {

@@ -493,6 +493,83 @@ cudaError_t sdb_launch_psd_group_mean(const SdbLaunchCtx &c, const float *psd, u
   return cudaGetLastError();
 }
 
+// Peak detectors of the main PSD (SPEC PK, oracle/SPEC_PK.md): per (stream, bin), the frames of the feed update the
+// carried group maximum and minimum with fmaxf / fminf (maxNum / minNum: a NaN operand is ignored); every P-th frame of
+// the running count finishes a group, written to both outputs (fft-shifted and in dB with shift_db, the expression of
+// k_psd_shift_db, after the extreme is taken).  An empty group holds NaN, which the group's first frame replaces
+// (fmaxf(NaN, x) = x): that is PK.2's "the first frame starts the value" without a branch.  psd is [S][frames][n],
+// outputs [S][groups][n], carries [S][n]; `carried` frames of the current group precede this feed.
+// Each thread owns 4 consecutive bins (n is a power of two >= 16, so a float4 never straddles a stream or the fft-shift
+// seam, and every row is 16-byte aligned): loads and stores are 16-byte and coalesced across the warp, and the frame
+// loop issues UNROLL independent loads before the compares.  4 bins a thread moved more bytes per second than 1 on an
+// H100 (DESIGN.md, kernel table).
+#define SDB_PEAK_UNROLL 8
+static __device__ __forceinline__ float4 peak_fmax4(float4 a, float4 b)
+{
+  return make_float4(fmaxf(a.x, b.x), fmaxf(a.y, b.y), fmaxf(a.z, b.z), fmaxf(a.w, b.w));
+}
+static __device__ __forceinline__ float4 peak_fmin4(float4 a, float4 b)
+{
+  return make_float4(fminf(a.x, b.x), fminf(a.y, b.y), fminf(a.z, b.z), fminf(a.w, b.w));
+}
+static __device__ __forceinline__ float4 peak_out4(float4 a, int shift_db)
+{
+  if (!shift_db) return a;
+  return make_float4(10.0f * d_log10f(a.x + 1e-8f), 10.0f * d_log10f(a.y + 1e-8f), 10.0f * d_log10f(a.z + 1e-8f),
+                     10.0f * d_log10f(a.w + 1e-8f));
+}
+
+static __global__ void __launch_bounds__(256) k_psd_group_peak(const float4 *__restrict__ psd, unsigned frames,
+                                                                unsigned n4, size_t n_streams, unsigned P,
+                                                                unsigned carried, unsigned groups, int shift_db,
+                                                                float4 *__restrict__ carry_max,
+                                                                float4 *__restrict__ carry_min,
+                                                                float4 *__restrict__ out_max,
+                                                                float4 *__restrict__ out_min)
+{
+  const size_t t = blockIdx.x * (size_t) blockDim.x + threadIdx.x;
+  if (t >= n_streams * n4) return;
+  const size_t s = t / n4;
+  const unsigned k4 = (unsigned) (t - s * n4);
+  const float4 *__restrict__ x = psd + s * (size_t) frames * n4 + k4;
+  size_t o = s * (size_t) groups * n4 + (shift_db ? ((k4 + (n4 >> 1)) & (n4 - 1)) : k4);
+  const float q = __int_as_float(0x7fffffff);
+  const float4 empty = make_float4(q, q, q, q);
+  // as in k_psd_group_mean, the carries move only while a group stays open across a feed boundary
+  float4 mx = carried ? carry_max[t] : empty, mn = carried ? carry_min[t] : empty;
+  unsigned cnt = carried;
+  for (unsigned f0 = 0; f0 < frames; f0 += SDB_PEAK_UNROLL) {
+    float4 v[SDB_PEAK_UNROLL];
+#pragma unroll
+    for (int u = 0; u < SDB_PEAK_UNROLL; ++u) v[u] = f0 + u < frames ? __ldg(x + (size_t) (f0 + u) * n4) : empty;
+#pragma unroll
+    for (int u = 0; u < SDB_PEAK_UNROLL; ++u) {
+      if (f0 + u < frames) {
+        mx = peak_fmax4(mx, v[u]); mn = peak_fmin4(mn, v[u]);
+        if (++cnt == P) {
+          out_max[o] = peak_out4(mx, shift_db); out_min[o] = peak_out4(mn, shift_db);
+          o += n4; mx = mn = empty; cnt = 0;
+        }
+      }
+    }
+  }
+  if (cnt) { carry_max[t] = mx; carry_min[t] = mn; }
+}
+
+cudaError_t sdb_launch_psd_group_peak(const SdbLaunchCtx &c, const float *psd, unsigned frames, unsigned n,
+                                      size_t n_streams, unsigned P, unsigned carried, unsigned groups, int shift_db,
+                                      float *carry_max, float *carry_min, float *out_max, float *out_min)
+{
+  if (frames == 0 || n_streams * n == 0) return cudaSuccess;
+  const size_t threads = n_streams * (n / 4);
+  k_psd_group_peak<<<(unsigned) ((threads + 255) / 256), 256, 0, c.stream>>>(
+      reinterpret_cast<const float4 *>(psd), frames, n / 4, n_streams, P, carried, groups, shift_db,
+      reinterpret_cast<float4 *>(carry_max), reinterpret_cast<float4 *>(carry_min), reinterpret_cast<float4 *>(out_max),
+      reinterpret_cast<float4 *>(out_min));
+  if (c.launch_counter) ++*c.launch_counter;
+  return cudaGetLastError();
+}
+
 static cudaError_t sdb_launch_psd_shift_db(cudaStream_t s, const float *lin, float *db, size_t n_frames, unsigned n)
 {
   const size_t total = n_frames * n;
