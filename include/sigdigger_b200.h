@@ -245,6 +245,22 @@ int sdb_engine_set_estimator(sdb_engine_t *e, int handle, int estimator_id, int 
 int sdb_engine_read_spectrum(sdb_engine_t *e, int handle, float *out, uint32_t *sizes);
 /* latest estimates of one channel, all streams: values[n_streams], valid[n_streams] */
 int sdb_engine_read_estimate(sdb_engine_t *e, int handle, int estimator_id, float *values, int32_t *valid);
+/* Scheduled spectra and estimates (oracle/SPEC_US.md): with an interval I >= 1, the channel emits at every t_j = j I
+ * channel samples since it started (from t_j >= size + 1 on) over the frame c[t_j - size - 1 .. t_j - 1], carried
+ * across feeds, so that narrow channels emit and wide ones emit at a fixed rate whatever the feed size.  I = 0 (the
+ * default) keeps one emission per feed as above.  Call before sdb_engine_commit() on a channel with a spectrum
+ * source or an estimator.  A feed emits at most ceil(max_feed channel samples / I) <= SDB_SPECTRUM_EMITS_MAX times;
+ * commit refuses a larger count.  The ring of the last size + 1 samples costs n_streams (size + 1) 8 bytes. */
+#define SDB_SPECTRUM_EMITS_MAX 256
+#define SDB_SPECTRUM_INTERVAL_MAX (1ull << 62)   /* larger intervals are refused */
+int  sdb_engine_set_spectrum_interval(sdb_engine_t *e, int handle, uint64_t interval);
+/* every emission of the last feed, all streams: out[n_streams][cap][out_size] (out_size = size, or size / 2 for
+ * "fac"), ends[cap] = t_j of each emission (the same in every stream).  Returns the emission count (<= cap; the same
+ * for every stream), -1 on error.  On a scheduled channel sdb_engine_read_spectrum / _read_estimate give the last
+ * emission of the feed, or size 0 / invalid when it had none. */
+long sdb_engine_read_spectra(sdb_engine_t *e, int handle, float *out, uint64_t *ends, size_t cap);
+/* values[n_streams][cap], valid[n_streams][cap] of every emission of the last feed; returns the emission count */
+long sdb_engine_read_estimates(sdb_engine_t *e, int handle, int estimator_id, float *values, int32_t *valid, size_t cap);
 
 /* ---- channel detector on the main PSD (SURVEY.md 8(f) rank 3; SPEC.md section K) ----
  * struct suscan_analyzer_params.detector_params.{alpha, beta, gamma, snr} + channel_update_int
@@ -290,10 +306,11 @@ void    *sdb_engine_stream(const sdb_engine_t *e);
 uint64_t sdb_engine_launch_count(const sdb_engine_t *e);
 /* average device time (ms) of the named kernel family over the launches since the last reset, measured
  * with CUDA events on the engine stream; families: "fft_cols", "fft_rows_psd", "fft_rows_chan",
- * "chan_ifft", "inspector", "psd_average", "power", "psd_peak".  A 65536-point plan's fused forward transform counts as
+ * "chan_ifft", "inspector", "psd_average", "power", "psd_peak", "spectsrc_sched".  A 65536-point plan's fused forward transform counts as
  * "fft_cols"; its "fft_rows_psd" / "fft_rows_chan" stay at zero launches; "psd_average" (the group means) records none
  * while averaging is off, "power" (the power inspectors' integration) none while no channel has a power inspector,
- * "psd_peak" (the group extremes) none while peak detection is off */
+ * "psd_peak" (the group extremes) none while peak detection is off, "spectsrc_sched" (the scheduled spectra: frame
+ * gather, transforms and ring update) none in a feed that neither emits nor keeps samples */
 int      sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches);
 void     sdb_engine_timing(sdb_engine_t *e, int enable);
 /* inspector-kernel stage balance since the last reset: out[0..3] = busy SM cycles of the gain / carrier /
@@ -491,6 +508,14 @@ typedef struct {
    * interval, or the mean with psd_average.  sdb_analyzer_new and _set_params_async refuse other values; wide-spectrum
    * sweeps ignore it. */
   int32_t psd_detector;
+  /* Seconds between inspector spectra and baud estimates.  > 0: every inspector with a spectrum source or an
+   * estimator takes 4096-point frames from a window carried across blocks and emits every
+   * I = max(1, llround(spectrum_update_int * channel rate)) channel samples (oracle/SPEC_US.md), one SPECTRUM message
+   * and one ESTIMATOR message per valid estimate each time, in order, after the block's SAMPLES.  An I that would
+   * allow more than SDB_SPECTRUM_EMITS_MAX emissions in one block is raised to ceil(channel samples per block /
+   * SDB_SPECTRUM_EMITS_MAX).  0 = one emission per block that fills a frame, of the largest power of two <= 4096 the
+   * block fills.  sdb_analyzer_new and _set_params_async refuse negative values, infinities and NaN. */
+  float   spectrum_update_int;
 } sdb_analyzer_params;
 enum { SDB_PSD_DETECTOR_DEFAULT = 0, SDB_PSD_DETECTOR_POS_PEAK = 1, SDB_PSD_DETECTOR_NEG_PEAK = 2 };
 

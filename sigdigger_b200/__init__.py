@@ -296,6 +296,9 @@ _PROTOS = {
     "sdb_engine_set_estimator": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "sdb_engine_read_spectrum": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_read_estimate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdb_engine_set_spectrum_interval": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
+    "sdb_engine_read_spectra": (C.c_long, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "sdb_engine_read_estimates": (C.c_long, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t]),
     "sdb_engine_set_channel_detector": (C.c_int, [C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_uint32]),
     "sdb_engine_read_channels": (C.c_long, [C.c_void_p, C.c_uint32, C.c_double, C.c_void_p, C.c_size_t, C.c_void_p]),
     "sdb_chdet_new": (C.c_void_p, [C.c_int, C.c_uint32, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_uint32]),
@@ -519,7 +522,7 @@ class Engine:
         self._L = L
         self.n_streams, self.psd_size, self.samp_rate = n_streams, psd_size, samp_rate
         self.st_window_size = st_window_size or psd_size
-        self.device = device
+        self.device, self.max_feed = device, max_feed
         self._h = L.sdb_engine_new(C.byref(p), samp_rate)
         if not self._h:
             raise SdbError(last_error())
@@ -646,6 +649,8 @@ class Engine:
         _check(self._L.sdb_engine_set_spectrum_source(self._h, h, k, size))
         self._spect_size = getattr(self, "_spect_size", {})
         self._spect_size[h] = size
+        self._spect_kind = getattr(self, "_spect_kind", {})
+        self._spect_kind[h] = k
 
     def set_estimator(self, h, estimator, enabled=True):
         e = ESTIMATOR[estimator] if isinstance(estimator, str) else int(estimator)
@@ -665,6 +670,38 @@ class Engine:
         valid = np.zeros(self.n_streams, np.int32)
         _check(self._L.sdb_engine_read_estimate(self._h, h, e, vals.ctypes.data, valid.ctypes.data))
         return vals, valid
+
+    def set_spectrum_interval(self, h, interval):
+        """Emit h's spectrum and estimates every `interval` channel samples, from a window carried across feeds
+        (SPEC US); 0 = once per feed (SPEC U.1).  Before commit."""
+        _check(self._L.sdb_engine_set_spectrum_interval(self._h, h, int(interval)))
+        self._spect_interval = getattr(self, "_spect_interval", {})
+        self._spect_interval[h] = int(interval)
+
+    def _emits_cap(self, h):
+        # ceil(channel samples per max_feed / I): what one feed can emit
+        n_max = (self.max_feed // (self.st_window_size // 2)) * (self.channel_info(h).size // 2)
+        return -(-n_max // self._spect_interval[h])
+
+    def read_spectra(self, h):
+        """-> (spectra [n_streams, emissions, out_size] float32, ends [emissions] uint64: t_j of each): every emission
+        of the last feed on a scheduled channel (SPEC US); out_size = size, or size / 2 for "fac"."""
+        cap = self._emits_cap(h)
+        size = getattr(self, "_spect_size", {}).get(h, 1024)
+        w = size // 2 if getattr(self, "_spect_kind", {}).get(h) == SPECTSRC["fac"] else size
+        out = np.zeros((self.n_streams, cap, w), np.float32)
+        ends = np.zeros(cap, np.uint64)
+        n = _check(self._L.sdb_engine_read_spectra(self._h, h, out.ctypes.data, ends.ctypes.data, cap))
+        return out[:, :n].copy(), ends[:n].copy()
+
+    def read_estimates(self, h, estimator):
+        """-> (values [n_streams, emissions] float32, valid [n_streams, emissions] int32) of the last feed (SPEC US)"""
+        e = ESTIMATOR[estimator] if isinstance(estimator, str) else int(estimator)
+        cap = self._emits_cap(h)
+        vals = np.zeros((self.n_streams, cap), np.float32)
+        valid = np.zeros((self.n_streams, cap), np.int32)
+        n = _check(self._L.sdb_engine_read_estimates(self._h, h, e, vals.ctypes.data, valid.ctypes.data, cap))
+        return vals[:, :n].copy(), valid[:, :n].copy()
 
     def read_channel(self, stream, h, cap=None):
         cap = cap or (1 << 24)

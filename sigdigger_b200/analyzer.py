@@ -33,7 +33,7 @@ class DetectorParams(C.Structure):
 class AnalyzerParams(C.Structure):
     _fields_ = [("mode", C.c_int32), ("detector_params", DetectorParams), ("channel_update_int", C.c_float),
                 ("psd_update_int", C.c_float), ("min_freq", C.c_double), ("max_freq", C.c_double),
-                ("psd_average", C.c_int32), ("psd_detector", C.c_int32)]
+                ("psd_average", C.c_int32), ("psd_detector", C.c_int32), ("spectrum_update_int", C.c_float)]
 
 
 READ_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.c_void_p, C.c_size_t)
@@ -85,11 +85,13 @@ class Analyzer:
     def __init__(self, samp_rate, window_size=8192, window="hann", psd_update_int=0.04, data=None, read=None,
                  read_size=0, loop=False, freq=0.0, device=0, channel_update_int=0.0, alpha=0.25, beta=0.25,
                  gamma=0.5, snr=8.0, wide=False, min_freq=0.0, max_freq=0.0, set_frequency=None, decimation=1,
-                 psd_average=0, psd_detector=0):
+                 psd_average=0, psd_detector=0, spectrum_update_int=0.0):
         """decimation: source decimation D (SPEC L); the analyzer then runs at samp_rate / D.
         psd_average: non-zero posts the mean of the frames of every psd_update_int instead of one frame (SPEC A).
         psd_detector: "pos_peak" / "neg_peak" (or PSD_DETECTOR's numbers) post the per-bin maximum / minimum of those
-        frames instead (SPEC PK); 0 or "default" leaves the choice to psd_average."""
+        frames instead (SPEC PK); 0 or "default" leaves the choice to psd_average.
+        spectrum_update_int: > 0 emits inspector spectra and baud estimates every that many seconds of channel time,
+        over 4096-point frames carried across blocks (SPEC US); 0 = once per block that fills a frame."""
         self._L = load_library()
         p = AnalyzerParams()
         p.mode = 1 if wide else 0                      # SDB_ANALYZER_MODE_{CHANNEL, WIDE_SPECTRUM}
@@ -102,6 +104,7 @@ class Analyzer:
         p.channel_update_int = channel_update_int
         p.psd_average = psd_average
         p.psd_detector = PSD_DETECTOR[psd_detector] if isinstance(psd_detector, str) else psd_detector
+        p.spectrum_update_int = spectrum_update_int
         self.params = p
         s = SourceConfig()
         s.samp_rate, s.freq, s.read_size, s.loop, s.device = samp_rate, freq, read_size, int(loop), device
@@ -276,7 +279,8 @@ class Analyzer:
                 m = C.cast(ptr, C.POINTER(AnalyzerParams)).contents
                 out = dict(mode=m.mode, window_size=m.detector_params.window_size, window=m.detector_params.window,
                            psd_update_int=m.psd_update_int, channel_update_int=m.channel_update_int,
-                           psd_average=m.psd_average, psd_detector=m.psd_detector)
+                           psd_average=m.psd_average, psd_detector=m.psd_detector,
+                           spectrum_update_int=m.spectrum_update_int)
             elif name in ("EOS", "READ_ERROR", "HALT", "SOURCE_INIT"):
                 m = C.cast(ptr, C.POINTER(StatusMsg)).contents
                 out = dict(code=m.code, err_msg=(m.err_msg or b"").decode())

@@ -19,6 +19,7 @@
 #include "sdb_internal.h"
 
 #include <algorithm>
+#include <cmath>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -69,6 +70,7 @@ struct Insp {
   uint32_t spectsrc_id;   // 0 = none (index 0 of the GUI's combo)
   uint32_t est_mask;
   uint32_t spect_size;    // frame size chosen at rebuild time (0 = too few channel samples per block)
+  bool spect_sched;       // emitting on the spectrum_update_int schedule (SPEC US) instead of once per block
 };
 
 // class names in SDB_INSP_* order, as requests and inspector messages carry them
@@ -277,8 +279,22 @@ struct sdb_analyzer {
       i.bandwidth = (float) (i.channel.f_hi - i.channel.f_lo); i.lo = (float) i.channel.fc;
       sdb_engine_set_inspector(e.get(), h, &i.cfg);
       // spectrum source / estimators: the largest frame (<= 4096) a steady-state block can fill (SPEC U.1)
-      i.spect_size = 0;
-      if (i.spectsrc_id || i.est_mask) {
+      i.spect_size = 0; i.spect_sched = false;
+      if ((i.spectsrc_id || i.est_mask) && params.spectrum_update_int > 0) {
+        // SPEC US: 4096-point frames every spectrum_update_int of channel time, whatever the block size.  An interval
+        // shorter than a block allows (more than SDB_SPECTRUM_EMITS_MAX emissions in one feed, which the engine
+        // refuses) is raised to the shortest that fits: emitting as often as possible beats stopping the session.
+        const uint32_t W = ep.st_window_size ? ep.st_window_size : ep.psd_size;
+        const uint64_t n_max = (uint64_t) (ep.max_feed / (W / 2)) * (info.size / 2);
+        const double I_min = (double) std::max<uint64_t>(1, (n_max + SDB_SPECTRUM_EMITS_MAX - 1) / SDB_SPECTRUM_EMITS_MAX);
+        const double I = std::min(std::max(I_min, std::floor((double) params.spectrum_update_int * (double) i.fs + 0.5)),
+                                  (double) SDB_SPECTRUM_INTERVAL_MAX);
+        i.spect_size = 4096; i.spect_sched = true;
+        sdb_engine_set_spectrum_source(e.get(), h, (int) i.spectsrc_id, 4096);
+        for (int k = 0; k < SDB_ESTIMATOR_COUNT; ++k)
+          if (i.est_mask & (1u << k)) sdb_engine_set_estimator(e.get(), h, k, 1);
+        sdb_engine_set_spectrum_interval(e.get(), h, (uint64_t) I);
+      } else if (i.spectsrc_id || i.est_mask) {
         const size_t n_ch = hops_per_block * (info.size / 2);
         uint32_t ns = 4096;
         while (ns >= 64 && (size_t) ns + 1 > n_ch) ns >>= 1;
@@ -770,34 +786,74 @@ struct sdb_analyzer {
     for (auto &i : insps) if (i.open && i.parent < 0) deliver_symbols(eng.get(), i, block);
   }
 
-  // kind=SPECTRUM / kind=ESTIMATOR inspector messages (one per block that filled a frame)
+  void post_spectrum(const Insp &i, const float *sp, uint32_t n)
+  {
+    sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_SPECTRUM, i.handle, i.inspector_id,
+                                                  kClassNames[i.cls]);
+    m->spectsrc_id = i.spectsrc_id; m->spectrum_size = n; m->samp_rate = (uint64_t) i.fs;
+    m->fs = (float) rate; m->equiv_fs = i.fs;
+    m->spectrum_data = (float *) malloc(n * sizeof(float));
+    memcpy(m->spectrum_data, sp, n * sizeof(float));
+    post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
+  }
+  void post_estimate(const Insp &i, int e, float v)
+  {
+    sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_ESTIMATOR, i.handle, i.inspector_id,
+                                                  kClassNames[i.cls]);
+    m->estimator_id = (uint32_t) e; m->enabled = 1; m->value = v;
+    post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
+  }
+
+  // SPEC US: every emission of the block, in t_j order: its spectrum, then its valid estimates.  The read buffers
+  // (sched_*) are kept across blocks: they grow once, and a block without emissions copies nothing.
+  std::vector<float> sched_sp, sched_vals[SDB_ESTIMATOR_COUNT];
+  std::vector<int32_t> sched_ok[SDB_ESTIMATOR_COUNT];
+  std::vector<uint64_t> sched_ends;
+  void publish_scheduled(sdb_engine_t *ie, const Insp &i)
+  {
+    const size_t cap = SDB_SPECTRUM_EMITS_MAX;
+    const uint32_t w = i.spectsrc_id == SDB_SPECTSRC_FAC ? i.spect_size / 2 : i.spect_size;
+    std::vector<float> &sp = sched_sp, *vals = sched_vals;
+    std::vector<int32_t> *ok = sched_ok;
+    std::vector<uint64_t> &ends = sched_ends;
+    if (ends.size() < cap) ends.resize(cap);
+    long n = -1;
+    if (i.spectsrc_id) {
+      if (sp.size() < cap * w) sp.resize(cap * w);
+      n = sdb_engine_read_spectra(ie, i.engine_handle, sp.data(), ends.data(), cap);
+      if (n < 0) return;
+    }
+    for (int e = 0; e < SDB_ESTIMATOR_COUNT; ++e) {
+      if (!(i.est_mask & (1u << e))) continue;
+      if (vals[e].size() < cap) { vals[e].resize(cap); ok[e].resize(cap); }
+      const long m = sdb_engine_read_estimates(ie, i.engine_handle, e, vals[e].data(), ok[e].data(), cap);
+      if (m < 0) return;
+      n = m;
+    }
+    for (long j = 0; j < n; ++j) {
+      if (i.spectsrc_id) post_spectrum(i, sp.data() + (size_t) j * w, w);
+      for (int e = 0; e < SDB_ESTIMATOR_COUNT; ++e)
+        if ((i.est_mask & (1u << e)) && ok[e][j]) post_estimate(i, e, vals[e][j]);
+    }
+  }
+
+  // kind=SPECTRUM / kind=ESTIMATOR inspector messages (one per block that filled a frame, or on the schedule)
   void publish_spectra()
   {
     for (auto &i : insps) {
       sdb_engine_t *ie = engine_of(i);
       if (!i.open || i.engine_handle < 0 || !i.spect_size || !ie) continue;
+      if (i.spect_sched) { publish_scheduled(ie, i); continue; }
       if (i.spectsrc_id) {
         std::vector<float> sp(i.spect_size);
         uint32_t emitted = 0;
-        if (sdb_engine_read_spectrum(ie, i.engine_handle, sp.data(), &emitted) == 0 && emitted) {
-          sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_SPECTRUM, i.handle, i.inspector_id,
-                                                        kClassNames[i.cls]);
-          m->spectsrc_id = i.spectsrc_id; m->spectrum_size = emitted; m->samp_rate = (uint64_t) i.fs;
-          m->fs = (float) rate; m->equiv_fs = i.fs;
-          m->spectrum_data = (float *) malloc(emitted * sizeof(float));
-          memcpy(m->spectrum_data, sp.data(), emitted * sizeof(float));
-          post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
-        }
+        if (sdb_engine_read_spectrum(ie, i.engine_handle, sp.data(), &emitted) == 0 && emitted)
+          post_spectrum(i, sp.data(), emitted);
       }
       for (int e = 0; e < SDB_ESTIMATOR_COUNT; ++e) {
         if (!(i.est_mask & (1u << e))) continue;
         float v = 0; int32_t ok = 0;
-        if (sdb_engine_read_estimate(ie, i.engine_handle, e, &v, &ok) == 0 && ok) {
-          sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_ESTIMATOR, i.handle, i.inspector_id,
-                                                        kClassNames[i.cls]);
-          m->estimator_id = (uint32_t) e; m->enabled = 1; m->value = v;
-          post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
-        }
+        if (sdb_engine_read_estimate(ie, i.engine_handle, e, &v, &ok) == 0 && ok) post_estimate(i, e, v);
       }
     }
   }
@@ -877,6 +933,10 @@ extern "C" sdb_analyzer_t *sdb_analyzer_new(const sdb_analyzer_params *params, c
   if (params->psd_detector < SDB_PSD_DETECTOR_DEFAULT || params->psd_detector > SDB_PSD_DETECTOR_NEG_PEAK) {
     fail("psd_detector must be SDB_PSD_DETECTOR_DEFAULT, _POS_PEAK or _NEG_PEAK, got " +
          std::to_string(params->psd_detector));
+    return nullptr;
+  }
+  if (!(params->spectrum_update_int >= 0.0f) || !std::isfinite(params->spectrum_update_int)) {
+    fail("spectrum_update_int must be a finite number of seconds >= 0");
     return nullptr;
   }
   const uint32_t D = src->decimation ? src->decimation : 1;
@@ -1127,6 +1187,7 @@ extern "C" int sdb_analyzer_set_params_async(sdb_analyzer_t *a, const sdb_analyz
   const uint64_t N = p->detector_params.window_size;
   if (N < 16 || (N & (N - 1))) return -1;
   if (p->psd_detector < SDB_PSD_DETECTOR_DEFAULT || p->psd_detector > SDB_PSD_DETECTOR_NEG_PEAK) return -1;
+  if (!(p->spectrum_update_int >= 0.0f) || !std::isfinite(p->spectrum_update_int)) return -1;
   Cmd c; c.kind = Cmd::SET_PARAMS; c.req_id = req_id; c.params = *p;
   return push_cmd(a, std::move(c));
 }

@@ -41,13 +41,14 @@ struct Channel {
   bool has_insp;
   sdb_inspector_config cfg;
   int spect_kind = 0; unsigned spect_size = 0, est_mask = 0;   // SPEC U
+  uint64_t spect_interval = 0;                                    // SPEC US (0: once per feed, SPEC U.1)
 };
 
 struct TimedSpan { int family; Event a, b; };
 enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_POWER, FAM_PSD_PEAK,
-       FAM_COUNT };
+       FAM_SPECTSCHED, FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
-                                            "inspector", "psd_average", "power", "psd_peak" };
+                                            "inspector", "psd_average", "power", "psd_peak", "spectsrc_sched" };
 
 // SPEC PW: samples per mean of a power inspector (power.integrate-samples, 0 read as 1)
 static uint64_t power_m(const sdb_inspector_config &c) { return c.power_integrate_samples ? c.power_integrate_samples : 1; }
@@ -66,6 +67,10 @@ struct Slot {
   float2 *chan = nullptr;
   float2 *soft = nullptr; uint8_t *hard = nullptr; uint32_t *counts = nullptr;
   DevBuf<unsigned long long> sym_off;               // packed read-out: start of every chain, 16-symbol aligned
+  // scheduled spectra (SPEC US): per emission slot [S][slot] spectrum (ns floats), size, estimates and validity, and
+  // on the host the emission count and first t_j of each scheduled channel in this feed
+  DevBuf<float> sched_spect, sched_est; DevBuf<uint32_t> sched_size; DevBuf<int> sched_valid;
+  std::vector<uint32_t> sched_n; std::vector<uint64_t> sched_first;
   Event psd_ready, psd_read, sym_read, insp;
 };
 
@@ -116,6 +121,21 @@ struct Plan {
   std::vector<SdbSpectCfg> h_spect; SdbSpectCfg *d_spectcfg = nullptr;
   float *d_spect = nullptr; size_t spect_stride = 0; int spect_max_ns = 0;
   uint32_t *d_spect_size = nullptr; float *d_est = nullptr; int *d_est_valid = nullptr;
+  // scheduled spectrum sources / estimators (SPEC US; spectsched_kernels.cu).  A scheduled channel has an empty entry
+  // in the per-feed tables above and owns `slots` consecutive emission slots: k_spectsrc runs over the slots with
+  // n_hops = 1, each slot's channel entry holding one frame (halfsz = Ns + 1, set by the gather) or none (0).
+  struct Sched {
+    int k; unsigned ns, kind, est_mask; uint64_t interval; uint32_t slot0, slots;
+    size_t out0;            // slot e's spectrum at out0 + e ns in a stream's block
+    uint64_t t = 0;         // channel samples since the channel started
+    uint64_t v = 0;         // the ring holds c[m] for every m in [max(v, t - ns - 1), t)
+  };
+  std::vector<Sched> sched; std::vector<int> sched_of;   // sched_of[k]: index into sched, or -1
+  std::vector<SdbSchedChan> h_sched; DevBuf<SdbSchedChan> d_sched;
+  DevBuf<int> d_slot_chan; DevBuf<SdbSpectCfg> d_slot_cfg; DevBuf<SdbChannelDev> d_slot_dev;
+  DevBuf<float2> d_ring, d_frames;
+  int n_slots = 0, sched_max_ns = 0;
+  size_t ring_stride = 0, frame_stride = 0, sched_spect_stride = 0;
   // DC removal (SDB_FLAG_DC_REMOVE, SPEC R): per-stream estimate, the estimate the current block is corrected with,
   // run sums, and the corrected float32 copy of the block the rest of the path reads
   float2 *d_dc_state = nullptr, *d_dc_cur = nullptr, *d_xdc = nullptr; double2 *d_dc_part = nullptr;
@@ -442,12 +462,124 @@ extern "C" int sdb_engine_set_estimator(sdb_engine_t *e, int handle, int estimat
   return 0;
 }
 
+extern "C" int sdb_engine_set_spectrum_interval(sdb_engine_t *e, int handle, uint64_t interval)
+{
+  if (!e) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (e->plan) return fail("engine already committed");
+  Channel &c = e->channels[handle];
+  if (c.spect_kind == 0 && c.est_mask == 0)
+    return fail("spectrum interval on a channel without a spectrum source or estimator");
+  if (interval > SDB_SPECTRUM_INTERVAL_MAX) return fail("spectrum interval must be at most 2^62 channel samples");
+  c.spect_interval = interval;
+  return 0;
+}
+
+static int sched_index(const Plan &p, int handle)
+{
+  return handle < (int) p.sched_of.size() ? p.sched_of[handle] : -1;
+}
+static unsigned sched_out_size(const Plan::Sched &q) { return q.kind == SDB_SPECTSRC_FAC ? q.ns / 2 : q.ns; }
+
+// Emissions [e0, e0 + n) of scheduled channel q in the latest feed, every stream: spectra into out (rows of out_size
+// floats, estimator < 0) or estimates into values / valid; stream s starts `pitch` elements after stream s - 1.
+// Fenced on the feed's inspector work like the PSD reads.
+static int read_sched(sdb_engine_t *e, const Plan::Sched &q, int estimator, uint32_t e0, uint32_t n, size_t pitch,
+                      float *out, float *values, int32_t *valid)
+{
+  Plan &p = *e->plan;
+  Slot &sl = p.cur();
+  const unsigned S = e->prm.n_streams;
+  CK(cudaSetDevice(e->prm.device));
+  CK(sl.insp.wait_on(p.d2h_stream));
+  const size_t slot = (size_t) q.slot0 + e0;
+  for (unsigned s = 0; s < S; ++s) {
+    if (estimator < 0) {
+      const unsigned w = sched_out_size(q);
+      CK(cudaMemcpy2DAsync(out + (size_t) s * pitch, (size_t) w * sizeof(float),
+                           sl.sched_spect + (size_t) s * p.sched_spect_stride + q.out0 + (size_t) e0 * q.ns,
+                           (size_t) q.ns * sizeof(float), (size_t) w * sizeof(float), n, cudaMemcpyDeviceToHost,
+                           p.d2h_stream));
+    } else {
+      const size_t off = ((size_t) s * p.n_slots + slot) * 2 + (size_t) estimator;
+      CK(cudaMemcpy2DAsync(values + (size_t) s * pitch, sizeof(float), sl.sched_est + off, 2 * sizeof(float),
+                           sizeof(float), n, cudaMemcpyDeviceToHost, p.d2h_stream));
+      CK(cudaMemcpy2DAsync(valid + (size_t) s * pitch, sizeof(int32_t), sl.sched_valid + off, 2 * sizeof(int),
+                           sizeof(int32_t), n, cudaMemcpyDeviceToHost, p.d2h_stream));
+    }
+  }
+  CK(cudaStreamSynchronize(p.d2h_stream));
+  return 0;
+}
+
+static int sched_check(sdb_engine_t *e, int handle, int estimator, const Plan::Sched **q)
+{
+  if (!e->plan) return fail("engine not committed");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  const int i = sched_index(*e->plan, handle);
+  if (i < 0) return fail("no spectrum interval on this channel");
+  *q = &e->plan->sched[i];
+  if (estimator < 0 && (*q)->kind == 0) return fail("no spectrum source on this channel");
+  if (estimator >= SDB_ESTIMATOR_COUNT) return fail("unknown estimator");
+  if (estimator >= 0 && !((*q)->est_mask & (1u << estimator))) return fail("estimator not enabled on this channel");
+  return 0;
+}
+
+// sdb_engine_read_spectrum / _read_estimate on a scheduled channel: the feed's last emission, or none
+static int read_sched_last(sdb_engine_t *e, int handle, int estimator, float *out, uint32_t *sizes, int32_t *valid)
+{
+  const Plan::Sched *q = nullptr;
+  if (sched_check(e, handle, estimator, &q)) return -1;
+  const Plan &p = *e->plan;
+  const unsigned S = e->prm.n_streams;
+  const uint32_t n = p.feed_index ? p.slot[(p.feed_index - 1) & 1u].sched_n[sched_index(p, handle)] : 0;
+  if (n == 0) {
+    for (unsigned s = 0; s < S; ++s) { if (sizes) sizes[s] = 0; if (valid) valid[s] = 0; }
+    return 0;
+  }
+  if (estimator < 0) {
+    for (unsigned s = 0; s < S; ++s) sizes[s] = sched_out_size(*q);
+    return read_sched(e, *q, -1, n - 1, 1, q->ns, out, nullptr, nullptr);   // [S][size], as on a per-feed channel
+  }
+  return read_sched(e, *q, estimator, n - 1, 1, 1, nullptr, out, valid);
+}
+
+extern "C" long sdb_engine_read_spectra(sdb_engine_t *e, int handle, float *out, uint64_t *ends, size_t cap)
+{
+  if (!e || !out || !ends) return fail("null argument");
+  const Plan::Sched *q = nullptr;
+  if (sched_check(e, handle, -1, &q)) return -1;
+  const Plan &p = *e->plan;
+  if (p.feed_index == 0) return 0;
+  const Slot &sl = p.slot[(p.feed_index - 1) & 1u];
+  const int i = sched_index(p, handle);
+  const uint32_t n = (uint32_t) std::min<size_t>(sl.sched_n[i], cap);
+  for (uint32_t j = 0; j < n; ++j) ends[j] = sl.sched_first[i] + (uint64_t) j * q->interval;
+  if (n && read_sched(e, *q, -1, 0, n, cap * sched_out_size(*q), out, nullptr, nullptr)) return -1;
+  return (long) n;
+}
+
+extern "C" long sdb_engine_read_estimates(sdb_engine_t *e, int handle, int estimator_id, float *values, int32_t *valid,
+                                          size_t cap)
+{
+  if (!e || !values || !valid) return fail("null argument");
+  if (estimator_id < 0) return fail("unknown estimator");
+  const Plan::Sched *q = nullptr;
+  if (sched_check(e, handle, estimator_id, &q)) return -1;
+  const Plan &p = *e->plan;
+  if (p.feed_index == 0) return 0;
+  const uint32_t n = (uint32_t) std::min<size_t>(p.slot[(p.feed_index - 1) & 1u].sched_n[sched_index(p, handle)], cap);
+  if (n && read_sched(e, *q, estimator_id, 0, n, cap, nullptr, values, valid)) return -1;
+  return (long) n;
+}
+
 extern "C" int sdb_engine_read_spectrum(sdb_engine_t *e, int handle, float *out, uint32_t *sizes)
 {
   if (!e || !out || !sizes) return fail("null argument");
   if (!e->plan) return fail("engine not committed");
   const Plan &p = *e->plan;
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (sched_index(p, handle) >= 0) return read_sched_last(e, handle, -1, out, sizes, nullptr);
   if (!p.d_spect || p.h_spect[handle].kind == 0) return fail("no spectrum source on this channel");
   CK(cudaSetDevice(e->prm.device));
   CK(cudaStreamSynchronize(p.insp_stream));
@@ -467,6 +599,7 @@ extern "C" int sdb_engine_read_estimate(sdb_engine_t *e, int handle, int estimat
   const Plan &p = *e->plan;
   if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
   if (estimator_id < 0 || estimator_id >= SDB_ESTIMATOR_COUNT) return fail("unknown estimator");
+  if (sched_index(p, handle) >= 0) return read_sched_last(e, handle, estimator_id, values, nullptr, valid);
   if (!p.d_est || !(p.h_spect[handle].est_mask & (1u << estimator_id))) return fail("estimator not enabled on this channel");
   CK(cudaSetDevice(e->prm.device));
   CK(cudaStreamSynchronize(p.insp_stream));
@@ -784,17 +917,24 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       CK(cudaMemcpy(g.d_ids, kv.second.data(), kv.second.size() * sizeof(int), cudaMemcpyHostToDevice));
       p.groups.push_back(g);
     }
-    // ---- inspector spectrum sources / estimators (SPEC U)
+    // ---- inspector spectrum sources / estimators, once per feed (SPEC U) or on a schedule (SPEC US)
     {
-      std::vector<SdbSpectCfg> sc(K);
+      std::vector<SdbSpectCfg> sc(K), slot_cfg;
+      std::vector<SdbChannelDev> slot_dev;
+      std::vector<int> slot_chan;
       std::map<unsigned, float *> bh_windows;   // Blackman-Harris windows by size
-      size_t off = 0; int max_ns = 0; bool any = false;
+      size_t off = 0, soff = 0, ring_off = 0, frame_off = 0; int max_ns = 0; bool any = false;
+      p.sched_of.assign(K, -1);
       for (int k = 0; k < K; ++k) {
         const Channel &c = e->channels[k];
-        SdbSpectCfg &q = sc[k];
+        SdbSpectCfg q;
         memset(&q, 0, sizeof(q));
-        if (c.spect_kind == 0 && c.est_mask == 0) continue;
-        any = true;
+        memset(&sc[k], 0, sizeof(q));          // scheduled channels keep this empty entry
+        if (c.spect_kind == 0 && c.est_mask == 0) {
+          if (c.spect_interval)
+            return fail("spectrum interval on channel " + std::to_string(k) + ", which has no spectrum source or estimator");
+          continue;
+        }
         const unsigned ns = c.spect_size ? c.spect_size : 1024u;
         q.kind = c.spect_kind; q.ns = (int) ns; q.logns = ilog2u(ns); q.est_mask = c.est_mask;
         q.fs_ch = (float) (e->samp_rate * (double) c.size / (double) W);
@@ -810,8 +950,62 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
           it = bh_windows.emplace(ns, d).first;
         }
         q.window = it->second;
-        q.out_off = off; off += ns;
-        max_ns = std::max(max_ns, (int) ns);
+        const uint64_t I = c.spect_interval;
+        if (!I) {
+          any = true;
+          q.out_off = off; off += ns;
+          max_ns = std::max(max_ns, (int) ns);
+          sc[k] = q;
+          continue;
+        }
+        // a feed emits at every multiple of I among its channel samples: at most ceil(samples / I) times
+        const uint64_t n_max = (uint64_t) max_hops * c.halfsz, slots = (n_max + I - 1) / I;
+        if (slots > SDB_SPECTRUM_EMITS_MAX)
+          return fail("spectrum interval " + std::to_string(I) + " on channel " + std::to_string(k) + " allows " +
+                      std::to_string(slots) + " emissions per feed of max_feed samples; at most " +
+                      std::to_string(SDB_SPECTRUM_EMITS_MAX));
+        Plan::Sched sd;
+        sd.k = k; sd.ns = ns; sd.kind = (unsigned) c.spect_kind; sd.est_mask = c.est_mask; sd.interval = I;
+        sd.slot0 = (uint32_t) slot_cfg.size(); sd.slots = (uint32_t) slots; sd.out0 = soff;
+        SdbSchedChan h;
+        memset(&h, 0, sizeof(h));
+        h.in_off = p.h_chans[k].out_off; h.ring_off = ring_off; h.frame_off = frame_off;
+        h.ns1 = ns + 1; h.slot0 = sd.slot0; h.interval = I;
+        for (uint64_t j = 0; j < slots; ++j) {
+          SdbSpectCfg qe = q;
+          qe.out_off = soff + j * ns;
+          slot_cfg.push_back(qe);
+          SdbChannelDev d;
+          memset(&d, 0, sizeof(d));
+          d.out_off = frame_off + j * (ns + 1);   // halfsz: set per feed by the gather
+          slot_dev.push_back(d);
+          slot_chan.push_back((int) p.sched.size());
+        }
+        soff += slots * ns; ring_off += ns + 1; frame_off += slots * (ns + 1);
+        p.sched_max_ns = std::max(p.sched_max_ns, (int) ns);
+        p.sched_of[k] = (int) p.sched.size();
+        p.sched.push_back(sd); p.h_sched.push_back(h);
+      }
+      if (!p.sched.empty()) {
+        const size_t ns_ = p.sched.size();
+        p.n_slots = (int) slot_cfg.size();
+        p.ring_stride = ring_off; p.frame_stride = frame_off; p.sched_spect_stride = soff;
+        if (p.d_sched.alloc(ns_) || p.d_slot_chan.alloc(p.n_slots) || p.d_slot_cfg.alloc(p.n_slots) ||
+            p.d_slot_dev.alloc(p.n_slots) || p.d_ring.alloc((size_t) S * ring_off) ||
+            p.d_frames.alloc((size_t) S * frame_off))
+          return fail("out of device memory (scheduled spectra)");
+        for (Slot &sl : p.slot) {
+          if (sl.sched_spect.alloc((size_t) S * soff) || sl.sched_size.alloc((size_t) S * p.n_slots) ||
+              sl.sched_est.alloc((size_t) S * p.n_slots * 2) || sl.sched_valid.alloc((size_t) S * p.n_slots * 2))
+            return fail("out of device memory (scheduled spectra)");
+          CK(cudaMemset(sl.sched_size, 0, (size_t) S * p.n_slots * sizeof(uint32_t)));
+          CK(cudaMemset(sl.sched_valid, 0, (size_t) S * p.n_slots * 2 * sizeof(int)));
+          sl.sched_n.assign(ns_, 0); sl.sched_first.assign(ns_, 0);
+        }
+        CK(cudaMemcpy(p.d_slot_chan, slot_chan.data(), slot_chan.size() * sizeof(int), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(p.d_slot_cfg, slot_cfg.data(), slot_cfg.size() * sizeof(SdbSpectCfg), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(p.d_slot_dev, slot_dev.data(), slot_dev.size() * sizeof(SdbChannelDev), cudaMemcpyHostToDevice));
+        CK(cudaMemset(p.d_ring, 0, (size_t) S * ring_off * sizeof(float2)));
       }
       if (any) {
         p.spect_stride = off; p.spect_max_ns = max_ns; p.h_spect = sc;
@@ -908,6 +1102,49 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
   CK(p.ev_h2d.create());
   if (big && big->path == SDB_FFT_F5) pin_scratch(e, p, *big);
   e->plan = std::move(plan);
+  return 0;
+}
+
+// SPEC US for one feed of `hops` channeliser hops.  On the host: every scheduled channel's emission points in
+// (t, t + samples] whose frame lies in the history (t_j - Ns - 1 >= v; for a channel that started, t_j >= Ns + 1) and
+// the feed samples a later frame can still need, [max(t, t_next - Ns - 1), t + samples).  On the inspector stream,
+// after the feed's channel samples: the frame gather, k_spectsrc over the emitted frames, the ring update.
+static int sched_feed(sdb_engine *e, Plan &p, Slot &sl, const SdbLaunchCtx &ictx, uint64_t hops)
+{
+  const int S = (int) e->prm.n_streams;
+  uint32_t total = 0;
+  bool writes = false;
+  for (size_t i = 0; i < p.sched.size(); ++i) {
+    Plan::Sched &q = p.sched[i];
+    SdbSchedChan &h = p.h_sched[i];
+    const uint64_t I = q.interval, ns1 = q.ns + 1, T0 = q.t, n = hops * (uint64_t) p.h_chans[q.k].halfsz, T1 = T0 + n;
+    uint64_t first = (T0 / I + 1) * I;
+    if (first < q.v + ns1) first += (q.v + ns1 - first + I - 1) / I * I;
+    const uint32_t cnt = first <= T1 ? (uint32_t) ((T1 - first) / I + 1) : 0;
+    const uint64_t next = (T1 / I + 1) * I;
+    const uint64_t a = std::min(T1, std::max(T0, next > ns1 ? next - ns1 : 0));
+    h.t0 = T0; h.t_first = first; h.n_emit = cnt;
+    h.w_from = (uint32_t) (a - T0); h.w_to = (uint32_t) n;
+    if (a > T0) q.v = a;                   // the ring holds [a, T1) only
+    q.t = T1;
+    sl.sched_n[i] = cnt; sl.sched_first[i] = first;
+    total += cnt;
+    writes = writes || a < T1;
+  }
+  if (!total && !writes) return 0;
+  e->span_begin(FAM_SPECTSCHED, ictx.stream);
+  CK(cudaMemcpyAsync(p.d_sched, p.h_sched.data(), p.h_sched.size() * sizeof(SdbSchedChan), cudaMemcpyHostToDevice,
+                     ictx.stream));
+  if (total) {
+    CK(sdb_launch_spectsched_gather(ictx, p.d_sched, p.d_slot_chan, p.d_slot_dev, p.n_slots, S, sl.chan, p.chan_stride,
+                                    p.d_ring, p.ring_stride, p.d_frames, p.frame_stride));
+    CK(sdb_launch_spectsrc(ictx, p.d_slot_cfg, p.d_slot_dev, p.n_slots, S, p.sched_max_ns, p.d_frames, p.frame_stride,
+                           1u, sl.sched_spect, p.sched_spect_stride, sl.sched_size, sl.sched_est, sl.sched_valid));
+  }
+  if (writes)
+    CK(sdb_launch_spectsched_ring(ictx, p.d_sched, (int) p.sched.size(), S, sl.chan, p.chan_stride, p.d_ring,
+                                  p.ring_stride));
+  e->span_end(ictx.stream);
   return 0;
 }
 
@@ -1087,6 +1324,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
         CK(sdb_launch_spectsrc(ictx, p.d_spectcfg, p.d_chans, K, (int) S, p.spect_max_ns, sl.chan,
                                p.chan_stride, (uint32_t) wps, p.d_spect, p.spect_stride, p.d_spect_size,
                                p.d_est, p.d_est_valid));
+      if (!p.sched.empty() && sched_feed(e, p, sl, ictx, (uint64_t) wps)) return -1;
       if (p.insp_ctas > 0) {                      // (every channel a power inspector: no chain)
         e->span_begin(FAM_INSPECTOR, ictx.stream);
         CK(sdb_launch_inspectors_n(ictx, p.d_cfg, K, (int) S, p.d_chain_map, p.insp_ctas, p.d_state, p.d_pool,
@@ -1103,6 +1341,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
       }
       CK(sl.insp.record(ictx.stream));
     } else {
+      std::fill(sl.sched_n.begin(), sl.sched_n.end(), 0u);   // no channel samples: no emission
       CK(sl.sym_read.wait_on(p.insp_stream));
       CK(cudaMemsetAsync(sl.counts, 0, (size_t) S * K * sizeof(uint32_t), p.insp_stream));
       CK(sl.insp.record(p.insp_stream));
@@ -1448,6 +1687,15 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
                       from.tail_stride * sizeof(float2), (size_t) cn.halfsz * sizeof(float2), S, cudaMemcpyDeviceToDevice));
       CK(cudaMemcpy2D(to.d_lo_phase + kn, (size_t) Kn * sizeof(float), from.d_lo_phase + ko, (size_t) Ko * sizeof(float),
                       sizeof(float), S, cudaMemcpyDeviceToDevice));
+      // SPEC US: the channel's sample count and ring go on while both schedule it with the same Ns, whatever its
+      // kind, estimators or interval
+      const int qn = sched_index(to, kn), qo = sched_index(from, ko);
+      if (qn >= 0 && qo >= 0 && to.sched[qn].ns == from.sched[qo].ns) {
+        const SdbSchedChan &hn = to.h_sched[qn], &ho = from.h_sched[qo];
+        CK(cudaMemcpy2D(to.d_ring.get() + hn.ring_off, to.ring_stride * sizeof(float2), from.d_ring.get() + ho.ring_off,
+                        from.ring_stride * sizeof(float2), (size_t) hn.ns1 * sizeof(float2), S, cudaMemcpyDeviceToDevice));
+        to.sched[qn].t = from.sched[qo].t; to.sched[qn].v = from.sched[qo].v;
+      }
     }
     if (!cn.has_insp || !co.has_insp) continue;
     if (is_power(cn) || is_power(co)) {

@@ -431,6 +431,26 @@ cudaError_t sdb_launch_spectsrc(const SdbLaunchCtx &c, const SdbSpectCfg *cfg_de
                                 int n_channels, int n_streams, int max_ns, const float2 *chan_in,
                                 size_t chan_stream_stride, uint32_t n_hops, float *spect, size_t spect_stream_stride,
                                 uint32_t *spect_size, float *est, int *est_valid);
+// spectsched_kernels.cu: scheduled spectrum sources / estimators (SPEC US).  One entry per scheduled channel: where
+// its samples, ring and frames live (offsets inside one stream's block) and this feed's schedule.
+struct SdbSchedChan {
+  size_t   in_off;          // the channel's offset in a stream's channel block
+  size_t   ring_off;        // its ring (Ns + 1 entries) in a stream's ring block
+  size_t   frame_off;       // its first emission slot's frame (Ns + 1 samples) in a stream's frame block
+  uint32_t ns1;             // Ns + 1
+  uint32_t slot0;           // index of its first emission slot
+  unsigned long long t0;        // channel samples before this feed (T_before)
+  unsigned long long t_first;   // the feed's first emission point
+  unsigned long long interval;  // I
+  uint32_t n_emit;          // emissions of this feed
+  uint32_t w_from, w_to;    // feed samples [w_from, w_to) go to the ring
+};
+cudaError_t sdb_launch_spectsched_gather(const SdbLaunchCtx &c, const SdbSchedChan *sched, const int *slot_chan,
+                                         SdbChannelDev *slot_dev, int n_slots, int n_streams, const float2 *chan_in,
+                                         size_t chan_stride, const float2 *ring, size_t ring_stride, float2 *frames,
+                                         size_t frame_stride);
+cudaError_t sdb_launch_spectsched_ring(const SdbLaunchCtx &c, const SdbSchedChan *sched, int n_sched, int n_streams,
+                                       const float2 *chan_in, size_t chan_stride, float2 *ring, size_t ring_stride);
 // sview_kernels.cu: frame-averaged main PSD (SPEC A); psd [S][frames][n] -> out [S][means][n], carry [S][n]
 cudaError_t sdb_launch_psd_group_mean(const SdbLaunchCtx &c, const float *psd, unsigned frames, unsigned n,
                                       size_t n_streams, unsigned A, unsigned carried, unsigned means, int shift_db,

@@ -610,6 +610,8 @@ sdb_analyzer_params to_sdb_params(const struct suscan_analyzer_params *p)
   q.detector_params.gamma = p->detector_params.gamma; q.detector_params.snr = p->detector_params.snr;
   q.channel_update_int = p->channel_update_int; q.psd_update_int = p->psd_update_int;
   q.min_freq = p->min_freq; q.max_freq = p->max_freq;
+  // the inspector spectrum's 100 ms update period (Default/GenericInspector/InspectorUI.cpp:971-975)
+  q.spectrum_update_int = 0.1f;
   return q;
 }
 
