@@ -68,8 +68,16 @@ struct Fft65536K {
 
 static __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 static __device__ __forceinline__ void cluster_wait()   { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+// store v at shared-memory address `addr` of the cluster's CTA `rank`: 32-bit shared::cluster addresses, where
+// map_shared_rank's generic pointers take two registers each
+static __device__ __forceinline__ void st_cluster(unsigned addr, unsigned rank, float2 v)
+{
+  unsigned ra;
+  asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(addr), "r"(rank));
+  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" :: "r"(ra), "f"(v.x), "f"(v.y) : "memory");
+}
 
-__global__ void __cluster_dims__(16, 1, 1) __launch_bounds__(256, 3) k_fft65536(const Fft65536K p)
+__global__ void __cluster_dims__(16, 1, 1) __launch_bounds__(256, 4) k_fft65536(const Fft65536K p)
 {
   // one buffer, three uses: pass A's exchange, the 16 rows the cluster sends this CTA, pass B's exchange
   __shared__ float2 sm[16 * LDC];
@@ -102,33 +110,29 @@ __global__ void __cluster_dims__(16, 1, 1) __launch_bounds__(256, 3) k_fft65536(
   const char *__restrict__ xs = reinterpret_cast<const char *>(a.x) + (size_t) stream * a.stream_stride * sdb_fmt_bytes(fmt);
   const float2 *__restrict__ hs = psd ? nullptr : a.hist + (size_t) stream * hist_len;
 
-  const float *__restrict__ wp = psd && a.window ? a.window + t * 256 + col : nullptr;
+  const int o = t * 256 + col;                      // row n1 = t + 16 j sits at o + 4096 j
+  const float *__restrict__ wp = psd && a.window ? a.window + o : nullptr;
   float2 v[16];
-  if (fmt == SDB_FMT_F32) {
-    const float2 *__restrict__ xf = reinterpret_cast<const float2 *>(xs);
-    if (v0 >= hist_len) {                           // CTA-uniform: the window lies wholly in the new samples
-      const float2 *__restrict__ src = xf + (v0 - hist_len) + t * 256 + col;
+  // Two halves of 8 rows.  Window starts and the history length are multiples of 32768, so half h (samples
+  // [32768 h, 32768 h + 32768) of the window) lies wholly in the history or wholly in the new samples: one CTA-uniform
+  // source per half, and every load an immediate offset from it.
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        v[j] = __ldg(src + j * 4096);    // row n1 = t + 16 j
-        if (wp) { const float wv = __ldg(wp + j * 4096); v[j] = sdb_mul2(v[j], make_float2(wv, wv)); }
-      }
-    } else {
+  for (int h = 0; h < 2; ++h) {
+    const long s0 = v0 + 32768 * h - hist_len;      // the half's first sample, relative to the new samples
+    if (s0 < 0 || fmt == SDB_FMT_F32) {
+      const float2 *__restrict__ src = (s0 < 0 ? hs + (s0 + hist_len) : reinterpret_cast<const float2 *>(xs) + s0) + o;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int r = t + 16 * j;
-        const long vi = v0 + (long) r * 256 + col;
-        v[j] = vi < hist_len ? __ldg(hs + vi) : __ldg(xf + (vi - hist_len));
-        if (wp) { const float wv = __ldg(wp + j * 4096); v[j] = sdb_mul2(v[j], make_float2(wv, wv)); }
-      }
+      for (int u = 0; u < 8; ++u) v[8 * h + u] = __ldg(src + u * 4096);
+    } else {                                        // 8 / 16-bit SDR samples: converted in the load
+#pragma unroll
+      for (int u = 0; u < 8; ++u) v[8 * h + u] = sdb_ld_iq(xs, s0 + o + u * 4096, fmt);
     }
-  } else {                                          // 8 / 16-bit SDR samples: converted in the load
+    if (wp) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int r = t + 16 * j;
-      const long vi = v0 + (long) r * 256 + col;
-      v[j] = vi < hist_len ? __ldg(hs + vi) : sdb_ld_iq(xs, vi - hist_len, fmt);
-      if (wp) { const float wv = __ldg(wp + j * 4096); v[j] = sdb_mul2(v[j], make_float2(wv, wv)); }
+      for (int u = 0; u < 8; ++u) {
+        const float wv = __ldg(wp + (8 * h + u) * 4096);
+        v[8 * h + u] = sdb_mul2(v[8 * h + u], make_float2(wv, wv));
+      }
     }
   }
   fft16(v);                                         // over j: Y[t][ka], ka = REV16(position)
@@ -147,17 +151,15 @@ __global__ void __cluster_dims__(16, 1, 1) __launch_bounds__(256, 3) k_fft65536(
     for (int tt = 0; tt < 16; ++tt) v[tt] = sm[c * LDC + ka * 17 + tt];
     cluster_arrive();                               // this CTA's exchange buffer is free for the rows it receives
     fft16(v);                                       // over t: X[ka + 16 kb], kb = REV16(position)
+    const float2 *__restrict__ tq = p.twpq + ka * 256 + col;
 #pragma unroll
-    for (int q = 0; q < 16; ++q) {
-      const int k1 = ka + 16 * REV16(q);
-      v[q] = cmulf(v[q], __ldg(p.twpq + k1 * 256 + col));      // SPEC F.4 inter-pass twiddle
-    }
+    for (int q = 0; q < 16; ++q)                    // SPEC F.4 inter-pass twiddle of row k1 = ka + 16 kb
+      v[q] = cmulf(v[q], __ldg(tq + 4096 * REV16(q)));
     cluster_wait();                                 // every CTA of the window has read its exchange buffer
+    const unsigned dst = (unsigned) __cvta_generic_to_shared(sm + ka * LDX + col);
 #pragma unroll
-    for (int q = 0; q < 16; ++q) {                  // row k1 = ka + 16 kb to CTA kb, its row ka
-      float2 *dst = cluster.map_shared_rank(sm, REV16(q));
-      dst[ka * LDX + col] = v[q];
-    }
+    for (int q = 0; q < 16; ++q)                    // row k1 = ka + 16 kb to CTA kb, its row ka
+      st_cluster(dst, REV16(q), v[q]);
   }
   cluster_arrive();
   cluster_wait();                                   // all 16 rows of this CTA have arrived

@@ -604,13 +604,16 @@ static __device__ __forceinline__ void group_sync(int bar_id, int per)
   else asm volatile("barrier.sync %0, %1;" :: "r"(bar_id), "r"(per) : "memory");
 }
 
-// s: padded buffer of M points; jb = 0 .. M/16-1 (the `per` = M/16 threads of one group); M >= 16
+// s: padded buffer of M points; jb = 0 .. M/16-1 (the `per` = M/16 threads of one group); M >= 256, so that e and q are
+// multiples of 16.  Every address is PADI(a) + PADI(b) with b a multiple of 16, which equals PADI(a + b): one
+// per-thread base and offsets that are immediates when M is a constant.
 template <int DIR>
 static __device__ __forceinline__ void group_fft16(float2 *s, const int M, const int logM, const int jb,
                                                    const int per, const int bar_id,
                                                    const float2 *__restrict__ tw)
 {
   const int q = M >> 2, e = M >> 4;
+  const int pj = PADI(jb);
   float2 v[4][4];                                      // v[u][t] = s[jb + u e + t q]
   int logNs = 0;
   for (; logNs + 4 <= logM; logNs += 4) {
@@ -618,7 +621,7 @@ static __device__ __forceinline__ void group_fft16(float2 *s, const int M, const
 #pragma unroll
     for (int u = 0; u < 4; ++u)
 #pragma unroll
-      for (int t = 0; t < 4; ++t) v[u][t] = s[PADI(jb + u * e + t * q)];
+      for (int t = 0; t < 4; ++t) v[u][t] = s[pj + PADI(u * e + t * q)];
     group_sync(bar_id, per);
     // level Ns: butterflies j = jb + u e, all with the same k (e is a multiple of Ns)
     if (logNs > 0) {
@@ -643,11 +646,12 @@ static __device__ __forceinline__ void group_fft16(float2 *s, const int M, const
         r4_core<DIR>(v[0][t], v[1][t], v[2][t], v[3][t]);
       }
     }
-    const int base = ((jb - k) << 4) + k;
+    // Ns = 16^i: base + m Ns (m < 16) crosses a 16-point boundary only by whole multiples of 16 points
+    const int base = PADI(((jb - k) << 4) + k);
 #pragma unroll
     for (int u = 0; u < 4; ++u)
 #pragma unroll
-      for (int t = 0; t < 4; ++t) s[PADI(base + (t + 4 * u) * Ns)] = v[u][t];
+      for (int t = 0; t < 4; ++t) s[base + (t + 4 * u) * Ns + (((t + 4 * u) * Ns) >> 4)] = v[u][t];
     group_sync(bar_id, per);
   }
   if (logNs + 2 <= logM) {                             // one level left over: four independent butterflies
@@ -655,7 +659,7 @@ static __device__ __forceinline__ void group_fft16(float2 *s, const int M, const
 #pragma unroll
     for (int u = 0; u < 4; ++u)
 #pragma unroll
-      for (int t = 0; t < 4; ++t) v[u][t] = s[PADI(jb + u * e + t * q)];
+      for (int t = 0; t < 4; ++t) v[u][t] = s[pj + PADI(u * e + t * q)];
     group_sync(bar_id, per);
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
@@ -678,17 +682,20 @@ static __device__ __forceinline__ void group_fft16(float2 *s, const int M, const
     for (int b = 0; b < 8; ++b) {
       const int j = jb + b * e;
       const float2 w = twd<DIR>(tw, j);
-      const float2 a = s[PADI(j)], t = cmulf(s[PADI(j + h)], w);
-      s[PADI(j)]     = cadd(a, t);
-      s[PADI(j + h)] = csub(a, t);
+      const float2 a = s[pj + PADI(b * e)], t = cmulf(s[pj + PADI(b * e + h)], w);
+      s[pj + PADI(b * e)]     = cadd(a, t);
+      s[pj + PADI(b * e + h)] = csub(a, t);
     }
     group_sync(bar_id, per);
   }
 }
 
 #define IFFT16_THREADS 256
-// 3 CTAs per SM (42 KB of shared memory at 1024 points): 80 registers, no spills
-__global__ void __launch_bounds__(IFFT16_THREADS, 3)
+// One instance per channel size, so that the transform's shared-memory offsets are immediates.  4 CTAs per SM up to
+// 2048 points (64 registers, no spills; 42 KB of shared memory at 1024 points); 4096-point hops take 66 KB, so
+// shared memory holds that size to 3 CTAs per SM and its instance keeps 80 registers.
+template <int SIZE>
+__global__ void __launch_bounds__(IFFT16_THREADS, SIZE < 4096 ? 4 : 3)
 k_chan_ifft16(const SdbChannelDev *__restrict__ chans, const int *__restrict__ group, int n_channels,
               const float2 *__restrict__ cspec, int n_bins, int wps, int any_precise,
               float2 *__restrict__ tails, size_t tail_stream_stride, float *__restrict__ lo_phase,
@@ -696,20 +703,21 @@ k_chan_ifft16(const SdbChannelDev *__restrict__ chans, const int *__restrict__ g
 {
   extern __shared__ float2 sm[];
   const int ci = group[blockIdx.x];
-  const SdbChannelDev ch = chans[ci];
+  const SdbChannelDev &ch = chans[ci];
   const int s = blockIdx.y;
-  const int size = ch.size, hs = ch.halfsz, hw = ch.halfw;
-  const int per = size >> 4, P = IFFT16_THREADS / per;  // threads per hop, hops per round
-  const int padsz = size + (size >> 4);
+  constexpr int size = SIZE, hs = SIZE / 2, log2size = SIZE == 512 ? 9 : SIZE == 1024 ? 10 : SIZE == 2048 ? 11 : 12;
+  const int hw = ch.halfw;
+  constexpr int per = size >> 4, P = IFFT16_THREADS / per;  // threads per hop, hops per round
+  constexpr int padsz = size + (size >> 4);
   float2 *bufs = sm;                                    // [P][padsz]
-  float2 *prevb[2] = { sm + (size_t) P * padsz, sm + (size_t) P * padsz + hs };
+  float2 *prevb = sm + (size_t) P * padsz;             // [2][hs]: the carried half, alternating between rounds
   float *phase = reinterpret_cast<float *>(sm + (size_t) P * padsz + 2 * hs);   // [P][hs], precise channels only
   const int tid = threadIdx.x;
   const int g = tid / per, l = tid - g * per;
   float2 *__restrict__ tail = tails + (size_t) s * tail_stream_stride + ch.tail_off;
   float2 *__restrict__ out = chan_out + (size_t) s * chan_stream_stride + ch.out_off;
 
-  for (int i = tid; i < hs; i += IFFT16_THREADS) prevb[0][i] = tail[i];
+  for (int i = tid; i < hs; i += IFFT16_THREADS) prevb[i] = tail[i];
   float lo_phi = (any_precise && ch.precise) ? lo_phase[(size_t) s * n_channels + ci] : 0.0f;
   int pb = 0;
   __syncthreads();
@@ -755,14 +763,14 @@ k_chan_ifft16(const SdbChannelDev *__restrict__ chans, const int *__restrict__ g
     }
     if (active) {
       group_sync(1 + g, per);
-      group_fft16<+1>(buf, size, ch.log2size, l, per, 1 + g, ch.tw);
+      group_fft16<+1>(buf, size, log2size, l, per, 1 + g, ch.tw);
     }
     __syncthreads();
     if (active) {
       const float2 *pvb = g > 0 ? buf - padsz : nullptr;
       for (int i = l; i < hs; i += per) {
         const float al = __ldg(ch.xfade + i), be = __ldg(ch.xfade + i + hs);
-        const float2 cu = buf[PADI(i)], pv = g > 0 ? pvb[PADI(i + hs)] : prevb[pb][i];
+        const float2 cu = buf[PADI(i)], pv = g > 0 ? pvb[PADI(i + hs)] : prevb[pb * hs + i];
         float2 o = make_float2(al * cu.x + be * pv.x, al * cu.y + be * pv.y);
         if (any_precise && ch.precise) {
           float sn, cs_;
@@ -770,13 +778,13 @@ k_chan_ifft16(const SdbChannelDev *__restrict__ chans, const int *__restrict__ g
           o = cmulc(o, make_float2(cs_, sn));
         }
         out[(size_t) (j0 + g) * hs + i] = o;
-        if (g == Pg - 1) prevb[pb ^ 1][i] = buf[PADI(i + hs)];
+        if (g == Pg - 1) prevb[(pb ^ 1) * hs + i] = buf[PADI(i + hs)];
       }
     }
     pb ^= 1;
     __syncthreads();
   }
-  for (int i = tid; i < hs; i += IFFT16_THREADS) tail[i] = prevb[pb][i];
+  for (int i = tid; i < hs; i += IFFT16_THREADS) tail[i] = prevb[pb * hs + i];
   if (any_precise && ch.precise && tid == IFFT16_THREADS - 1) lo_phase[(size_t) s * n_channels + ci] = lo_phi;
 }
 
@@ -790,15 +798,24 @@ cudaError_t sdb_launch_chan_ifft_group(const SdbLaunchCtx &c, const SdbChannelDe
   static std::atomic<unsigned long long> attr_done{ 0 };   // one bit per device: function attributes are per context
   if (size >= 512 && size <= 4096) {
     static std::atomic<unsigned long long> attr16_done{ 0 };
-    if (sdb_first_on_device(attr16_done))
-      cudaFuncSetAttribute(k_chan_ifft16, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    if (sdb_first_on_device(attr16_done)) {
+      cudaFuncSetAttribute(k_chan_ifft16<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+      cudaFuncSetAttribute(k_chan_ifft16<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+      cudaFuncSetAttribute(k_chan_ifft16<2048>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+      cudaFuncSetAttribute(k_chan_ifft16<4096>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    }
     const int per = size / 16, P = IFFT16_THREADS / per;
     const size_t smem = (size_t) P * (size + size / 16) * sizeof(float2) + (size_t) size * sizeof(float2)
                         + (any_precise ? (size_t) P * (size / 2) * sizeof(float) : 0);
     dim3 grid(group_len, n_streams);
-    k_chan_ifft16<<<grid, IFFT16_THREADS, smem, c.stream>>>(chans_dev, group_dev, n_channels, cspec, n_bins, wps,
-                                                            any_precise, tails, tail_stream_stride, lo_phase,
-                                                            chan_out, chan_stream_stride);
+#define IFFT16_CASE(N_) case N_: k_chan_ifft16<N_><<<grid, IFFT16_THREADS, smem, c.stream>>>(                    \
+        chans_dev, group_dev, n_channels, cspec, n_bins, wps, any_precise, tails, tail_stream_stride, lo_phase,   \
+        chan_out, chan_stream_stride); break
+    switch (size) {
+      IFFT16_CASE(512); IFFT16_CASE(1024); IFFT16_CASE(2048); IFFT16_CASE(4096);
+      default: return cudaErrorInvalidValue;
+    }
+#undef IFFT16_CASE
     if (c.launch_counter) ++*c.launch_counter;
     return cudaGetLastError();
   }
