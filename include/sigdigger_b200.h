@@ -145,9 +145,9 @@ int sdb_inspector_config_default(sdb_inspector_config *cfg, int insp_class, floa
 /* freezes the channel plan and allocates device buffers; required before the first feed */
 int sdb_engine_commit(sdb_engine_t *e);
 /* Live re-plan: `dst` (committed, not yet fed) takes over the running state of `src` (same streams / window /
- * device): input history, the partial group of the frame-averaged PSD when psd_size, psd_window and psd_average match
- * (otherwise `dst` starts an empty group), the partial group of the peak detectors when psd_size, psd_window and
- * psd_peak match (likewise), and per channel with identical parameters the cross-fade tail, the LO phase
+ * device): input history, the partial group of the frame-averaged PSD and of the peak detectors, each when psd_size,
+ * psd_window and its group size (psd_average, psd_peak) match (otherwise `dst` starts an empty group), and per channel
+ * with identical parameters the cross-fade tail, the LO phase
  * and -- if the inspector class and the sizes of its state lines are unchanged -- the loop state of every chain; a power
  * inspector that stays one with the same power_integrate_samples keeps its partial group (SPEC PW).  This is how an
  * analyzer opens, closes, retunes or reconfigures ONE inspector at a block boundary while the others keep running

@@ -151,14 +151,14 @@ struct sdb_analyzer {
   // geometry set by rebuild).
   std::mutex insp_m;
   double psd_credit = 0;
-  // frame-averaged PSD (params.psd_average, SPEC A): the A, window size and window function of the baseband engine,
-  // whether A was clamped, and the frames of the engine's current partial group (its carry survives a re-plan exactly
-  // when A, N and the window stay, see sdb_engine_migrate)
-  uint32_t avg_A = 0, avg_N = 0; int32_t avg_window = 0; bool avg_clamped = false;
-  uint64_t avg_frames = 0;
-  // peak detectors (params.psd_detector, SPEC PK), kept the same way; pk_neg: post the minima instead of the maxima
-  uint32_t pk_P = 0, pk_N = 0; int32_t pk_window = 0; bool pk_clamped = false, pk_neg = false;
-  uint64_t pk_frames = 0;
+  // the baseband engine's frame-group stage, SPEC A's means or SPEC PK's extremes: G frames per group (< 2: off), N,
+  // the window function, whether G was clamped, whether the minima are posted, and the frames of the engine's open group
+  // (its carry survives a re-plan exactly when the kind, G, N and the window stay, see sdb_engine_migrate)
+  struct PsdGroups {
+    enum Kind { NONE, MEAN, PEAK } kind = NONE;
+    uint32_t G = 0, N = 0; int32_t window = 0; bool clamped = false, neg = false;
+    uint64_t frames = 0;
+  } psd_groups;
   // source-side options of the worker loop (Suscan/Analyzer.cpp:117-135, 229-244; SourceWidget.cpp:1156-1184)
   bool iq_reverse = false, dc_remove = false;
   double throttle = 0;                                  // samples / s, 0 = as fast as the source delivers
@@ -346,19 +346,17 @@ struct sdb_analyzer {
       *clamped = (long long) f != r;
       return f;
     };
-    // a peak detector takes precedence over averaging (SPEC PK.5)
+    // a peak detector takes precedence over averaging (SPEC PK.5); G = 1: every frame is a group of its own
     const bool peaks = params.psd_detector != SDB_PSD_DETECTOR_DEFAULT;
-    // frames per averaged PSD (1 = every frame, averaging off) and per peak group (1 = every frame, its own extreme)
-    avg_clamped = pk_clamped = false;
-    const uint32_t A = params.psd_average && !peaks ? interval_frames(SDB_PSD_AVERAGE_MAX, &avg_clamped) : 0;
-    const uint32_t P = peaks ? interval_frames(SDB_PSD_PEAK_MAX, &pk_clamped) : 0;
-    ep.psd_average = A;
-    ep.psd_peak = P;
-    pk_neg = params.psd_detector == SDB_PSD_DETECTOR_NEG_PEAK;
-    if (!old || P != pk_P || ep.psd_size != pk_N || ep.psd_window != pk_window) pk_frames = 0;
-    pk_P = P; pk_N = ep.psd_size; pk_window = ep.psd_window;
-    if (!old || A != avg_A || ep.psd_size != avg_N || ep.psd_window != avg_window) avg_frames = 0;
-    avg_A = A; avg_N = ep.psd_size; avg_window = ep.psd_window;
+    PsdGroups g;
+    g.kind = peaks ? PsdGroups::PEAK : params.psd_average ? PsdGroups::MEAN : PsdGroups::NONE;
+    if (g.kind != PsdGroups::NONE) g.G = interval_frames(peaks ? SDB_PSD_PEAK_MAX : SDB_PSD_AVERAGE_MAX, &g.clamped);
+    g.N = ep.psd_size; g.window = ep.psd_window;
+    g.neg = params.psd_detector == SDB_PSD_DETECTOR_NEG_PEAK;
+    (peaks ? ep.psd_peak : ep.psd_average) = g.G;
+    const PsdGroups &o = psd_groups;
+    if (old && g.kind == o.kind && g.G == o.G && g.N == o.N && g.window == o.window) g.frames = o.frames;
+    psd_groups = g;
     eng = plan_level(ep, rate, -1, old_handle, old.get());
     if (!eng) return false;
     // sub-carrier engines: one per inspector that has open children, parents before children (an inspector's handle
@@ -718,29 +716,28 @@ struct sdb_analyzer {
   {
     const size_t N = (size_t) params.detector_params.window_size, frames = block / N;
     // the extremes (SPEC PK) or the means (SPEC A) of the groups the block completed, G frames each
-    const bool peaks = pk_P >= 2;
-    if (peaks || avg_A >= 2) {
-      const uint32_t G = peaks ? pk_P : avg_A;
-      uint64_t &open = peaks ? pk_frames : avg_frames;
+    PsdGroups &pg = psd_groups;
+    if (pg.G >= 2) {
+      const bool peaks = pg.kind == PsdGroups::PEAK;
       const size_t groups = peaks ? sdb_engine_psd_peak_groups(eng.get()) : sdb_engine_psd_average_frames(eng.get());
       // group j of the block starts j G - carried frames after the block's first (earlier blocks hold its start when
       // that is negative).  Unless G was clamped a group lasts exactly the interval the credit is measured against, so
       // every group is posted.
-      const uint64_t carried = open;
-      open = (open + frames) % G;
+      const uint64_t carried = pg.frames;
+      pg.frames = (pg.frames + frames) % pg.G;
       psd.resize(groups * N);
-      if (groups && (peaks ? sdb_engine_read_psd_peak(eng.get(), pk_neg ? nullptr : psd.data(),
-                                                      pk_neg ? psd.data() : nullptr, psd.size())
+      if (groups && (peaks ? sdb_engine_read_psd_peak(eng.get(), pg.neg ? nullptr : psd.data(),
+                                                      pg.neg ? psd.data() : nullptr, psd.size())
                            : sdb_engine_read_psd_average(eng.get(), psd.data(), psd.size())))
         return;
-      const double per_group = (double) G * (double) N / rate;
-      const double interval = (peaks ? pk_clamped : avg_clamped) ? (double) params.psd_update_int : per_group;
+      const double per_group = (double) pg.G * (double) N / rate;
+      const double interval = pg.clamped ? (double) params.psd_update_int : per_group;
       const int64_t block_start = (int64_t) (total_samples - block * decim);
       for (size_t j = 0; j < groups; ++j) {
         psd_credit += per_group;
         if (psd_credit + 1e-12 >= interval) {
           psd_credit = fmod(psd_credit, interval);
-          const int64_t first = (int64_t) (j * G) - (int64_t) carried;
+          const int64_t first = (int64_t) (j * pg.G) - (int64_t) carried;
           post_psd((int64_t) src.freq, rate, &psd[j * N], N,
                    (double) (block_start + first * (int64_t) (N * decim)) / src.samp_rate, looped, (uint64_t) hist_fill);
         }

@@ -60,8 +60,6 @@ struct ChdetDeleter { void operator()(sdb_chdet *d) const { sdb_chdet_destroy(d)
 // kernels of feed i (three copy/compute streams).  Each event guards its slot's buffers between the streams.
 struct Slot {
   float *psd = nullptr;                             // [S][frames][Np]
-  float *psd_avg = nullptr;                         // [S][means][Np], frame averaging only (SPEC A)
-  float *psd_max = nullptr, *psd_min = nullptr;     // [S][groups][Np] each, peak detection only (SPEC PK)
   // channel streams: the (latency-bound, 1-CTA-per-32-chains) inspector kernel of feed i runs on its own stream
   // while the FFT kernels of feed i+1 fill the other slot
   float2 *chan = nullptr;
@@ -72,6 +70,18 @@ struct Slot {
   DevBuf<float> sched_spect, sched_est; DevBuf<uint32_t> sched_size; DevBuf<int> sched_valid;
   std::vector<uint32_t> sched_n; std::vector<uint64_t> sched_first;
   Event psd_ready, psd_read, sym_read, insp;
+};
+
+// A reduction over groups of G consecutive main-PSD frames: the frame-averaged PSD (SPEC A, one output: the means) or
+// the peak detectors (SPEC PK, two outputs: the maxima and the minima).  Each output has a carry, the open group of
+// every stream (one frame count serves all: a feed has the same frames per stream), and is double-buffered by parity.
+struct FrameGroups {
+  int fam, n_out;                       // timing family; outputs
+  unsigned G = 0;                       // frames per group, 0: off
+  DevBuf<float> carry[2];               // [output]: [S][Np]
+  DevBuf<float> out[2][2];              // [feed parity][output]: [S][ceil(max_frames / G)][Np]
+  unsigned count = 0;                   // frames of the open group
+  size_t last = 0;                      // groups the latest feed completed
 };
 
 // Everything sdb_engine_commit builds, and the running state that exists only after a commit.  A commit builds it
@@ -139,21 +149,17 @@ struct Plan {
   // DC removal (SDB_FLAG_DC_REMOVE, SPEC R): per-stream estimate, the estimate the current block is corrected with,
   // run sums, and the corrected float32 copy of the block the rest of the path reads
   float2 *d_dc_state = nullptr, *d_dc_cur = nullptr, *d_xdc = nullptr; double2 *d_dc_part = nullptr;
-  // frame averaging (SPEC A): per-stream partial sums of the current group, and its frame count (the same in every
-  // stream: each feed has the same frames per stream)
-  float *d_avg_carry = nullptr;         // [S][Np]
-  unsigned avg_count = 0;
-  // peak detection (SPEC PK): per-stream partial maxima and minima of the current group, and its frame count
-  float *d_peak_max = nullptr, *d_peak_min = nullptr;   // [S][Np] each
-  unsigned peak_count = 0;
+  // frame averaging (SPEC A) and peak detection (SPEC PK), in the order they run
+  FrameGroups avg{FAM_PSD_AVERAGE, 1}, peak{FAM_PSD_PEAK, 2};
   // running state
   unsigned feed_index = 0, host_feeds = 0;
   bool first_feed = true;               // (engines without channels keep no history)
   uint64_t n_fed = 0;                   // samples fed so far
-  size_t last_frames = 0, last_hops = 0, last_means = 0, last_peaks = 0;
+  size_t last_frames = 0, last_hops = 0;
 
-  // the slot of the latest feed (slot 0 before the first)
-  Slot &cur() { return slot[feed_index ? (feed_index - 1) & 1u : 0]; }
+  // the parity of the latest feed (0 before the first) and its slot
+  unsigned cur_parity() const { return feed_index ? (feed_index - 1) & 1u : 0; }
+  Slot &cur() { return slot[cur_parity()]; }
   template <typename T> T *dalloc(size_t n)
   {
     DevBuf<unsigned char> b;
@@ -763,6 +769,72 @@ static int check_group_size(const char *name, unsigned v, unsigned max, unsigned
   return 0;
 }
 
+// G >= 2 turns the stage on: outputs for feeds of at most max_frames frames, and a zero carry
+static int groups_commit(FrameGroups &g, unsigned G, size_t S, unsigned Np, size_t max_frames, const char *oom)
+{
+  if (G < 2) return 0;
+  g.G = G;
+  // a feed completes at most ceil(max_frames / G) groups (G - 1 carried frames + max_frames)
+  const size_t max_groups = (max_frames + G - 1) / G;
+  for (int k = 0; k < g.n_out; ++k) {
+    if (g.out[0][k].alloc(S * max_groups * Np) || g.out[1][k].alloc(S * max_groups * Np) || g.carry[k].alloc(S * Np))
+      return fail(oom);
+    CK(cudaMemset(g.carry[k], 0, S * Np * sizeof(float)));
+  }
+  return 0;
+}
+
+// the groups of this feed's `frames` PSD frames (slot `parity`), on lc's stream
+static int groups_feed(sdb_engine *e, FrameGroups &g, const SdbLaunchCtx &lc, unsigned parity, const float *psd,
+                       unsigned frames, int shift_db)
+{
+  if (!g.G) return 0;
+  const size_t S = e->prm.n_streams;
+  const unsigned groups = (g.count + frames) / g.G;
+  const DevBuf<float> *o = g.out[parity];
+  e->span_begin(g.fam, lc.stream);
+  if (g.n_out == 1)
+    CK(sdb_launch_psd_group_mean(lc, psd, frames, e->Np, S, g.G, g.count, groups, shift_db, g.carry[0], o[0]));
+  else
+    CK(sdb_launch_psd_group_peak(lc, psd, frames, e->Np, S, g.G, g.count, groups, shift_db, g.carry[0], g.carry[1],
+                                 o[0], o[1]));
+  e->span_end(lc.stream);
+  g.count = (g.count + frames) % g.G;
+  g.last = groups;
+  return 0;
+}
+
+// live re-plan: the partial group carries over when both engines group the same frames the same way
+static int groups_migrate(FrameGroups &to, const FrameGroups &from, const sdb_engine *dst, const sdb_engine *src)
+{
+  if (!to.G || to.G != from.G || dst->Np != src->Np || dst->prm.psd_window != src->prm.psd_window) return 0;
+  for (int k = 0; k < to.n_out; ++k)
+    CK(cudaMemcpy(to.carry[k], from.carry[k], to.carry[k].size() * sizeof(float), cudaMemcpyDeviceToDevice));
+  to.count = from.count;
+  return 0;
+}
+
+// blocking read of the latest feed's groups, fenced like sdb_engine_read_psd; g: null without a plan, dst: NULL skips
+static int groups_read(sdb_engine *e, const FrameGroups *g, float *dst0, float *dst1, size_t cap, const char *off)
+{
+  if (!g || !g->G) return fail(off);
+  Plan &p = *e->plan;
+  if (p.feed_index == 0) return fail("no PSD available");
+  const size_t n = (size_t) e->prm.n_streams * g->last * e->Np;
+  if (cap < n) return fail("destination too small");
+  if (n == 0 || (!dst0 && !dst1)) return 0;
+  float *const dst[2] = { dst0, dst1 };
+  Slot &sl = p.cur();
+  CK(cudaSetDevice(e->prm.device));
+  CK(sl.psd_ready.wait_on(p.d2h_stream));
+  for (int k = 0; k < g->n_out; ++k)
+    if (dst[k])
+      CK(cudaMemcpyAsync(dst[k], g->out[p.cur_parity()][k], n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
+  CK(sl.psd_read.record(p.d2h_stream));
+  CK(cudaStreamSynchronize(p.d2h_stream));
+  return 0;
+}
+
 extern "C" int sdb_engine_commit(sdb_engine_t *e)
 {
   if (!e) return fail("null engine");
@@ -796,29 +868,9 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       sl.psd = p.dalloc<float>((size_t) S * max_frames * Np);
       if (!sl.psd) return fail("out of device memory (psd)");
     }
-    if (A >= 2) {
-      // a feed completes at most ceil(max_frames / A) groups (A - 1 carried frames + max_frames)
-      const size_t max_means = (max_frames + A - 1) / A;
-      for (Slot &sl : p.slot) {
-        sl.psd_avg = p.dalloc<float>((size_t) S * max_means * Np);
-        if (!sl.psd_avg) return fail("out of device memory (averaged psd)");
-      }
-      p.d_avg_carry = p.dalloc<float>((size_t) S * Np);
-      if (!p.d_avg_carry) return fail("out of device memory (averaged psd)");
-      CK(cudaMemset(p.d_avg_carry, 0, (size_t) S * Np * sizeof(float)));
-    }
-    if (P >= 2) {
-      // as for the means: at most ceil(max_frames / P) groups a feed, each written to both outputs
-      const size_t max_groups = (max_frames + P - 1) / P;
-      for (Slot &sl : p.slot) {
-        sl.psd_max = p.dalloc<float>((size_t) S * max_groups * Np);
-        sl.psd_min = p.dalloc<float>((size_t) S * max_groups * Np);
-        if (!sl.psd_max || !sl.psd_min) return fail("out of device memory (psd peaks)");
-      }
-      p.d_peak_max = p.dalloc<float>((size_t) S * Np);
-      p.d_peak_min = p.dalloc<float>((size_t) S * Np);
-      if (!p.d_peak_max || !p.d_peak_min) return fail("out of device memory (psd peaks)");
-    }
+    if (groups_commit(p.avg, A, S, Np, max_frames, "out of device memory (averaged psd)") ||
+        groups_commit(p.peak, P, S, Np, max_frames, "out of device memory (psd peaks)"))
+      return -1;
     if (e->cd_enabled) {
       p.chdet.reset(sdb_chdet_new(e->prm.device, Np, S, e->cd_alpha, e->cd_gamma, e->cd_snr, e->cd_min_bins));
       if (!p.chdet) return fail("out of device memory (channel detector)");
@@ -1174,33 +1226,14 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
   // with frame averaging or peak detection the flag applies to their group outputs: the transforms keep the per-frame
   // PSD linear
   const int groups_db = (e->prm.flags & SDB_FLAG_PSD_SHIFT_DB) ? 1 : 0;
-  const int shift_db = p.d_avg_carry || p.d_peak_max ? 0 : groups_db;
+  const int shift_db = p.avg.G || p.peak.G ? 0 : groups_db;
   Slot &sl = p.slot[p.feed_index & 1u];     // result buffers of this feed
 
   const int frames = Np ? (int) (n / Np) : 0;
-  // SPEC A group means of this feed, on the stream of its PSD transforms, after the last of them
-  auto group_means = [&](const SdbLaunchCtx &lc) -> int {
-    if (!p.d_avg_carry) return 0;
-    const unsigned A = e->prm.psd_average, means = (p.avg_count + (unsigned) frames) / A;
-    e->span_begin(FAM_PSD_AVERAGE, lc.stream);
-    CK(sdb_launch_psd_group_mean(lc, sl.psd, (unsigned) frames, Np, S, A, p.avg_count, means, groups_db,
-                                 p.d_avg_carry, sl.psd_avg));
-    e->span_end(lc.stream);
-    p.avg_count = (p.avg_count + (unsigned) frames) % A;
-    p.last_means = means;
-    return 0;
-  };
-  // SPEC PK group extremes of this feed, on the same stream, after the means
-  auto group_peaks = [&](const SdbLaunchCtx &lc) -> int {
-    if (!p.d_peak_max) return 0;
-    const unsigned P = e->prm.psd_peak, groups = (p.peak_count + (unsigned) frames) / P;
-    e->span_begin(FAM_PSD_PEAK, lc.stream);
-    CK(sdb_launch_psd_group_peak(lc, sl.psd, (unsigned) frames, Np, S, P, p.peak_count, groups, groups_db,
-                                 p.d_peak_max, p.d_peak_min, sl.psd_max, sl.psd_min));
-    e->span_end(lc.stream);
-    p.peak_count = (p.peak_count + (unsigned) frames) % P;
-    p.last_peaks = groups;
-    return 0;
+  // the SPEC A means, then the SPEC PK extremes of this feed, on the stream of its PSD transforms after the last one
+  auto frame_groups = [&](const SdbLaunchCtx &lc) -> int {
+    return groups_feed(e, p.avg, lc, p.feed_index & 1u, sl.psd, (unsigned) frames, groups_db) ||
+           groups_feed(e, p.peak, lc, p.feed_index & 1u, sl.psd, (unsigned) frames, groups_db);
   };
   const int H = K ? (int) (n / (W / 2)) : 0;
   const int first = (K && p.first_feed) ? 1 : 0;
@@ -1261,7 +1294,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     }
     if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, p.psd_stream,
                                           &e->launches));
-    if (group_means(pctx) || group_peaks(pctx)) return -1;
+    if (frame_groups(pctx)) return -1;
     CK(sl.psd_ready.record(p.psd_stream));
     CK(sl.psd_ready.wait_on(e->stream));          // the main stream stays the engine's timeline
   } else {
@@ -1294,7 +1327,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
       }
       if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, e->stream,
                                             &e->launches));
-      if (group_means(ctx) || group_peaks(ctx)) return -1;
+      if (frame_groups(ctx)) return -1;
       CK(sl.psd_ready.record(e->stream));
     }
     // ---- channeliser forward transforms
@@ -1423,54 +1456,29 @@ extern "C" int sdb_engine_read_psd(sdb_engine_t *e, float *dst, size_t cap)
   return 0;
 }
 
-extern "C" size_t sdb_engine_psd_average_frames(const sdb_engine_t *e) { return e && e->plan ? e->plan->last_means : 0; }
+extern "C" size_t sdb_engine_psd_average_frames(const sdb_engine_t *e) { return e && e->plan ? e->plan->avg.last : 0; }
 extern "C" const float *sdb_engine_psd_average_device(const sdb_engine_t *e)
 {
-  return e && e->plan ? e->plan->cur().psd_avg : nullptr;
+  return e && e->plan ? e->plan->avg.out[e->plan->cur_parity()][0].get() : nullptr;
 }
 
 extern "C" int sdb_engine_read_psd_average(sdb_engine_t *e, float *dst, size_t cap)
 {
   if (!e || !dst) return fail("null argument");
-  if (!e->plan || !e->plan->d_avg_carry) return fail("PSD averaging not enabled");
-  Plan &p = *e->plan;
-  if (p.feed_index == 0) return fail("no PSD available");
-  const size_t n = (size_t) e->prm.n_streams * p.last_means * e->Np;
-  if (cap < n) return fail("destination too small");
-  if (n == 0) return 0;
-  Slot &sl = p.cur();
-  CK(cudaSetDevice(e->prm.device));
-  CK(sl.psd_ready.wait_on(p.d2h_stream));
-  CK(cudaMemcpyAsync(dst, sl.psd_avg, n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
-  CK(sl.psd_read.record(p.d2h_stream));
-  CK(cudaStreamSynchronize(p.d2h_stream));
-  return 0;
+  return groups_read(e, e->plan ? &e->plan->avg : nullptr, dst, nullptr, cap, "PSD averaging not enabled");
 }
 
-extern "C" size_t sdb_engine_psd_peak_groups(const sdb_engine_t *e) { return e && e->plan ? e->plan->last_peaks : 0; }
+extern "C" size_t sdb_engine_psd_peak_groups(const sdb_engine_t *e) { return e && e->plan ? e->plan->peak.last : 0; }
 extern "C" const float *sdb_engine_psd_peak_device(const sdb_engine_t *e, int which)
 {
   if (!e || !e->plan || (which != 0 && which != 1)) return nullptr;
-  return which ? e->plan->cur().psd_min : e->plan->cur().psd_max;
+  return e->plan->peak.out[e->plan->cur_parity()][which].get();
 }
 
 extern "C" int sdb_engine_read_psd_peak(sdb_engine_t *e, float *max_dst, float *min_dst, size_t cap)
 {
   if (!e) return fail("null argument");
-  if (!e->plan || !e->plan->d_peak_max) return fail("PSD peak detection not enabled");
-  Plan &p = *e->plan;
-  if (p.feed_index == 0) return fail("no PSD available");
-  const size_t n = (size_t) e->prm.n_streams * p.last_peaks * e->Np;
-  if (cap < n) return fail("destination too small");
-  if (n == 0 || (!max_dst && !min_dst)) return 0;
-  Slot &sl = p.cur();
-  CK(cudaSetDevice(e->prm.device));
-  CK(sl.psd_ready.wait_on(p.d2h_stream));
-  if (max_dst) CK(cudaMemcpyAsync(max_dst, sl.psd_max, n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
-  if (min_dst) CK(cudaMemcpyAsync(min_dst, sl.psd_min, n * sizeof(float), cudaMemcpyDeviceToHost, p.d2h_stream));
-  CK(sl.psd_read.record(p.d2h_stream));
-  CK(cudaStreamSynchronize(p.d2h_stream));
-  return 0;
+  return groups_read(e, e->plan ? &e->plan->peak : nullptr, max_dst, min_dst, cap, "PSD peak detection not enabled");
 }
 
 // Asynchronous variants: the copy is queued on the engine's D2H stream behind the kernels that produce
@@ -1655,19 +1663,8 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
     CK(cudaMemcpy(to.d_hist, from.d_hist, (size_t) S * (W / 2) * sizeof(float2), cudaMemcpyDeviceToDevice));
   if (to.d_dc_state && from.d_dc_state)
     CK(cudaMemcpy(to.d_dc_state, from.d_dc_state, S * sizeof(float2), cudaMemcpyDeviceToDevice));
-  // the partial SPEC A group, when both engines average the same frames the same way
-  if (to.d_avg_carry && from.d_avg_carry && dst->Np == src->Np && dst->prm.psd_window == src->prm.psd_window &&
-      dst->prm.psd_average == src->prm.psd_average) {
-    CK(cudaMemcpy(to.d_avg_carry, from.d_avg_carry, (size_t) S * dst->Np * sizeof(float), cudaMemcpyDeviceToDevice));
-    to.avg_count = from.avg_count;
-  }
-  // the partial SPEC PK group, under the same condition
-  if (to.d_peak_max && from.d_peak_max && dst->Np == src->Np && dst->prm.psd_window == src->prm.psd_window &&
-      dst->prm.psd_peak == src->prm.psd_peak) {
-    CK(cudaMemcpy(to.d_peak_max, from.d_peak_max, (size_t) S * dst->Np * sizeof(float), cudaMemcpyDeviceToDevice));
-    CK(cudaMemcpy(to.d_peak_min, from.d_peak_min, (size_t) S * dst->Np * sizeof(float), cudaMemcpyDeviceToDevice));
-    to.peak_count = from.peak_count;
-  }
+  // the partial SPEC A and SPEC PK groups
+  if (groups_migrate(to.avg, from.avg, dst, src) || groups_migrate(to.peak, from.peak, dst, src)) return -1;
   // an engine that had no channel so far kept no input history: its first window starts with this feed
   to.first_feed = from.d_hist ? from.first_feed : true;
   to.n_fed = from.n_fed;
