@@ -152,7 +152,9 @@ int sdb_engine_commit(sdb_engine_t *e);
  * inspector that stays one with the same power_integrate_samples keeps its partial group (SPEC PW).  This is how an
  * analyzer opens, closes, retunes or reconfigures ONE inspector at a block boundary while the others keep running
  * (suscan_analyzer_open_ex_async / close_async / set_inspector_config_async / set_inspector_freq_overridable,
- * Suscan/Analyzer.cpp:459-526).  `src` is synchronised and left intact. */
+ * Suscan/Analyzer.cpp:459-526).  `src` is synchronised and left intact.  The channel detector's state (SPEC K) is not
+ * carried: `dst`'s detector starts afresh, and so does its channel tracking (oracle/SPEC_KT.md), with track ids
+ * beginning again at 1. */
 int sdb_engine_migrate(sdb_engine_t *dst, sdb_engine_t *src);
 /* the same with the caller saying which old channel each new one continues: old_of_new[new handle] = old handle or
  * -1 (a retuned inspector keeps its loops even though its channel moved; only the cross-fade tail restarts) */
@@ -266,8 +268,9 @@ long sdb_engine_read_estimates(sdb_engine_t *e, int handle, int estimator_id, fl
  * struct suscan_analyzer_params.detector_params.{alpha, beta, gamma, snr} + channel_update_int
  * (Suscan/AnalyzerParams.cpp:27-66) -> SUSCAN_ANALYZER_MESSAGE_TYPE_CHANNEL lists of struct sigutils_channel
  * (Suscan/Messages/ChannelMessage.cpp:25-70; include/Suscan/Channel.h:26-32).  alpha = spectrum averaging,
- * gamma = noise-floor averaging, snr = linear power ratio over the floor; beta (signal-level averaging) is accepted
- * for ABI compatibility and unused: levels are reported per update.  One update per feed. */
+ * gamma = noise-floor averaging, snr = linear power ratio over the floor; beta (signal-level averaging) is used only
+ * by channel tracking (sdb_engine_set_channel_tracking): the detector reports levels per update.  One update per
+ * feed. */
 typedef struct {
   double   fc, f_lo, f_hi, bw;      /* Hz (sigutils_channel.fc / f_lo / f_hi / bw) */
   float    snr, S0, N0;             /* linear power: peak averaged level, noise floor, S0 / N0 */
@@ -284,6 +287,31 @@ long sdb_engine_read_channels(sdb_engine_t *e, uint32_t stream, double center_fr
 /* the lists of all streams in one read: centers[n_streams] (host), out[n_streams][cap], counts[n_streams] */
 int  sdb_engine_read_all_channels(sdb_engine_t *e, const double *centers, sdb_detected_channel *out, size_t cap,
                                   uint32_t *counts);
+/* ---- channel tracking across detector updates (oracle/SPEC_KT.md) ----
+ * Follows each detected channel from one update to the next: a detection continues the live track it overlaps most,
+ * whose peak level S0 is then smoothed by the detector's beta; a track no detection continues is kept for `hold`
+ * further updates (its range and S0 unchanged) and then removed; a detection no track continues opens a new track.
+ * At most 256 tracks per stream.  Enable with sdb_engine_set_channel_tracking() before sdb_engine_commit(), after
+ * sdb_engine_set_channel_detector(); beta must then be in (0, 1] (checked at commit).  Without it the engine issues
+ * the same launches as before and beta stays unused. */
+#define SDB_CHTRACK_HOLD_MAX 65535u
+typedef struct {
+  double   fc, f_lo, f_hi, bw;      /* Hz, as sdb_detected_channel, over the track's latest range */
+  float    snr, S0, N0;             /* beta-smoothed peak level, the detector's current floor, S0 / N0 */
+  uint32_t bin_lo, bin_hi;          /* [lo, hi) in ascending-frequency bin order */
+  uint32_t id;                      /* per stream, from 1 in order of opening */
+  uint32_t age, present, misses;    /* updates since opening, updates detected (sigutils_channel.age / .present),
+                                       updates missed in a row (> 0: in hold) */
+} sdb_tracked_channel;
+int  sdb_engine_set_channel_tracking(sdb_engine_t *e, uint32_t hold);
+/* live tracks of one stream after the latest feed, ascending (bin_lo, id); *total = live tracks before the cap,
+ * *dropped = detections not tracked because 256 tracks were live, since commit (either pointer may be NULL) */
+long sdb_engine_read_tracked_channels(sdb_engine_t *e, uint32_t stream, double center_freq, sdb_tracked_channel *out,
+                                      size_t cap, uint32_t *total, uint64_t *dropped);
+/* all streams in one read: centers[n_streams] (host), out[n_streams][cap], counts[n_streams], dropped[n_streams]
+ * (may be NULL) */
+int  sdb_engine_read_all_tracked_channels(sdb_engine_t *e, const double *centers, sdb_tracked_channel *out, size_t cap,
+                                          uint32_t *counts, uint64_t *dropped);
 /* stand-alone detector on any device-resident linear PSD (e.g. the stitched SpectrumView of the panoramic
  * scanner, BASELINE config 5 "per-GPU channel detector"): psd_dev[stream][frame][n_bins], DC at index 0 */
 typedef struct sdb_chdet sdb_chdet_t;
@@ -516,6 +544,14 @@ typedef struct {
    * SDB_SPECTRUM_EMITS_MAX).  0 = one emission per block that fills a frame, of the largest power of two <= 4096 the
    * block fills.  sdb_analyzer_new and _set_params_async refuse negative values, infinities and NaN. */
   float   spectrum_update_int;
+  /* Channel tracking (oracle/SPEC_KT.md), seconds.  0 (the default): none, and CHANNEL messages carry each update's
+   * detector list as before.  > 0: the detector follows channels across updates with
+   * hold = ceil(channel_hold_int / block duration) updates (at most SDB_CHTRACK_HOLD_MAX), and CHANNEL messages carry
+   * the tracked list: a channel that drops out for less than the hold stays one entry, S0 is smoothed by
+   * detector_params.beta (which must then be in (0, 1]), and tracked_list adds ids, age and present.  The detector
+   * runs only when channel_update_int > 0, so without it this has no effect.  Any re-plan restarts the tracks, as it
+   * restarts the detector.  Negative, NaN and infinite values are refused. */
+  float   channel_hold_int;
 } sdb_analyzer_params;
 enum { SDB_PSD_DETECTOR_DEFAULT = 0, SDB_PSD_DETECTOR_POS_PEAK = 1, SDB_PSD_DETECTOR_NEG_PEAK = 2 };
 
@@ -565,7 +601,11 @@ typedef struct {                  /* suscan_analyzer_inspector_msg, fields this 
 } sdb_analyzer_inspector_msg;
 /* suscan_analyzer_channel_msg (Suscan/Messages/ChannelMessage.cpp:25-70): posted every channel_update_int seconds
  * of signal time when channel_update_int > 0 */
-typedef struct { const void *source; uint32_t channel_count; sdb_detected_channel *channel_list; } sdb_analyzer_channel_msg;
+typedef struct {
+  const void *source; uint32_t channel_count; sdb_detected_channel *channel_list;
+  /* with channel_hold_int > 0: the same channel_count tracks in full, in the order of channel_list; otherwise NULL */
+  sdb_tracked_channel *tracked_list;
+} sdb_analyzer_channel_msg;
 typedef struct { int32_t code; char *err_msg; } sdb_analyzer_status_msg;   /* suscan_analyzer_status_msg */
 typedef struct {                  /* suscan_source_info, fields this path fills */
   uint64_t permissions, source_samp_rate, effective_samp_rate; float measured_samp_rate; double frequency;

@@ -41,6 +41,14 @@ class DetectedChannel(C.Structure):
                 ("bin_hi", C.c_uint32)]
 
 
+class TrackedChannel(C.Structure):
+    """sdb_tracked_channel: a detected channel followed across updates (oracle/SPEC_KT.md)."""
+    _fields_ = [("fc", C.c_double), ("f_lo", C.c_double), ("f_hi", C.c_double), ("bw", C.c_double),
+                ("snr", C.c_float), ("S0", C.c_float), ("N0", C.c_float), ("bin_lo", C.c_uint32),
+                ("bin_hi", C.c_uint32), ("id", C.c_uint32), ("age", C.c_uint32), ("present", C.c_uint32),
+                ("misses", C.c_uint32)]
+
+
 class CaptureInfo(C.Structure):
     """sdb_capture_info"""
     _fields_ = [("container", C.c_int32), ("sample_format", C.c_int32), ("samp_rate", C.c_double),
@@ -301,6 +309,11 @@ _PROTOS = {
     "sdb_engine_read_estimates": (C.c_long, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t]),
     "sdb_engine_set_channel_detector": (C.c_int, [C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_uint32]),
     "sdb_engine_read_channels": (C.c_long, [C.c_void_p, C.c_uint32, C.c_double, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sdb_engine_set_channel_tracking": (C.c_int, [C.c_void_p, C.c_uint32]),
+    "sdb_engine_read_tracked_channels": (C.c_long, [C.c_void_p, C.c_uint32, C.c_double, C.c_void_p, C.c_size_t,
+                                                    C.c_void_p, C.c_void_p]),
+    "sdb_engine_read_all_tracked_channels": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                        C.c_void_p]),
     "sdb_chdet_new": (C.c_void_p, [C.c_int, C.c_uint32, C.c_uint32, C.c_float, C.c_float, C.c_float, C.c_uint32]),
     "sdb_chdet_destroy": (None, [C.c_void_p]),
     "sdb_chdet_feed_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_size_t]),
@@ -642,6 +655,29 @@ class Engine:
         tot = C.c_uint32()
         n = _check(self._L.sdb_engine_read_channels(self._h, stream, center_freq, out, cap, C.byref(tot)))
         return [out[i] for i in range(n)], tot.value
+
+    # ---- channel tracking across detector updates (oracle/SPEC_KT.md): before commit, after set_channel_detector
+    def set_channel_tracking(self, hold):
+        """follow detected channels across updates; a channel no update detects is kept for `hold` more updates"""
+        _check(self._L.sdb_engine_set_channel_tracking(self._h, hold))
+
+    def read_tracked_channels(self, stream, center_freq=0.0, cap=256):
+        """-> (list of TrackedChannel in ascending (bin_lo, id), live tracks before the cap, detections dropped at
+        the 256-track cap since commit)"""
+        out = (TrackedChannel * cap)()
+        tot, dropped = C.c_uint32(), C.c_uint64()
+        n = _check(self._L.sdb_engine_read_tracked_channels(self._h, stream, center_freq, out, cap, C.byref(tot),
+                                                            C.byref(dropped)))
+        return [out[i] for i in range(n)], tot.value, dropped.value
+
+    def read_all_tracked_channels(self, centers, cap=256):
+        """-> per stream (list of TrackedChannel, dropped), from one read of every stream"""
+        S = len(centers)
+        c = (C.c_double * S)(*centers)
+        out = (TrackedChannel * (S * cap))()
+        counts, dropped = (C.c_uint32 * S)(), (C.c_uint64 * S)()
+        _check(self._L.sdb_engine_read_all_tracked_channels(self._h, c, out, cap, counts, dropped))
+        return [([out[s * cap + i] for i in range(counts[s])], dropped[s]) for s in range(S)]
 
     # ---- inspector spectrum sources / estimators (SPEC U; Suscan/Analyzer.cpp:539-565)
     def set_spectrum_source(self, h, kind, size=1024):

@@ -33,7 +33,8 @@ class DetectorParams(C.Structure):
 class AnalyzerParams(C.Structure):
     _fields_ = [("mode", C.c_int32), ("detector_params", DetectorParams), ("channel_update_int", C.c_float),
                 ("psd_update_int", C.c_float), ("min_freq", C.c_double), ("max_freq", C.c_double),
-                ("psd_average", C.c_int32), ("psd_detector", C.c_int32), ("spectrum_update_int", C.c_float)]
+                ("psd_average", C.c_int32), ("psd_detector", C.c_int32), ("spectrum_update_int", C.c_float),
+                ("channel_hold_int", C.c_float)]
 
 
 READ_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.c_void_p, C.c_size_t)
@@ -74,7 +75,8 @@ class InspectorMsg(C.Structure):
 
 
 class ChannelMsg(C.Structure):
-    _fields_ = [("source", C.c_void_p), ("channel_count", C.c_uint32), ("channel_list", C.c_void_p)]
+    _fields_ = [("source", C.c_void_p), ("channel_count", C.c_uint32), ("channel_list", C.c_void_p),
+                ("tracked_list", C.c_void_p)]
 
 
 class StatusMsg(C.Structure):
@@ -85,13 +87,16 @@ class Analyzer:
     def __init__(self, samp_rate, window_size=8192, window="hann", psd_update_int=0.04, data=None, read=None,
                  read_size=0, loop=False, freq=0.0, device=0, channel_update_int=0.0, alpha=0.25, beta=0.25,
                  gamma=0.5, snr=8.0, wide=False, min_freq=0.0, max_freq=0.0, set_frequency=None, decimation=1,
-                 psd_average=0, psd_detector=0, spectrum_update_int=0.0):
+                 psd_average=0, psd_detector=0, spectrum_update_int=0.0, channel_hold_int=0.0):
         """decimation: source decimation D (SPEC L); the analyzer then runs at samp_rate / D.
         psd_average: non-zero posts the mean of the frames of every psd_update_int instead of one frame (SPEC A).
         psd_detector: "pos_peak" / "neg_peak" (or PSD_DETECTOR's numbers) post the per-bin maximum / minimum of those
         frames instead (SPEC PK); 0 or "default" leaves the choice to psd_average.
         spectrum_update_int: > 0 emits inspector spectra and baud estimates every that many seconds of channel time,
-        over 4096-point frames carried across blocks (SPEC US); 0 = once per block that fills a frame."""
+        over 4096-point frames carried across blocks (SPEC US); 0 = once per block that fills a frame.
+        channel_hold_int: > 0 follows detected channels across blocks (SPEC KT): CHANNEL messages then list tracks,
+        kept through gaps shorter than this many seconds, with S0 smoothed by beta and id / age / present /
+        misses; needs channel_update_int > 0 (the detector)."""
         self._L = load_library()
         p = AnalyzerParams()
         p.mode = 1 if wide else 0                      # SDB_ANALYZER_MODE_{CHANNEL, WIDE_SPECTRUM}
@@ -105,6 +110,7 @@ class Analyzer:
         p.psd_average = psd_average
         p.psd_detector = PSD_DETECTOR[psd_detector] if isinstance(psd_detector, str) else psd_detector
         p.spectrum_update_int = spectrum_update_int
+        p.channel_hold_int = channel_hold_int
         self.params = p
         s = SourceConfig()
         s.samp_rate, s.freq, s.read_size, s.loop, s.device = samp_rate, freq, read_size, int(loop), device
@@ -271,6 +277,11 @@ class Analyzer:
                 arr = C.cast(m.channel_list, C.POINTER(DetectedChannel))
                 out = dict(channels=[dict(fc=arr[i].fc, f_lo=arr[i].f_lo, f_hi=arr[i].f_hi, bw=arr[i].bw,
                                           snr=arr[i].snr, S0=arr[i].S0, N0=arr[i].N0) for i in range(m.channel_count)])
+                if m.tracked_list:
+                    from . import TrackedChannel
+                    tr = C.cast(m.tracked_list, C.POINTER(TrackedChannel))
+                    for i, c in enumerate(out["channels"]):
+                        c.update(id=tr[i].id, age=tr[i].age, present=tr[i].present, misses=tr[i].misses)
             elif name == "SOURCE_INFO":
                 m = C.cast(ptr, C.POINTER(SourceInfo)).contents
                 out = dict(source_samp_rate=m.source_samp_rate, effective_samp_rate=m.effective_samp_rate,

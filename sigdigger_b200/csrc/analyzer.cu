@@ -310,6 +310,11 @@ struct sdb_analyzer {
       sdb_engine_set_channel_detector(e.get(), params.detector_params.alpha, params.detector_params.beta,
                                       params.detector_params.gamma,
                                       params.detector_params.snr > 0 ? params.detector_params.snr : 4.0f, 2);
+    if (parent < 0 && params.channel_update_int > 0 && params.channel_hold_int > 0) {
+      // SPEC KT: one tracking update per block, so the hold in seconds becomes whole blocks
+      const double h = std::ceil((double) params.channel_hold_int * rate / (double) block);
+      if (sdb_engine_set_channel_tracking(e.get(), (uint32_t) std::min<double>(h, SDB_CHTRACK_HOLD_MAX))) return nullptr;
+    }
     if (sdb_engine_commit(e.get())) return nullptr;
     if (old && sdb_engine_same_geometry(e.get(), old))
       sdb_engine_migrate_map(e.get(), old, old_of_new.data(), old_of_new.size());
@@ -864,6 +869,26 @@ struct sdb_analyzer {
       chan_credit = fmod(chan_credit, params.channel_update_int);
       std::vector<sdb_detected_channel> ch(256);
       uint32_t total = 0;
+      if (params.channel_hold_int > 0) {
+        // SPEC KT: the tracked list, and each track as a sigutils_channel with its smoothed S0
+        std::vector<sdb_tracked_channel> tr(256);
+        const long nc = sdb_engine_read_tracked_channels(eng.get(), 0, src.freq, tr.data(), tr.size(), &total, nullptr);
+        if (nc < 0) return;
+        for (long i = 0; i < nc; ++i) {
+          sdb_detected_channel &c = ch[i];
+          const sdb_tracked_channel &t = tr[i];
+          c.fc = t.fc; c.f_lo = t.f_lo; c.f_hi = t.f_hi; c.bw = t.bw; c.snr = t.snr; c.S0 = t.S0; c.N0 = t.N0;
+          c.bin_lo = t.bin_lo; c.bin_hi = t.bin_hi;
+        }
+        sdb_analyzer_channel_msg *m = (sdb_analyzer_channel_msg *) calloc(1, sizeof(*m));
+        m->channel_count = (uint32_t) nc;
+        m->channel_list = (sdb_detected_channel *) malloc(std::max<long>(1, nc) * sizeof(sdb_detected_channel));
+        memcpy(m->channel_list, ch.data(), (size_t) nc * sizeof(sdb_detected_channel));
+        m->tracked_list = (sdb_tracked_channel *) malloc(std::max<long>(1, nc) * sizeof(sdb_tracked_channel));
+        memcpy(m->tracked_list, tr.data(), (size_t) nc * sizeof(sdb_tracked_channel));
+        post(SDB_ANALYZER_MESSAGE_TYPE_CHANNEL, m);
+        return;
+      }
       long nc = sdb_engine_read_channels(eng.get(), 0, src.freq, ch.data(), ch.size(), &total);
       if (nc >= 0) {
         sdb_analyzer_channel_msg *m = (sdb_analyzer_channel_msg *) calloc(1, sizeof(*m));
@@ -936,6 +961,10 @@ extern "C" sdb_analyzer_t *sdb_analyzer_new(const sdb_analyzer_params *params, c
     fail("spectrum_update_int must be a finite number of seconds >= 0");
     return nullptr;
   }
+  if (!(params->channel_hold_int >= 0.0f) || !std::isfinite(params->channel_hold_int)) {
+    fail("channel_hold_int must be a finite number of seconds >= 0");
+    return nullptr;
+  }
   const uint32_t D = src->decimation ? src->decimation : 1;
   if (D > SDB_DECIMATION_MAX) {
     fail("source decimation must be at most " + std::to_string(SDB_DECIMATION_MAX) + ", got " + std::to_string(D));
@@ -996,7 +1025,8 @@ extern "C" void sdb_analyzer_dispose_message(uint32_t type, void *ptr)
       free(((sdb_analyzer_inspector_msg *) ptr)->class_name);
       free(((sdb_analyzer_inspector_msg *) ptr)->spectrum_data); break;
     case SDB_ANALYZER_MESSAGE_TYPE_CHANNEL:
-      free(((sdb_analyzer_channel_msg *) ptr)->channel_list); break;
+      free(((sdb_analyzer_channel_msg *) ptr)->channel_list);
+      free(((sdb_analyzer_channel_msg *) ptr)->tracked_list); break;
     case SDB_ANALYZER_MESSAGE_TYPE_EOS:
     case SDB_ANALYZER_MESSAGE_TYPE_READ_ERROR:
     case SDB_ANALYZER_MESSAGE_TYPE_SOURCE_INIT:
@@ -1185,6 +1215,7 @@ extern "C" int sdb_analyzer_set_params_async(sdb_analyzer_t *a, const sdb_analyz
   if (N < 16 || (N & (N - 1))) return -1;
   if (p->psd_detector < SDB_PSD_DETECTOR_DEFAULT || p->psd_detector > SDB_PSD_DETECTOR_NEG_PEAK) return -1;
   if (!(p->spectrum_update_int >= 0.0f) || !std::isfinite(p->spectrum_update_int)) return -1;
+  if (!(p->channel_hold_int >= 0.0f) || !std::isfinite(p->channel_hold_int)) return -1;
   Cmd c; c.kind = Cmd::SET_PARAMS; c.req_id = req_id; c.params = *p;
   return push_cmd(a, std::move(c));
 }

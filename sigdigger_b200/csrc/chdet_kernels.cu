@@ -503,3 +503,216 @@ extern "C" long sdb_chdet_read(sdb_chdet_t *d, uint32_t stream, double samp_rate
   }
   return (long) n;
 }
+
+// ---------------------------------------------------------------------------------------------
+// channel tracking across detector updates (oracle/SPEC_KT.md)
+// ---------------------------------------------------------------------------------------------
+// k_chtrack: one warp per stream, right after the detector on the same CUDA stream, over the detector's device list
+// (d_out / d_count).  The table of the previous update (ascending (a, id), so that index order is the KT.3 tie-break
+// order) is read from one parity and the new table written to the other.  Lane l keeps the ranges of tracks l + 32 j
+// in registers; each detection, in ascending frequency, takes the warp maximum of (overlap << 8 | 255 - index) over
+// the tracks not yet matched.  Survivors and new tracks are then gathered in shared memory and placed by their rank
+// in (a, id).
+struct SdbTrackDev { unsigned a, b; float s0, snr; unsigned id, age, present, misses; };
+struct SdbTrackHdr { unsigned count, issued; float n0; unsigned pad; unsigned long long dropped; };   // ids 1 ... issued
+
+struct ChtrackK {
+  const SdbDetectedDev *det; const unsigned *count; const float *n0;
+  const SdbTrackDev *tr_in; const SdbTrackHdr *hd_in;
+  SdbTrackDev *tr_out; SdbTrackHdr *hd_out;
+  float beta; unsigned hold;
+};
+
+__global__ void __launch_bounds__(32) k_chtrack(const ChtrackK p)
+{
+  __shared__ unsigned s_da[CHDET_CAP], s_db[CHDET_CAP];
+  __shared__ float s_ds[CHDET_CAP];
+  __shared__ short s_dm[CHDET_CAP];             // detection -> matched track, -1: none
+  __shared__ short s_tm[CHDET_CAP];             // matched track -> its detection
+  __shared__ SdbTrackDev s_new[CHDET_CAP];      // the new table before ordering
+  const int lane = threadIdx.x, st = blockIdx.x;
+  const SdbTrackHdr h = p.hd_in[st];
+  const unsigned nt = h.count, nd = p.count[st];
+  const SdbDetectedDev *__restrict__ det = p.det + (size_t) st * CHDET_CAP;
+  const SdbTrackDev *__restrict__ in = p.tr_in + (size_t) st * CHDET_CAP;
+  for (unsigned d = lane; d < nd; d += 32) { s_da[d] = det[d].bin_lo; s_db[d] = det[d].bin_hi; s_ds[d] = det[d].s0; }
+  unsigned ta[CHDET_CAP / 32], tb[CHDET_CAP / 32], matched = 0;
+#pragma unroll
+  for (int j = 0; j < CHDET_CAP / 32; ++j) {
+    const unsigned t = lane + 32 * j;
+    ta[j] = t < nt ? in[t].a : 0u; tb[j] = t < nt ? in[t].b : 0u;   // (an empty slot never overlaps)
+  }
+  __syncwarp();
+  // ---- KT.3: detections in ascending frequency; the largest overlap, then the smaller index (= smaller (a, id))
+  for (unsigned d = 0; d < nd; ++d) {
+    const int ad = (int) s_da[d], bd = (int) s_db[d];
+    unsigned best = 0;
+#pragma unroll
+    for (int j = 0; j < CHDET_CAP / 32; ++j) {
+      const int ov = min(bd, (int) tb[j]) - max(ad, (int) ta[j]);
+      if (!((matched >> j) & 1u) && ov > 0)
+        best = max(best, ((unsigned) ov << 8) | (255u - (unsigned) (lane + 32 * j)));
+    }
+    best = __reduce_max_sync(0xffffffffu, best);
+    const int t = best ? 255 - (int) (best & 255u) : -1;
+    if (t >= 0 && (t & 31) == lane) { matched |= 1u << (t >> 5); s_tm[t] = (short) d; }
+    if (lane == 0) s_dm[d] = (short) t;
+  }
+  __syncwarp();
+  // ---- KT.4 / KT.5: matched tracks take the detection, unmatched ones age and leave after `hold` misses
+  unsigned live = 0;
+  const unsigned lt = (1u << lane) - 1u;
+#pragma unroll
+  for (int j = 0; j < CHDET_CAP / 32; ++j) {
+    const unsigned t = lane + 32 * j;
+    SdbTrackDev r;
+    bool keep = false;
+    if (t < nt) {
+      r = in[t];
+      r.age += 1;
+      if ((matched >> j) & 1u) {
+        const int d = s_tm[t];
+        r.a = s_da[d]; r.b = s_db[d];
+        r.s0 = __fadd_rn(r.s0, __fmul_rn(p.beta, __fsub_rn(s_ds[d], r.s0)));
+        r.present += 1; r.misses = 0;
+        keep = true;
+      } else {
+        r.misses += 1;
+        keep = r.misses <= p.hold;
+      }
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, keep);
+    if (keep) s_new[live + __popc(m & lt)] = r;
+    live += __popc(m);
+  }
+  // ---- KT.6: unmatched detections open tracks in ascending frequency while fewer than 256 are live
+  unsigned unm = 0, issued = h.issued;
+  for (unsigned d0 = 0; d0 < nd; d0 += 32) {
+    const unsigned d = d0 + lane;
+    const bool u = d < nd && s_dm[d] < 0;
+    const unsigned m = __ballot_sync(0xffffffffu, u);
+    const unsigned k = unm + __popc(m & lt);              // rank among the unmatched detections
+    if (u && live + k < CHDET_CAP) {
+      SdbTrackDev r;
+      r.a = s_da[d]; r.b = s_db[d]; r.s0 = s_ds[d]; r.snr = 0.0f;
+      r.id = issued + k + 1; r.age = 1; r.present = 1; r.misses = 0;
+      s_new[live + k] = r;
+    }
+    unm += __popc(m);
+  }
+  const unsigned ins = min(unm, CHDET_CAP - live), n = live + ins;
+  __syncwarp();
+  // ---- KT.7: ascending (a, id) by rank (ids are unique), snr against the detector's current floor
+  const float n0 = p.n0[st];
+  SdbTrackDev *__restrict__ out = p.tr_out + (size_t) st * CHDET_CAP;
+  for (unsigned i = lane; i < n; i += 32) {
+    SdbTrackDev r = s_new[i];
+    const unsigned long long ki = ((unsigned long long) r.a << 32) | r.id;
+    unsigned rank = 0;
+    for (unsigned q = 0; q < n; ++q)
+      rank += (((unsigned long long) s_new[q].a << 32) | s_new[q].id) < ki;
+    r.snr = r.s0 / n0;
+    out[rank] = r;
+  }
+  if (lane == 0) {
+    SdbTrackHdr o;
+    o.count = n; o.issued = issued + ins; o.n0 = n0; o.pad = 0; o.dropped = h.dropped + (unm - ins);
+    p.hd_out[st] = o;
+  }
+}
+
+// host object of the tracker: the two tables and headers by update parity; `cur` holds the latest
+struct sdb_chtrack {
+  int device = 0; unsigned N = 0, S = 0, hold = 0, cur = 0;
+  float beta = 1.0f;
+  DevBuf<SdbTrackDev> tr[2]; DevBuf<SdbTrackHdr> hd[2];
+};
+
+void sdb_chtrack_destroy(sdb_chtrack *t)
+{
+  if (!t) return;
+  cudaSetDevice(t->device);
+  delete t;
+}
+
+sdb_chtrack *sdb_chtrack_new(int device, uint32_t n_bins, uint32_t n_streams, float beta, uint32_t hold)
+{
+  if (!(beta > 0.0f && beta <= 1.0f) || hold > SDB_CHTRACK_HOLD_MAX || n_streams < 1) return nullptr;
+  if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+  sdb_chtrack *t = new sdb_chtrack();
+  t->device = device; t->N = n_bins; t->S = n_streams; t->beta = beta; t->hold = hold;
+  const size_t S = n_streams;
+  bool ok = true;
+  for (int i = 0; i < 2 && ok; ++i)
+    ok = t->tr[i].alloc(S * CHDET_CAP) == cudaSuccess && t->hd[i].alloc(S) == cudaSuccess &&
+         cudaMemset(t->hd[i], 0, S * sizeof(SdbTrackHdr)) == cudaSuccess;   // no track, no id issued, nothing dropped
+  if (!ok || cudaDeviceSynchronize() != cudaSuccess) { cudaGetLastError(); sdb_chtrack_destroy(t); return nullptr; }
+  return t;
+}
+
+// KT.1: one update per detector update, i.e. per feed with frames, after sdb_chdet_feed_stream on the same stream
+cudaError_t sdb_chtrack_feed_stream(sdb_chtrack *t, const sdb_chdet *d, uint32_t frames, cudaStream_t stream,
+                                    uint64_t *launch_counter)
+{
+  if (frames == 0) return cudaSuccess;
+  ChtrackK p;
+  p.det = d->d_out; p.count = d->d_count; p.n0 = d->d_n0;
+  p.tr_in = t->tr[t->cur]; p.hd_in = t->hd[t->cur];
+  p.tr_out = t->tr[t->cur ^ 1u]; p.hd_out = t->hd[t->cur ^ 1u];
+  p.beta = t->beta; p.hold = t->hold;
+  k_chtrack<<<t->S, 32, 0, stream>>>(p);
+  if (launch_counter) *launch_counter += 1;
+  t->cur ^= 1u;
+  return cudaGetLastError();
+}
+
+static void track_to_host(const SdbTrackDev &q, float n0, double center, double df, double half, sdb_tracked_channel &c)
+{
+  c.bin_lo = q.a; c.bin_hi = q.b;
+  c.f_lo = center + ((double) q.a - half) * df;        // K.4 frequencies over the track's range
+  c.f_hi = center + ((double) q.b - half) * df;
+  c.fc = 0.5 * (c.f_lo + c.f_hi); c.bw = c.f_hi - c.f_lo;
+  c.S0 = q.s0; c.N0 = n0; c.snr = q.snr;
+  c.id = q.id; c.age = q.age; c.present = q.present; c.misses = q.misses;
+}
+
+// the tracks of one stream after the latest update; *total = live tracks, *dropped = detections not tracked so far
+long sdb_chtrack_read(sdb_chtrack *t, uint32_t stream, double samp_rate, double center_freq, sdb_tracked_channel *out,
+                      size_t cap, uint32_t *total, uint64_t *dropped)
+{
+  if (!t || stream >= t->S || (!out && cap)) return -1;
+  if (cudaSetDevice(t->device) != cudaSuccess) return -1;
+  SdbTrackHdr h;
+  if (cudaMemcpy(&h, t->hd[t->cur] + stream, sizeof(h), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+  const size_t n = h.count < cap ? h.count : cap;
+  std::vector<SdbTrackDev> q(n);
+  if (n && cudaMemcpy(q.data(), t->tr[t->cur] + (size_t) stream * CHDET_CAP, n * sizeof(SdbTrackDev),
+                      cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+  const double df = samp_rate / (double) t->N, half = (double) (t->N / 2);
+  for (size_t i = 0; i < n; ++i) track_to_host(q[i], h.n0, center_freq, df, half, out[i]);
+  if (total) *total = h.count;
+  if (dropped) *dropped = h.dropped;
+  return (long) n;
+}
+
+// every stream in two copies: centers[S] host, out[S][cap], counts[S] (clamped to cap), dropped[S] (may be NULL)
+int sdb_chtrack_read_all(sdb_chtrack *t, double samp_rate, const double *centers, sdb_tracked_channel *out, size_t cap,
+                         uint32_t *counts, uint64_t *dropped)
+{
+  if (!t || !centers || !out || !counts) return -1;
+  if (cudaSetDevice(t->device) != cudaSuccess) return -1;
+  const size_t S = t->S;
+  std::vector<SdbTrackHdr> h(S);
+  std::vector<SdbTrackDev> q(S * CHDET_CAP);
+  if (cudaMemcpy(h.data(), t->hd[t->cur], S * sizeof(SdbTrackHdr), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+  if (cudaMemcpy(q.data(), t->tr[t->cur], q.size() * sizeof(SdbTrackDev), cudaMemcpyDeviceToHost) != cudaSuccess)
+    return -1;
+  const double df = samp_rate / (double) t->N, half = (double) (t->N / 2);
+  for (size_t s = 0; s < S; ++s) {
+    const size_t n = h[s].count < cap ? h[s].count : cap;
+    counts[s] = (uint32_t) n;
+    if (dropped) dropped[s] = h[s].dropped;
+    for (size_t i = 0; i < n; ++i) track_to_host(q[s * CHDET_CAP + i], h[s].n0, centers[s], df, half, out[s * cap + i]);
+  }
+  return 0;
+}

@@ -46,15 +46,17 @@ struct Channel {
 
 struct TimedSpan { int family; Event a, b; };
 enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_POWER, FAM_PSD_PEAK,
-       FAM_SPECTSCHED, FAM_COUNT };
+       FAM_SPECTSCHED, FAM_CHAN_TRACK, FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
-                                            "inspector", "psd_average", "power", "psd_peak", "spectsrc_sched" };
+                                            "inspector", "psd_average", "power", "psd_peak", "spectsrc_sched",
+                                            "chan_track" };
 
 // SPEC PW: samples per mean of a power inspector (power.integrate-samples, 0 read as 1)
 static uint64_t power_m(const sdb_inspector_config &c) { return c.power_integrate_samples ? c.power_integrate_samples : 1; }
 static bool is_power(const Channel &c) { return c.has_insp && c.cfg.insp_class == SDB_INSP_POWER; }
 
 struct ChdetDeleter { void operator()(sdb_chdet *d) const { sdb_chdet_destroy(d); } };
+struct ChtrackDeleter { void operator()(sdb_chtrack *t) const { sdb_chtrack_destroy(t); } };
 
 // Host-buffer pipeline: results are double-buffered by feed parity so that the D2H reads of feed i-1 overlap the
 // kernels of feed i (three copy/compute streams).  Each event guards its slot's buffers between the streams.
@@ -127,6 +129,8 @@ struct Plan {
   DevBuf<SdbPowerCarry> power_carry;
   // channel detector on the main PSD (SPEC K; chdet_kernels.cu)
   std::unique_ptr<sdb_chdet, ChdetDeleter> chdet;
+  // channel tracking across the detector's updates (SPEC KT), when enabled
+  std::unique_ptr<sdb_chtrack, ChtrackDeleter> chtrack;
   // inspector spectrum sources / estimators (SPEC U)
   std::vector<SdbSpectCfg> h_spect; SdbSpectCfg *d_spectcfg = nullptr;
   float *d_spect = nullptr; size_t spect_stride = 0; int spect_max_ns = 0;
@@ -192,6 +196,8 @@ struct sdb_engine {
   // channel detector parameters
   bool cd_enabled = false;
   float cd_alpha = 0, cd_gamma = 0, cd_snr = 0; unsigned cd_min_bins = 1;
+  float cd_beta = 0;
+  bool ct_enabled = false; unsigned ct_hold = 0;    // channel tracking (SPEC KT)
   std::unique_ptr<Plan> plan;           // set by a successful sdb_engine_commit
   // timing
   std::vector<TimedSpan> spans;
@@ -397,7 +403,6 @@ extern "C" int sdb_engine_set_inspector(sdb_engine_t *e, int handle, const sdb_i
 extern "C" int sdb_engine_set_channel_detector(sdb_engine_t *e, float alpha, float beta, float gamma, float snr,
                                                uint32_t min_bins)
 {
-  (void) beta;
   if (!e) return fail("null argument");
   if (e->plan) return fail("engine already committed");
   if (!e->prm.psd_size) return fail("the channel detector needs the main PSD");
@@ -406,6 +411,17 @@ extern "C" int sdb_engine_set_channel_detector(sdb_engine_t *e, float alpha, flo
   if (!(snr > 0.0f) || !(alpha >= 0.0f && alpha <= 1.0f) || !(gamma >= 0.0f && gamma <= 1.0f))
     return fail("detector parameters out of range");
   e->cd_enabled = true; e->cd_alpha = alpha; e->cd_gamma = gamma; e->cd_snr = snr; e->cd_min_bins = min_bins ? min_bins : 1;
+  e->cd_beta = beta;                  // used by channel tracking only (checked at commit when tracking is on)
+  return 0;
+}
+
+extern "C" int sdb_engine_set_channel_tracking(sdb_engine_t *e, uint32_t hold)
+{
+  if (!e) return fail("null argument");
+  if (e->plan) return fail("engine already committed");
+  if (!e->cd_enabled) return fail("channel tracking needs the channel detector (sdb_engine_set_channel_detector)");
+  if (hold > SDB_CHTRACK_HOLD_MAX) return fail("channel tracking hold must be at most 65535 updates");
+  e->ct_enabled = true; e->ct_hold = hold;
   return 0;
 }
 
@@ -435,6 +451,36 @@ extern "C" int sdb_engine_read_all_channels(sdb_engine_t *e, const double *cente
   CK(cudaStreamSynchronize(p.psd_stream ? p.psd_stream.get() : e->stream.get()));
   CK(cudaStreamSynchronize(e->stream));
   if (sdb_chdet_read_all(p.chdet.get(), e->samp_rate, centers, out, cap, counts)) return fail("channel read failed");
+  return 0;
+}
+
+extern "C" long sdb_engine_read_tracked_channels(sdb_engine_t *e, uint32_t stream, double center_freq,
+                                                 sdb_tracked_channel *out, size_t cap, uint32_t *total, uint64_t *dropped)
+{
+  if (!e) return fail("null argument");
+  if (!e->plan || !e->plan->chtrack) return fail("channel tracking not enabled");
+  const Plan &p = *e->plan;
+  if (stream >= e->prm.n_streams) return fail("stream out of range");
+  if (!out && cap) return fail("null argument");
+  CK(cudaSetDevice(e->prm.device));
+  CK(cudaStreamSynchronize(p.psd_stream ? p.psd_stream.get() : e->stream.get()));
+  CK(cudaStreamSynchronize(e->stream));
+  const long n = sdb_chtrack_read(p.chtrack.get(), stream, e->samp_rate, center_freq, out, cap, total, dropped);
+  if (n < 0) return fail("tracked channel read failed");
+  return n;
+}
+
+extern "C" int sdb_engine_read_all_tracked_channels(sdb_engine_t *e, const double *centers, sdb_tracked_channel *out,
+                                                    size_t cap, uint32_t *counts, uint64_t *dropped)
+{
+  if (!e || !centers || !out || !counts) return fail("null argument");
+  if (!e->plan || !e->plan->chtrack) return fail("channel tracking not enabled");
+  const Plan &p = *e->plan;
+  CK(cudaSetDevice(e->prm.device));
+  CK(cudaStreamSynchronize(p.psd_stream ? p.psd_stream.get() : e->stream.get()));
+  CK(cudaStreamSynchronize(e->stream));
+  if (sdb_chtrack_read_all(p.chtrack.get(), e->samp_rate, centers, out, cap, counts, dropped))
+    return fail("tracked channel read failed");
   return 0;
 }
 
@@ -874,6 +920,11 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
     if (e->cd_enabled) {
       p.chdet.reset(sdb_chdet_new(e->prm.device, Np, S, e->cd_alpha, e->cd_gamma, e->cd_snr, e->cd_min_bins));
       if (!p.chdet) return fail("out of device memory (channel detector)");
+      if (e->ct_enabled) {
+        if (!(e->cd_beta > 0.0f && e->cd_beta <= 1.0f)) return fail("channel tracking needs a detector beta in (0, 1]");
+        p.chtrack.reset(sdb_chtrack_new(e->prm.device, Np, S, e->cd_beta, e->ct_hold));
+        if (!p.chtrack) return fail("out of device memory (channel tracking)");
+      }
     }
   }
   if (K > 0 && !make_plan(p, W, false, &p.fs_st)) return fail("out of device memory");
@@ -1235,6 +1286,13 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     return groups_feed(e, p.avg, lc, p.feed_index & 1u, sl.psd, (unsigned) frames, groups_db) ||
            groups_feed(e, p.peak, lc, p.feed_index & 1u, sl.psd, (unsigned) frames, groups_db);
   };
+  // SPEC KT: the tracking update of this feed, on the detector's stream right after it
+  auto chan_track = [&](cudaStream_t on) -> int {
+    e->span_begin(FAM_CHAN_TRACK, on);
+    CK(sdb_chtrack_feed_stream(p.chtrack.get(), p.chdet.get(), (uint32_t) frames, on, &e->launches));
+    e->span_end(on);
+    return 0;
+  };
   const int H = K ? (int) (n / (W / 2)) : 0;
   const int first = (K && p.first_feed) ? 1 : 0;
   const int wps = K ? H - first : 0;
@@ -1294,6 +1352,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
     }
     if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, p.psd_stream,
                                           &e->launches));
+    if (p.chtrack && chan_track(p.psd_stream)) return -1;
     if (frame_groups(pctx)) return -1;
     CK(sl.psd_ready.record(p.psd_stream));
     CK(sl.psd_ready.wait_on(e->stream));          // the main stream stays the engine's timeline
@@ -1327,6 +1386,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
       }
       if (p.chdet) CK(sdb_chdet_feed_stream(p.chdet.get(), sl.psd, (uint32_t) frames, (size_t) frames * Np, e->stream,
                                             &e->launches));
+      if (p.chtrack && chan_track(e->stream)) return -1;
       if (frame_groups(ctx)) return -1;
       CK(sl.psd_ready.record(e->stream));
     }

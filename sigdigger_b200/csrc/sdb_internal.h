@@ -484,6 +484,16 @@ cudaError_t sdb_chdet_feed_stream(sdb_chdet_t *d, const float *psd_dev, uint32_t
                                   cudaStream_t stream, uint64_t *launch_counter);
 cudaError_t sdb_chdet_pack_device(sdb_chdet_t *d, double samp_rate, const double *centers_dev,
                                   sdb_detected_channel *out_dev, size_t cap, int *counts_dev, cudaStream_t stream);
+// chdet_kernels.cu: channel tracking across detector updates (oracle/SPEC_KT.md), one update after every detector update
+struct sdb_chtrack;
+sdb_chtrack *sdb_chtrack_new(int device, uint32_t n_bins, uint32_t n_streams, float beta, uint32_t hold);
+void sdb_chtrack_destroy(sdb_chtrack *t);
+cudaError_t sdb_chtrack_feed_stream(sdb_chtrack *t, const sdb_chdet_t *d, uint32_t frames, cudaStream_t stream,
+                                    uint64_t *launch_counter);
+long sdb_chtrack_read(sdb_chtrack *t, uint32_t stream, double samp_rate, double center_freq, sdb_tracked_channel *out,
+                      size_t cap, uint32_t *total, uint64_t *dropped);
+int  sdb_chtrack_read_all(sdb_chtrack *t, double samp_rate, const double *centers, sdb_tracked_channel *out, size_t cap,
+                          uint32_t *counts, uint64_t *dropped);
 // stream-ordered pieces of the panoramic sweep (panoramic.cu): caller-owned device buffers, no host copies, no
 // default-stream work.  engine.cu:
 int sdb_engine_pack_channels_device(sdb_engine_t *e, const double *centers_dev, sdb_detected_channel *out_dev, size_t cap,

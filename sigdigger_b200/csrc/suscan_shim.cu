@@ -559,6 +559,10 @@ void *convert(suscan_analyzer *sa, uint32_t type, void *p)
         struct sigutils_channel *c = (struct sigutils_channel *) calloc(1, sizeof(*c));
         const sdb_detected_channel &d = s->channel_list[i];
         c->fc = d.fc; c->f_lo = d.f_lo; c->f_hi = d.f_hi; c->bw = (SUFLOAT) d.bw; c->snr = d.snr; c->S0 = d.S0; c->N0 = d.N0;
+        // channel tracking (SPEC KT) is off unless sdb_analyzer_params.channel_hold_int is set, which
+        // suscan_analyzer_params has no field for; with it on, each track's age and present fill the fields of the
+        // same names
+        if (s->tracked_list) { c->age = s->tracked_list[i].age; c->present = s->tracked_list[i].present; }
         m->channel_list[i] = c;
       }
       sdb_analyzer_dispose_message(type, s);
