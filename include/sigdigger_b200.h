@@ -264,6 +264,29 @@ long sdb_engine_read_spectra(sdb_engine_t *e, int handle, float *out, uint64_t *
 /* values[n_streams][cap], valid[n_streams][cap] of every emission of the last feed; returns the emission count */
 long sdb_engine_read_estimates(sdb_engine_t *e, int handle, int estimator_id, float *values, int32_t *valid, size_t cap);
 
+/* ---- the inspector's FAC tab (Default/GenericInspector/FACTab.cpp; oracle/SPEC_FC.md) ----
+ * The averaged, peak-marked autocorrelation of a psk / fsk / ask inspector's soft symbols, per stream.  Symbols fill
+ * blocks of `size` = 2^9 .. 2^19 (the tab's 65536 by default) across feeds; each completed block gives
+ * v[l] = |autocorrelation| at lag l < size / 2 (unnormalised), and fac[l] += alpha (v[l] / max - fac[l]) with max the
+ * running maximum of v over the lag window [lag_lo, lag_hi) since the channel started (lag_lo = lag_hi = 0: [0, size/2),
+ * the tab's default view).  alpha = 1 - averaging slider / 100.  Per feed, over the blocks it completed: the first
+ * lag of the largest v in the window (peak_lag), sigmas = that v / sqrt(mean v^2 of the window's values that set no
+ * running maximum), and marker = sigmas > sigma (the tab's peak detector; 5 by default).  sigmas and marker are 0
+ * when the feed completed no block, no value counted or the peak is infinite.  An all-zero input gives max = 0 and a
+ * NaN fac, as in the tab.
+ * set_fac: before commit; NULL turns the FAC off.  Device memory: n_streams (8 L + 2 L + slots 4 L, plus slots 8 L
+ * for L >= 8192) bytes per FAC channel, slots = the blocks one feed can complete, (L - 1 + n) / L with n the channel
+ * samples of a max_feed feed.
+ * read_fac: fac[n_streams][size / 2] and st[n_streams] after the latest feed (waits for it); either may be NULL.
+ * _fac_device: the engine's fac of stream 0 of the channel (the streams follow, size / 2 floats apart), or NULL.
+ * Migration keeps a channel's block, fill, max, min and fac when it continues with the same class, size and channel
+ * rate (alpha, the window and sigma may change); anything else restarts as after a resize. */
+typedef struct { uint32_t size; float alpha; uint32_t lag_lo, lag_hi; double sigma; } sdb_fac_params;
+typedef struct { uint32_t blocks, peak_lag; float max, min, sigmas; int32_t marker; } sdb_fac_status;
+int  sdb_engine_set_fac(sdb_engine_t *e, int handle, const sdb_fac_params *p);
+int  sdb_engine_read_fac(sdb_engine_t *e, int handle, float *fac, sdb_fac_status *st);
+const float *sdb_engine_fac_device(const sdb_engine_t *e, int handle);
+
 /* ---- channel detector on the main PSD (SURVEY.md 8(f) rank 3; SPEC.md section K) ----
  * struct suscan_analyzer_params.detector_params.{alpha, beta, gamma, snr} + channel_update_int
  * (Suscan/AnalyzerParams.cpp:27-66) -> SUSCAN_ANALYZER_MESSAGE_TYPE_CHANNEL lists of struct sigutils_channel
@@ -338,7 +361,8 @@ uint64_t sdb_engine_launch_count(const sdb_engine_t *e);
  * "fft_cols"; its "fft_rows_psd" / "fft_rows_chan" stay at zero launches; "psd_average" (the group means) records none
  * while averaging is off, "power" (the power inspectors' integration) none while no channel has a power inspector,
  * "psd_peak" (the group extremes) none while peak detection is off, "spectsrc_sched" (the scheduled spectra: frame
- * gather, transforms and ring update) none in a feed that neither emits nor keeps samples */
+ * gather, transforms and ring update) none in a feed that neither emits nor keeps samples, "fac" (the FAC tab's
+ * launches, sdb_engine_set_fac) none while no channel has the FAC on */
 int      sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches);
 void     sdb_engine_timing(sdb_engine_t *e, int enable);
 /* inspector-kernel stage balance since the last reset: out[0..3] = busy SM cycles of the gain / carrier /
@@ -513,7 +537,8 @@ enum {   /* SUSCAN_ANALYZER_INSPECTOR_MSGKIND_* (Suscan/AnalyzerRequestTracker.c
   SDB_INSPECTOR_MSGKIND_OPEN = 0, SDB_INSPECTOR_MSGKIND_SET_ID, SDB_INSPECTOR_MSGKIND_GET_CONFIG,
   SDB_INSPECTOR_MSGKIND_SET_CONFIG, SDB_INSPECTOR_MSGKIND_ESTIMATOR, SDB_INSPECTOR_MSGKIND_SPECTRUM,
   SDB_INSPECTOR_MSGKIND_CLOSE, SDB_INSPECTOR_MSGKIND_INVALID_CHANNEL, SDB_INSPECTOR_MSGKIND_WRONG_HANDLE,
-  SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, SDB_INSPECTOR_MSGKIND_WRONG_KIND
+  SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, SDB_INSPECTOR_MSGKIND_WRONG_KIND,
+  SDB_INSPECTOR_MSGKIND_FAC          /* this project's: the FAC tab (oracle/SPEC_FC.md); suscan has no such kind */
 };
 enum { SDB_ANALYZER_MODE_CHANNEL = 0, SDB_ANALYZER_MODE_WIDE_SPECTRUM = 1 };
 
@@ -598,6 +623,10 @@ typedef struct {                  /* suscan_analyzer_inspector_msg, fields this 
   uint32_t spectsrc_count, estimator_count;
   uint32_t spectsrc_id; float *spectrum_data; uint64_t spectrum_size; uint64_t samp_rate;
   uint32_t estimator_id; int32_t enabled; float value;
+  /* kind = FAC: the acknowledgement of sdb_analyzer_inspector_set_fac_async (no data), or, after the SAMPLES of every
+   * block that completed at least one FAC block, fac[size / 2] in spectrum_data / spectrum_size and the block's status
+   * here (sdb_engine_read_fac) */
+  sdb_fac_status fac;
 } sdb_analyzer_inspector_msg;
 /* suscan_analyzer_channel_msg (Suscan/Messages/ChannelMessage.cpp:25-70): posted every channel_update_int seconds
  * of signal time when channel_update_int > 0 */
@@ -634,6 +663,10 @@ int    sdb_analyzer_set_inspector_freq_overridable(sdb_analyzer_t *a, int32_t ha
 int    sdb_analyzer_set_inspector_bandwidth_overridable(sdb_analyzer_t *a, int32_t handle, double bw);
 /* suscan_analyzer_inspector_set_spectrum_async / _estimator_cmd_async (Suscan/Analyzer.cpp:539-565) */
 int    sdb_analyzer_inspector_set_spectrum_async(sdb_analyzer_t *a, int32_t handle, uint32_t spectsrc_id, uint32_t req_id);
+/* the FAC tab of a psk / fsk / ask inspector (sdb_engine_set_fac; p NULL = off), from the next block on, through the
+ * re-plan: the FAC state carries over as sdb_engine_migrate says.  Acknowledged by an INSPECTOR message of kind FAC;
+ * WRONG_HANDLE, WRONG_KIND (another class) or WRONG_OBJECT (parameters sdb_engine_set_fac refuses) otherwise. */
+int    sdb_analyzer_inspector_set_fac_async(sdb_analyzer_t *a, int32_t handle, const sdb_fac_params *p, uint32_t req_id);
 int    sdb_analyzer_inspector_estimator_cmd_async(sdb_analyzer_t *a, int32_t handle, uint32_t estimator_id,
                                                   int enabled, uint32_t req_id);
 int    sdb_analyzer_set_params_async(sdb_analyzer_t *a, const sdb_analyzer_params *p, uint32_t req_id);

@@ -49,6 +49,18 @@ class TrackedChannel(C.Structure):
                 ("misses", C.c_uint32)]
 
 
+class FacParams(C.Structure):
+    """sdb_fac_params: the FAC tab of one inspector (oracle/SPEC_FC.md)."""
+    _fields_ = [("size", C.c_uint32), ("alpha", C.c_float), ("lag_lo", C.c_uint32), ("lag_hi", C.c_uint32),
+                ("sigma", C.c_double)]
+
+
+class FacStatus(C.Structure):
+    """sdb_fac_status: the FAC tab's outputs of one stream's latest feed."""
+    _fields_ = [("blocks", C.c_uint32), ("peak_lag", C.c_uint32), ("max", C.c_float), ("min", C.c_float),
+                ("sigmas", C.c_float), ("marker", C.c_int32)]
+
+
 class CaptureInfo(C.Structure):
     """sdb_capture_info"""
     _fields_ = [("container", C.c_int32), ("sample_format", C.c_int32), ("samp_rate", C.c_double),
@@ -302,6 +314,9 @@ _PROTOS = {
     "sdb_estimator_name": (C.c_char_p, [C.c_int]),
     "sdb_engine_set_spectrum_source": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_uint32]),
     "sdb_engine_set_estimator": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
+    "sdb_engine_set_fac": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "sdb_engine_read_fac": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdb_engine_fac_device": (C.c_void_p, [C.c_void_p, C.c_int]),
     "sdb_engine_read_spectrum": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_read_estimate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_set_spectrum_interval": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
@@ -375,6 +390,7 @@ _PROTOS = {
     "sdb_analyzer_set_throttle_async": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint32]),
     "sdb_analyzer_register_baseband_filter": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "sdb_analyzer_inspector_set_spectrum_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32]),
+    "sdb_analyzer_inspector_set_fac_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32]),
     "sdb_analyzer_inspector_estimator_cmd_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_uint32, C.c_int, C.c_uint32]),
     "sdb_analyzer_get_samp_rate": (C.c_uint64, [C.c_void_p]),
     "sdb_analyzer_get_measured_samp_rate": (C.c_float, [C.c_void_p]),
@@ -540,6 +556,7 @@ class Engine:
         if not self._h:
             raise SdbError(last_error())
         self._info = []
+        self._fac_size = {}                 # FAC block size of every channel with the FAC on (set_fac)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -678,6 +695,30 @@ class Engine:
         counts, dropped = (C.c_uint32 * S)(), (C.c_uint64 * S)()
         _check(self._L.sdb_engine_read_all_tracked_channels(self._h, c, out, cap, counts, dropped))
         return [([out[s * cap + i] for i in range(counts[s])], dropped[s]) for s in range(S)]
+
+    # ---- the inspector's FAC tab (oracle/SPEC_FC.md): before commit, after set_inspector
+    def set_fac(self, h, size=65536, alpha=1.0, lags=None, sigma=5.0, enabled=True):
+        """Autocorrelate h's soft symbols in blocks of `size`, averaged with `alpha` (1 - slider / 100), with the peak
+        of the lag window `lags` = (lo, hi) (None: [0, size / 2)) marked above `sigma`; enabled=False turns it off."""
+        if not enabled:
+            _check(self._L.sdb_engine_set_fac(self._h, h, None))
+            self._fac_size.pop(h, None)
+            return
+        lo, hi = lags if lags is not None else (0, 0)
+        p = FacParams(size, alpha, lo, hi, sigma)
+        _check(self._L.sdb_engine_set_fac(self._h, h, C.byref(p)))
+        self._fac_size[h] = size
+
+    def read_fac(self, h):
+        """-> (fac [n_streams, size / 2] float32, list of FacStatus per stream) after the latest feed"""
+        if h not in self._fac_size:
+            _check(self._L.sdb_engine_read_fac(self._h, h, None, None))      # the engine's refusal and its message
+            raise SdbError("the FAC is not enabled on this channel")
+        size = self._fac_size[h]
+        out = np.zeros((self.n_streams, size // 2), np.float32)
+        st = (FacStatus * self.n_streams)()
+        _check(self._L.sdb_engine_read_fac(self._h, h, out.ctypes.data, st))
+        return out, list(st)
 
     # ---- inspector spectrum sources / estimators (SPEC U; Suscan/Analyzer.cpp:539-565)
     def set_spectrum_source(self, h, kind, size=1024):

@@ -6,7 +6,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import INSP, WINDOW, InspectorConfig, SdbError, last_error, load_library
+from . import INSP, WINDOW, FacParams, FacStatus, InspectorConfig, SdbError, last_error, load_library
 
 MSG = {"SOURCE_INFO": 0, "SOURCE_INIT": 1, "CHANNEL": 2, "EOS": 3, "READ_ERROR": 4, "INTERNAL": 5, "SAMPLES": 6,
        "INSPECTOR": 7, "PSD": 8, "PARAMS": 9, "HALT": 0xffffffff, "TIMEOUT": 0xfffffffe}
@@ -14,7 +14,7 @@ MSG_NAME = {v: k for k, v in MSG.items()}
 # sdb_analyzer_params.psd_detector (SPEC PK): which spectrum a PSD message carries
 PSD_DETECTOR = {"default": 0, "pos_peak": 1, "neg_peak": 2}
 KIND = {0: "OPEN", 1: "SET_ID", 2: "GET_CONFIG", 3: "SET_CONFIG", 4: "ESTIMATOR", 5: "SPECTRUM", 6: "CLOSE",
-        7: "INVALID_CHANNEL", 8: "WRONG_HANDLE", 9: "WRONG_OBJECT", 10: "WRONG_KIND"}
+        7: "INVALID_CHANNEL", 8: "WRONG_HANDLE", 9: "WRONG_OBJECT", 10: "WRONG_KIND", 11: "FAC"}
 
 
 class Timeval(C.Structure):
@@ -71,7 +71,7 @@ class InspectorMsg(C.Structure):
                 ("fs", C.c_float), ("equiv_fs", C.c_float), ("bandwidth", C.c_float), ("lo", C.c_float),
                 ("spectsrc_count", C.c_uint32), ("estimator_count", C.c_uint32), ("spectsrc_id", C.c_uint32),
                 ("spectrum_data", C.POINTER(C.c_float)), ("spectrum_size", C.c_uint64), ("samp_rate", C.c_uint64),
-                ("estimator_id", C.c_uint32), ("enabled", C.c_int32), ("value", C.c_float)]
+                ("estimator_id", C.c_uint32), ("enabled", C.c_int32), ("value", C.c_float), ("fac", FacStatus)]
 
 
 class ChannelMsg(C.Structure):
@@ -213,6 +213,15 @@ class Analyzer:
     def set_spectrum_source(self, handle, spectsrc_id, req_id=0):
         self._L.sdb_analyzer_inspector_set_spectrum_async(self._h, handle, spectsrc_id, req_id)
 
+    def set_fac(self, handle, size=65536, alpha=1.0, lags=None, sigma=5.0, enabled=True, req_id=0):
+        """the FAC tab of a psk / fsk / ask inspector (oracle/SPEC_FC.md), from the next block; enabled=False: off"""
+        if not enabled:
+            self._L.sdb_analyzer_inspector_set_fac_async(self._h, handle, None, req_id)
+            return
+        lo, hi = lags if lags is not None else (0, 0)
+        p = FacParams(size, alpha, lo, hi, sigma)
+        self._L.sdb_analyzer_inspector_set_fac_async(self._h, handle, C.byref(p), req_id)
+
     def estimator_cmd(self, handle, estimator_id, enabled=True, req_id=0):
         self._L.sdb_analyzer_inspector_estimator_cmd_async(self._h, handle, estimator_id, int(enabled), req_id)
 
@@ -271,6 +280,10 @@ class Analyzer:
                            samp_rate=m.samp_rate, spectrum=None)
                 if m.spectrum_data and m.spectrum_size:
                     out["spectrum"] = np.ctypeslib.as_array(m.spectrum_data, shape=(m.spectrum_size,)).copy()
+                if out["kind"] == "FAC":
+                    f = m.fac
+                    out["fac"] = dict(blocks=f.blocks, peak_lag=f.peak_lag, max=f.max, min=f.min, sigmas=f.sigmas,
+                                      marker=f.marker)
             elif name == "CHANNEL":
                 from . import DetectedChannel
                 m = C.cast(ptr, C.POINTER(ChannelMsg)).contents

@@ -39,7 +39,7 @@ namespace {
 struct Cmd {
   enum Kind { OPEN, SET_ID, SET_CONFIG, CLOSE, SET_PARAMS, SET_SPECTRUM, ESTIMATOR_CMD, SET_IQ_REVERSE, SET_THROTTLE, SET_WATERMARK,
               SET_FREQ, SET_BANDWIDTH, SEEK, SET_HOP_RANGE, SET_REL_BW, SET_BUFFERING, SET_STRATEGY,
-              SET_PARTITIONING, SET_HISTORY, REPLAY, SET_DC_REMOVE } kind;
+              SET_PARTITIONING, SET_HISTORY, REPLAY, SET_DC_REMOVE, SET_FAC } kind;
   double value2 = 0;
   uint32_t req_id = 0;
   uint32_t aux_id = 0; int enabled = 0;       // spectrum source id / estimator id + enable flag
@@ -52,6 +52,7 @@ struct Cmd {
   int precise = 0;
   sdb_inspector_config cfg{};
   sdb_analyzer_params params{};
+  sdb_fac_params fac{};                       // SET_FAC (enabled: on)
 };
 
 struct Insp {
@@ -71,6 +72,8 @@ struct Insp {
   uint32_t est_mask;
   uint32_t spect_size;    // frame size chosen at rebuild time (0 = too few channel samples per block)
   bool spect_sched;       // emitting on the spectrum_update_int schedule (SPEC US) instead of once per block
+  bool fac_on;            // the FAC tab (SPEC FC) with these parameters
+  sdb_fac_params fac;
 };
 
 // class names in SDB_INSP_* order, as requests and inspector messages carry them
@@ -278,6 +281,7 @@ struct sdb_analyzer {
       i.fs = (float) (in_rate / info.decimation);
       i.bandwidth = (float) (i.channel.f_hi - i.channel.f_lo); i.lo = (float) i.channel.fc;
       sdb_engine_set_inspector(e.get(), h, &i.cfg);
+      if (i.fac_on) sdb_engine_set_fac(e.get(), h, &i.fac);      // (checked when requested; the class cannot change)
       // spectrum source / estimators: the largest frame (<= 4096) a steady-state block can fill (SPEC U.1)
       i.spect_size = 0; i.spect_sched = false;
       if ((i.spectsrc_id || i.est_mask) && params.spectrum_update_int > 0) {
@@ -437,6 +441,7 @@ struct sdb_analyzer {
         case Cmd::SET_CONFIG:
         case Cmd::SET_SPECTRUM:
         case Cmd::ESTIMATOR_CMD:
+        case Cmd::SET_FAC:
         case Cmd::CLOSE: {
           Insp *ip = open_insp(c.handle);
           if (!ip) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_HANDLE, c, nullptr); break; }
@@ -450,6 +455,11 @@ struct sdb_analyzer {
             if (c.enabled) i.est_mask |= 1u << c.aux_id; else i.est_mask &= ~(1u << c.aux_id);
             plan_dirty = true;
             post_inspector(SDB_INSPECTOR_MSGKIND_ESTIMATOR, c, &i);    // acknowledgement: value follows per block
+          } else if (c.kind == Cmd::SET_FAC) {
+            if (c.enabled && i.cls > SDB_INSP_ASK) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_KIND, c, nullptr); break; }
+            if (c.enabled && sdb_fac_check(&c.fac)) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, c, nullptr); break; }
+            i.fac_on = c.enabled != 0; i.fac = c.fac; plan_dirty = true;
+            post_inspector(SDB_INSPECTOR_MSGKIND_FAC, c, &i);         // acknowledgement: data follows per block
           } else if (c.kind == Cmd::SET_ID) {
             i.inspector_id = c.inspector_id; i.has_id = true;
             post_inspector(SDB_INSPECTOR_MSGKIND_SET_ID, c, &i);
@@ -860,6 +870,26 @@ struct sdb_analyzer {
     }
   }
 
+  // kind=FAC inspector messages (SPEC FC): one per block that completed a FAC block, after the block's SAMPLES
+  std::vector<float> fac_buf;
+  void publish_fac()
+  {
+    for (auto &i : insps) {
+      sdb_engine_t *ie = engine_of(i);
+      if (!i.open || !i.fac_on || i.engine_handle < 0 || !ie) continue;
+      sdb_fac_status st;
+      fac_buf.resize(i.fac.size / 2);
+      if (sdb_engine_read_fac(ie, i.engine_handle, fac_buf.data(), &st) || !st.blocks) continue;
+      sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_FAC, i.handle, i.inspector_id,
+                                                    kClassNames[i.cls]);
+      m->spectrum_size = fac_buf.size(); m->samp_rate = (uint64_t) i.fs;
+      m->fs = (float) rate; m->equiv_fs = i.fs; m->fac = st;
+      m->spectrum_data = (float *) malloc(fac_buf.size() * sizeof(float));
+      memcpy(m->spectrum_data, fac_buf.data(), fac_buf.size() * sizeof(float));
+      post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
+    }
+  }
+
   // MESSAGE_TYPE_CHANNEL at channel_update_int cadence of signal time
   void publish_channels()
   {
@@ -918,6 +948,7 @@ struct sdb_analyzer {
     pace();
     publish_psd();
     publish_symbols();
+    publish_fac();
     publish_spectra();
     publish_channels();
     return true;
@@ -1200,6 +1231,14 @@ extern "C" int sdb_analyzer_inspector_set_spectrum_async(sdb_analyzer_t *a, int3
                                                          uint32_t req_id)
 {
   Cmd c; c.kind = Cmd::SET_SPECTRUM; c.req_id = req_id; c.handle = handle; c.aux_id = spectsrc_id;
+  return push_cmd(a, std::move(c));
+}
+extern "C" int sdb_analyzer_inspector_set_fac_async(sdb_analyzer_t *a, int32_t handle, const sdb_fac_params *p,
+                                                    uint32_t req_id)
+{
+  Cmd c; c.kind = Cmd::SET_FAC; c.req_id = req_id; c.handle = handle;
+  c.enabled = p ? 1 : 0;
+  if (p) c.fac = *p;
   return push_cmd(a, std::move(c));
 }
 extern "C" int sdb_analyzer_inspector_estimator_cmd_async(sdb_analyzer_t *a, int32_t handle, uint32_t estimator_id,

@@ -21,6 +21,7 @@
 #include <vector>
 #include <cstdio>
 #include <cstring>
+#include <cmath>
 
 thread_local std::string g_err;
 extern "C" const char *sdb_last_error(void) { return g_err.c_str(); }
@@ -42,14 +43,15 @@ struct Channel {
   sdb_inspector_config cfg;
   int spect_kind = 0; unsigned spect_size = 0, est_mask = 0;   // SPEC U
   uint64_t spect_interval = 0;                                    // SPEC US (0: once per feed, SPEC U.1)
+  bool has_fac = false; sdb_fac_params fac{};                     // SPEC FC
 };
 
 struct TimedSpan { int family; Event a, b; };
 enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_POWER, FAM_PSD_PEAK,
-       FAM_SPECTSCHED, FAM_CHAN_TRACK, FAM_COUNT };
+       FAM_SPECTSCHED, FAM_CHAN_TRACK, FAM_FAC, FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
                                             "inspector", "psd_average", "power", "psd_peak", "spectsrc_sched",
-                                            "chan_track" };
+                                            "chan_track", "fac" };
 
 // SPEC PW: samples per mean of a power inspector (power.integrate-samples, 0 read as 1)
 static uint64_t power_m(const sdb_inspector_config &c) { return c.power_integrate_samples ? c.power_integrate_samples : 1; }
@@ -153,6 +155,14 @@ struct Plan {
   // DC removal (SDB_FLAG_DC_REMOVE, SPEC R): per-stream estimate, the estimate the current block is corrected with,
   // run sums, and the corrected float32 copy of the block the rest of the path reads
   float2 *d_dc_state = nullptr, *d_dc_cur = nullptr, *d_xdc = nullptr; double2 *d_dc_part = nullptr;
+  // the FAC tab (SPEC FC; fac_kernels.cu): one chain per (FAC channel, stream), channel-major, with its running state;
+  // first[k] is channel k's stream-0 chain or -1.  Per feed: its blocks' work areas, tile records and status.
+  struct Fac {
+    std::vector<SdbFacChan> h; std::vector<int> first;
+    DevBuf<SdbFacChan> chans; DevBuf<SdbFacState> state; DevBuf<float2> blk, scr; DevBuf<float> fac, work, slot_max;
+    DevBuf<SdbFacTile> tiles; DevBuf<uint32_t> offs, nb; DevBuf<sdb_fac_status> status;
+    int grid[SDB_FAC_KINDS] = {0, 0, 0, 0};
+  } fac;
   // frame averaging (SPEC A) and peak detection (SPEC PK), in the order they run
   FrameGroups avg{FAM_PSD_AVERAGE, 1}, peak{FAM_PSD_PEAK, 2};
   // running state
@@ -501,6 +511,54 @@ extern "C" int sdb_engine_set_spectrum_source(sdb_engine_t *e, int handle, int s
   if (c.spect_size && c.spect_size != size && c.est_mask) return fail("spectrum size already fixed by an estimator");
   c.spect_kind = spectsrc_id; c.spect_size = size;
   return 0;
+}
+
+int sdb_fac_check(const sdb_fac_params *p)
+{
+  if (!is_pow2(p->size) || p->size < 512 || p->size > (1u << 19)) return fail("FAC size must be a power of two in [512, 2^19]");
+  if (!(p->alpha >= 0.0f && p->alpha <= 1.0f)) return fail("FAC alpha must be in [0, 1]");
+  if ((p->lag_lo || p->lag_hi) && !(p->lag_lo < p->lag_hi && p->lag_hi <= p->size / 2))
+    return fail("FAC lag window must satisfy lag_lo < lag_hi <= size / 2");
+  if (std::isnan(p->sigma)) return fail("FAC sigma must not be NaN");
+  return 0;
+}
+
+extern "C" int sdb_engine_set_fac(sdb_engine_t *e, int handle, const sdb_fac_params *p)
+{
+  if (!e) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (e->plan) return fail("engine already committed");
+  Channel &c = e->channels[handle];
+  if (!p) { c.has_fac = false; return 0; }
+  if (sdb_fac_check(p)) return -1;
+  if (!c.has_insp || c.cfg.insp_class > SDB_INSP_ASK) return fail("the FAC needs a psk, fsk or ask inspector");
+  c.fac = *p; c.has_fac = true;
+  return 0;
+}
+
+extern "C" int sdb_engine_read_fac(sdb_engine_t *e, int handle, float *fac, sdb_fac_status *st)
+{
+  if (!e) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (!e->plan) return fail("engine not committed");
+  const Plan::Fac &f = e->plan->fac;
+  if (f.first.empty() || f.first[handle] < 0) return fail("the FAC is not enabled on this channel");
+  const SdbFacChan &h = f.h[f.first[handle]];
+  const unsigned S = e->prm.n_streams;
+  CK(cudaSetDevice(e->prm.device));
+  CK(e->join());
+  CK(cudaStreamSynchronize(e->stream));
+  if (fac) CK(cudaMemcpy(fac, f.fac.get() + h.fac_off, (size_t) S * (h.L / 2) * sizeof(float), cudaMemcpyDeviceToHost));
+  if (st) CK(cudaMemcpy(st, f.status.get() + f.first[handle], S * sizeof(sdb_fac_status), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+extern "C" const float *sdb_engine_fac_device(const sdb_engine_t *e, int handle)
+{
+  if (!e || !e->plan || handle < 0 || handle >= (int) e->plan->fac.first.size() || e->plan->fac.first[handle] < 0)
+    return nullptr;
+  const Plan::Fac &f = e->plan->fac;
+  return f.fac.get() + f.h[f.first[handle]].fac_off;
 }
 
 extern "C" int sdb_engine_set_estimator(sdb_engine_t *e, int handle, int estimator_id, int enabled)
@@ -881,6 +939,88 @@ static int groups_read(sdb_engine *e, const FrameGroups *g, float *dst0, float *
   return 0;
 }
 
+// SPEC FC: the FAC chains of every channel with the FAC on, their state (empty blocks, max = -inf, min = +inf, fac = 0)
+// and per-feed work areas for the most blocks one feed can complete.  Persistent launches get at most two CTAs per SM.
+static int fac_commit(sdb_engine *e, Plan &p, size_t max_hops)
+{
+  const unsigned S = e->prm.n_streams;
+  const int K = (int) e->channels.size();
+  Plan::Fac &f = p.fac;
+  f.first.assign(K, -1);
+  size_t blk = 0, facn = 0, work = 0, scr = 0;
+  uint32_t slots_total = 0, tiles_total = 0;
+  uint64_t units[SDB_FAC_KINDS] = {0, 0, 0, 0};
+  for (int k = 0; k < K; ++k) {
+    const Channel &c = e->channels[k];
+    if (!c.has_fac) continue;
+    if (!c.has_insp || c.cfg.insp_class > SDB_INSP_ASK) return fail("the FAC needs a psk, fsk or ask inspector");
+    const uint32_t L = c.fac.size;
+    SdbFacChan h{};
+    h.L = L; h.logL = (uint32_t) ilog2u(L);
+    h.lo = c.fac.lag_lo; h.hi = c.fac.lag_hi ? c.fac.lag_hi : L / 2;
+    h.ntiles = (h.hi - h.lo + 1023) / 1024;
+    h.alpha = c.fac.alpha; h.sigma = c.fac.sigma;
+    h.tw = p.twiddle(L);
+    if (L > 4096) {                      // SPEC F.3: N1 = 2^floor(l / 2)
+      h.N1 = 1u << (h.logL / 2); h.N2 = L / h.N1;
+      h.logN1 = (uint32_t) ilog2u(h.N1); h.logN2 = (uint32_t) ilog2u(h.N2);
+      h.twN1 = p.twiddle(h.N1); h.twN2 = p.twiddle(h.N2);
+      if (!h.twN1 || !h.twN2) return fail("out of device memory (FAC)");
+    }
+    if (!h.tw) return fail("out of device memory (FAC)");
+    // a chain emits at most one symbol per channel sample (the bound the symbol rows are sized by): a feed brings at
+    // most max_hops halfsz of them, and completes at most (L - 1 + that) / L blocks
+    const size_t sym_max = max_hops * c.halfsz;
+    const uint32_t slots = (uint32_t) ((L - 1 + sym_max) / L);
+    f.first[k] = (int) f.h.size();
+    for (unsigned s = 0; s < S; ++s) {
+      h.row = s * (uint32_t) K + (uint32_t) k;
+      h.slot_off = slots_total; h.tile_off = tiles_total;
+      h.blk_off = blk; h.fac_off = facn; h.work_off = work; h.scr_off = scr;
+      slots_total += slots; tiles_total += slots * h.ntiles;
+      blk += L; facn += L / 2; work += (size_t) slots * L;
+      if (L > 4096) scr += (size_t) slots * L;
+      units[L <= 4096 ? 0 : 1] += L <= 4096 ? slots : (uint64_t) slots * (L / 4096);
+      units[2] += (uint64_t) slots * h.ntiles;
+      units[3] += (L / 2 + 1023) / 1024;
+      f.h.push_back(h);
+    }
+  }
+  if (f.h.empty()) return 0;
+  const size_t C = f.h.size();
+  if (f.chans.alloc(C) || f.state.alloc(C) || f.blk.alloc(blk) || f.fac.alloc(facn) || f.work.alloc(work) ||
+      (scr && f.scr.alloc(scr)) || f.slot_max.alloc(slots_total) || f.tiles.alloc(tiles_total) ||
+      f.offs.alloc(SDB_FAC_KINDS * (C + 1)) || f.nb.alloc(C) || f.status.alloc(C))
+    return fail("out of device memory (FAC)");
+  CK(cudaMemcpy(f.chans, f.h.data(), C * sizeof(SdbFacChan), cudaMemcpyHostToDevice));
+  const std::vector<SdbFacState> st(C, SdbFacState{ 0u, -INFINITY, INFINITY });
+  CK(cudaMemcpy(f.state, st.data(), C * sizeof(SdbFacState), cudaMemcpyHostToDevice));
+  const std::vector<sdb_fac_status> none(C, sdb_fac_status{ 0u, 0u, -INFINITY, INFINITY, 0.0f, 0 });
+  CK(cudaMemcpy(f.status, none.data(), C * sizeof(sdb_fac_status), cudaMemcpyHostToDevice));
+  CK(cudaMemset(f.fac, 0, facn * sizeof(float)));
+  CK(cudaMemset(f.blk, 0, blk * sizeof(float2)));
+  int sms = 0;
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->prm.device));
+  for (int k = 0; k < SDB_FAC_KINDS; ++k) f.grid[k] = (int) std::min<uint64_t>(units[k], 2 * (uint64_t) sms);
+  return 0;
+}
+
+// SPEC FC for one feed, on the inspector stream after the chains: the blocks the feed's symbols complete
+static int fac_feed(sdb_engine *e, Plan &p, Slot &sl, const SdbLaunchCtx &ictx)
+{
+  Plan::Fac &f = p.fac;
+  if (f.h.empty()) return 0;
+  SdbFacArgs a{};
+  a.chans = f.chans; a.n_chans = (int) f.h.size();
+  a.state = f.state; a.blk = f.blk; a.fac = f.fac; a.work = f.work; a.scr = f.scr; a.slot_max = f.slot_max;
+  a.tiles = f.tiles; a.offs = f.offs; a.nb = f.nb;
+  a.soft = sl.soft; a.counts = sl.counts; a.sym_cap = p.sym_cap; a.status = f.status;
+  e->span_begin(FAM_FAC, ictx.stream);
+  CK(sdb_launch_fac(ictx, a, f.grid));
+  e->span_end(ictx.stream);
+  return 0;
+}
+
 extern "C" int sdb_engine_commit(sdb_engine_t *e)
 {
   if (!e) return fail("null engine");
@@ -1189,6 +1329,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       CK(cudaMemcpy(p.d_power, pw.data(), pw.size() * sizeof(SdbPowerChain), cudaMemcpyHostToDevice));
       CK(cudaMemset(p.power_carry, 0, chains * sizeof(SdbPowerCarry)));
     }
+    if (fac_commit(e, p, max_hops)) return -1;
   }
   if (e->prm.flags & SDB_FLAG_DC_REMOVE) {
     p.d_dc_state = p.dalloc<float2>(S); p.d_dc_cur = p.dalloc<float2>(S);
@@ -1432,11 +1573,13 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
                                       sl.hard, sl.counts, p.sym_cap));
         e->span_end(ictx.stream);
       }
+      if (fac_feed(e, p, sl, ictx)) return -1;
       CK(sl.insp.record(ictx.stream));
     } else {
       std::fill(sl.sched_n.begin(), sl.sched_n.end(), 0u);   // no channel samples: no emission
       CK(sl.sym_read.wait_on(p.insp_stream));
       CK(cudaMemsetAsync(sl.counts, 0, (size_t) S * K * sizeof(uint32_t), p.insp_stream));
+      if (fac_feed(e, p, sl, SdbLaunchCtx{ p.insp_stream.get(), &e->launches })) return -1;   // (a status of no blocks)
       CK(sl.insp.record(p.insp_stream));
     }
     // keep the last half window of every stream as history for the next feed
@@ -1753,6 +1896,17 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
                         from.ring_stride * sizeof(float2), (size_t) hn.ns1 * sizeof(float2), S, cudaMemcpyDeviceToDevice));
         to.sched[qn].t = from.sched[qo].t; to.sched[qn].v = from.sched[qo].v;
       }
+    }
+    // SPEC FC: the FAC goes on while the channel keeps its inspector class, block size and channel rate
+    const int fn = to.fac.first.empty() ? -1 : to.fac.first[kn], fo = from.fac.first.empty() ? -1 : from.fac.first[ko];
+    if (fn >= 0 && fo >= 0 && cn.cfg.insp_class == co.cfg.insp_class && cn.fac.size == co.fac.size &&
+        cn.cfg.fs == co.cfg.fs) {
+      const size_t L = cn.fac.size;
+      CK(cudaMemcpy(to.fac.state.get() + fn, from.fac.state.get() + fo, S * sizeof(SdbFacState), cudaMemcpyDeviceToDevice));
+      CK(cudaMemcpy(to.fac.blk.get() + to.fac.h[fn].blk_off, from.fac.blk.get() + from.fac.h[fo].blk_off,
+                    S * L * sizeof(float2), cudaMemcpyDeviceToDevice));
+      CK(cudaMemcpy(to.fac.fac.get() + to.fac.h[fn].fac_off, from.fac.fac.get() + from.fac.h[fo].fac_off,
+                    S * (L / 2) * sizeof(float), cudaMemcpyDeviceToDevice));
     }
     if (!cn.has_insp || !co.has_insp) continue;
     if (is_power(cn) || is_power(co)) {

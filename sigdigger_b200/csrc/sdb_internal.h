@@ -494,6 +494,33 @@ long sdb_chtrack_read(sdb_chtrack *t, uint32_t stream, double samp_rate, double 
                       size_t cap, uint32_t *total, uint64_t *dropped);
 int  sdb_chtrack_read_all(sdb_chtrack *t, double samp_rate, const double *centers, sdb_tracked_channel *out, size_t cap,
                           uint32_t *counts, uint64_t *dropped);
+// fac_kernels.cu: the FAC tab (oracle/SPEC_FC.md).  One chain per (FAC channel, stream), channel-major.
+#define SDB_FAC_KINDS 4     // work units of a feed: F.2 blocks, F.3 4096-point units, statistics tiles, averaging units
+struct SdbFacChan {
+  uint32_t L, logL, lo, hi, ntiles;   // block size, lag window [lo, hi), its 1024-lag tiles
+  uint32_t N1, N2, logN1, logN2;      // F.3 split (L >= 8192)
+  float alpha; double sigma;
+  uint32_t row;                       // s * K + k: the chain's row of soft / counts
+  uint32_t slot_off, tile_off;        // its first block slot and first tile record; slots * ntiles records
+  size_t blk_off, fac_off;            // carried block [L] (float2), averaged FAC [L / 2]
+  size_t work_off, scr_off;           // per slot: [L] floats of P / v, [L] float2 of F.3 scratch (L >= 8192)
+  const float2 *tw, *twN1, *twN2;     // W_L (F.2, and F.3's inter-pass twiddle), W_N1, W_N2
+};
+struct SdbFacState { uint32_t p; float max, min; };
+struct SdbFacTile { float max, min, pre, pow; uint32_t pos, cnt; };   // pre: the feed's running maximum before it
+struct SdbFacArgs {
+  const SdbFacChan *chans; int n_chans;
+  SdbFacState *state; float2 *blk; float *fac;
+  float *work; float2 *scr; float *slot_max; SdbFacTile *tiles;
+  uint32_t *offs;                     // [SDB_FAC_KINDS][n_chans + 1]: per-chain exclusive prefix sums, totals last
+  uint32_t *nb;                       // blocks each chain completes in this feed
+  const float2 *soft; const uint32_t *counts; size_t sym_cap;
+  sdb_fac_status *status;
+};
+// engine.cu: the parameter checks of sdb_engine_set_fac (0, or -1 with sdb_last_error() set), shared with the analyzer
+int sdb_fac_check(const sdb_fac_params *p);
+// grid[k]: CTAs of the persistent launches over units of kind k (0: no chain has that kind)
+cudaError_t sdb_launch_fac(const SdbLaunchCtx &c, const SdbFacArgs &a, const int grid[SDB_FAC_KINDS]);
 // stream-ordered pieces of the panoramic sweep (panoramic.cu): caller-owned device buffers, no host copies, no
 // default-stream work.  engine.cu:
 int sdb_engine_pack_channels_device(sdb_engine_t *e, const double *centers_dev, sdb_detected_channel *out_dev, size_t cap,
