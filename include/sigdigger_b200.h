@@ -287,6 +287,29 @@ int  sdb_engine_set_fac(sdb_engine_t *e, int handle, const sdb_fac_params *p);
 int  sdb_engine_read_fac(sdb_engine_t *e, int handle, float *fac, sdb_fac_status *st);
 const float *sdb_engine_fac_device(const sdb_engine_t *e, int handle);
 
+/* ---- the inspector's SNR meter (InspectorUI::feed, Default/GenericInspector/InspectorUI.cpp:807-833; Misc/
+ * SNREstimator.cpp; oracle/SPEC_SN.md) ----
+ * Per stream of a psk / fsk / ask inspector: every feed's soft symbols (what SAMPLES carries) are binned into a
+ * decision-space histogram h[bins] (the argument on [-pi, pi] for psk and fsk, the modulus on [0, 1) for ask, where
+ * values at or above 1 are not counted), and every feed that brought at least one symbol runs one gradient step of the
+ * comb fit (SPEC Y.7) with K = 2^bits_per_symbol (0 read as 1) Gaussians of width sigma: sigma -= alpha delta.
+ * SNR = 1 / (K sigma).  When a bin reaches 2^31, every bin is halved.
+ * set_snr: before commit; NULL turns the meter off.  bins 16 .. 1024 (the GUI's 256), sigma and alpha finite and > 0
+ * (the GUI's toggle: sigma 1, alpha 1 / K).  Device memory: n_streams (8 bins + 32) bytes per channel.
+ * reset_snr: between feeds, sets sigma of every stream of the channel from the next feed on; h is kept (the GUI's
+ * reset button).
+ * read_snr: hist[n_streams][bins], model[n_streams][bins] (the fitted comb, normalised to a maximum of 1) and
+ * st[n_streams] after the latest feed (waits for it); any of them may be NULL.
+ * Migration (SPEC SN.4): a channel that keeps its inspector class and bins keeps h, the model, sigma and the step count
+ * when its inspector configuration is unchanged; any other configuration clears h and keeps sigma, which restarts at
+ * 1/8 when bits_per_symbol changed.  Anything else starts afresh.  alpha always comes from the new parameters. */
+typedef struct { uint32_t bins; float sigma, alpha; } sdb_snr_params;
+/* counted = sum of h; steps = gradient steps so far; stepped = 1 when the latest feed ran one; delta = its gradient */
+typedef struct { uint64_t counted; uint32_t steps, stepped; float sigma, snr, delta; } sdb_snr_status;
+int  sdb_engine_set_snr(sdb_engine_t *e, int handle, const sdb_snr_params *p);
+int  sdb_engine_reset_snr(sdb_engine_t *e, int handle, float sigma);
+int  sdb_engine_read_snr(sdb_engine_t *e, int handle, uint32_t *hist, float *model, sdb_snr_status *st);
+
 /* ---- channel detector on the main PSD (SURVEY.md 8(f) rank 3; SPEC.md section K) ----
  * struct suscan_analyzer_params.detector_params.{alpha, beta, gamma, snr} + channel_update_int
  * (Suscan/AnalyzerParams.cpp:27-66) -> SUSCAN_ANALYZER_MESSAGE_TYPE_CHANNEL lists of struct sigutils_channel
@@ -362,7 +385,8 @@ uint64_t sdb_engine_launch_count(const sdb_engine_t *e);
  * while averaging is off, "power" (the power inspectors' integration) none while no channel has a power inspector,
  * "psd_peak" (the group extremes) none while peak detection is off, "spectsrc_sched" (the scheduled spectra: frame
  * gather, transforms and ring update) none in a feed that neither emits nor keeps samples, "fac" (the FAC tab's
- * launches, sdb_engine_set_fac) none while no channel has the FAC on */
+ * launches, sdb_engine_set_fac) none while no channel has the FAC on, "snr" (the SNR meter's k_snr, sdb_engine_set_snr)
+ * none while no channel has the meter on */
 int      sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches);
 void     sdb_engine_timing(sdb_engine_t *e, int enable);
 /* inspector-kernel stage balance since the last reset: out[0..3] = busy SM cycles of the gain / carrier /
@@ -538,7 +562,8 @@ enum {   /* SUSCAN_ANALYZER_INSPECTOR_MSGKIND_* (Suscan/AnalyzerRequestTracker.c
   SDB_INSPECTOR_MSGKIND_SET_CONFIG, SDB_INSPECTOR_MSGKIND_ESTIMATOR, SDB_INSPECTOR_MSGKIND_SPECTRUM,
   SDB_INSPECTOR_MSGKIND_CLOSE, SDB_INSPECTOR_MSGKIND_INVALID_CHANNEL, SDB_INSPECTOR_MSGKIND_WRONG_HANDLE,
   SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, SDB_INSPECTOR_MSGKIND_WRONG_KIND,
-  SDB_INSPECTOR_MSGKIND_FAC          /* this project's: the FAC tab (oracle/SPEC_FC.md); suscan has no such kind */
+  SDB_INSPECTOR_MSGKIND_FAC,         /* this project's: the FAC tab (oracle/SPEC_FC.md); suscan has no such kind */
+  SDB_INSPECTOR_MSGKIND_SNR          /* this project's: the SNR meter (oracle/SPEC_SN.md); suscan has no such kind */
 };
 enum { SDB_ANALYZER_MODE_CHANNEL = 0, SDB_ANALYZER_MODE_WIDE_SPECTRUM = 1 };
 
@@ -627,6 +652,11 @@ typedef struct {                  /* suscan_analyzer_inspector_msg, fields this 
    * block that completed at least one FAC block, fac[size / 2] in spectrum_data / spectrum_size and the block's status
    * here (sdb_engine_read_fac) */
   sdb_fac_status fac;
+  /* kind = SNR: the acknowledgement of sdb_analyzer_inspector_set_snr_async / _reset_snr_async (no data), or, after the
+   * SAMPLES of every block in which the meter stepped, the model[bins] in spectrum_data / spectrum_size, the status here
+   * and h[bins] in snr_histogram (freed with the message) (sdb_engine_read_snr) */
+  sdb_snr_status snr;
+  uint32_t *snr_histogram;
 } sdb_analyzer_inspector_msg;
 /* suscan_analyzer_channel_msg (Suscan/Messages/ChannelMessage.cpp:25-70): posted every channel_update_int seconds
  * of signal time when channel_update_int > 0 */
@@ -667,6 +697,13 @@ int    sdb_analyzer_inspector_set_spectrum_async(sdb_analyzer_t *a, int32_t hand
  * re-plan: the FAC state carries over as sdb_engine_migrate says.  Acknowledged by an INSPECTOR message of kind FAC;
  * WRONG_HANDLE, WRONG_KIND (another class) or WRONG_OBJECT (parameters sdb_engine_set_fac refuses) otherwise. */
 int    sdb_analyzer_inspector_set_fac_async(sdb_analyzer_t *a, int32_t handle, const sdb_fac_params *p, uint32_t req_id);
+/* the SNR meter of a psk / fsk / ask inspector (sdb_engine_set_snr; p NULL = off), from the next block on, through the
+ * re-plan: its state carries over as SPEC SN.4 says.  The meter steps once per block, not once per SAMPLES batch.
+ * reset_snr sets sigma (sdb_engine_reset_snr) at the next block boundary, without a re-plan.  Both are acknowledged
+ * by an INSPECTOR message of kind SNR; WRONG_HANDLE, WRONG_KIND (another class) or WRONG_OBJECT (parameters
+ * sdb_engine_set_snr refuses, or a reset with the meter off or a sigma that is not finite and positive) otherwise. */
+int    sdb_analyzer_inspector_set_snr_async(sdb_analyzer_t *a, int32_t handle, const sdb_snr_params *p, uint32_t req_id);
+int    sdb_analyzer_inspector_reset_snr_async(sdb_analyzer_t *a, int32_t handle, float sigma, uint32_t req_id);
 int    sdb_analyzer_inspector_estimator_cmd_async(sdb_analyzer_t *a, int32_t handle, uint32_t estimator_id,
                                                   int enabled, uint32_t req_id);
 int    sdb_analyzer_set_params_async(sdb_analyzer_t *a, const sdb_analyzer_params *p, uint32_t req_id);

@@ -61,6 +61,17 @@ class FacStatus(C.Structure):
                 ("sigmas", C.c_float), ("marker", C.c_int32)]
 
 
+class SnrParams(C.Structure):
+    """sdb_snr_params: the SNR meter of one inspector (oracle/SPEC_SN.md)."""
+    _fields_ = [("bins", C.c_uint32), ("sigma", C.c_float), ("alpha", C.c_float)]
+
+
+class SnrStatus(C.Structure):
+    """sdb_snr_status: the SNR meter's state after one stream's latest feed."""
+    _fields_ = [("counted", C.c_uint64), ("steps", C.c_uint32), ("stepped", C.c_uint32), ("sigma", C.c_float),
+                ("snr", C.c_float), ("delta", C.c_float)]
+
+
 class CaptureInfo(C.Structure):
     """sdb_capture_info"""
     _fields_ = [("container", C.c_int32), ("sample_format", C.c_int32), ("samp_rate", C.c_double),
@@ -317,6 +328,9 @@ _PROTOS = {
     "sdb_engine_set_fac": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "sdb_engine_read_fac": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_fac_device": (C.c_void_p, [C.c_void_p, C.c_int]),
+    "sdb_engine_set_snr": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "sdb_engine_reset_snr": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
+    "sdb_engine_read_snr": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sdb_engine_read_spectrum": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_read_estimate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_set_spectrum_interval": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
@@ -391,6 +405,8 @@ _PROTOS = {
     "sdb_analyzer_register_baseband_filter": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "sdb_analyzer_inspector_set_spectrum_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32]),
     "sdb_analyzer_inspector_set_fac_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32]),
+    "sdb_analyzer_inspector_set_snr_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32]),
+    "sdb_analyzer_inspector_reset_snr_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.c_uint32]),
     "sdb_analyzer_inspector_estimator_cmd_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_uint32, C.c_int, C.c_uint32]),
     "sdb_analyzer_get_samp_rate": (C.c_uint64, [C.c_void_p]),
     "sdb_analyzer_get_measured_samp_rate": (C.c_float, [C.c_void_p]),
@@ -557,6 +573,8 @@ class Engine:
             raise SdbError(last_error())
         self._info = []
         self._fac_size = {}                 # FAC block size of every channel with the FAC on (set_fac)
+        self._snr_bins = {}                 # histogram bins of every channel with the SNR meter on (set_snr)
+        self._bps = {}                      # bits_per_symbol of every channel's inspector (set_inspector)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -586,6 +604,7 @@ class Engine:
                 raise KeyError(k)
             setattr(cfg, k, v)
         _check(self._L.sdb_engine_set_inspector(self._h, h, C.byref(cfg)))
+        self._bps[h] = cfg.bits_per_symbol
 
     def commit(self):
         _check(self._L.sdb_engine_commit(self._h))
@@ -719,6 +738,36 @@ class Engine:
         st = (FacStatus * self.n_streams)()
         _check(self._L.sdb_engine_read_fac(self._h, h, out.ctypes.data, st))
         return out, list(st)
+
+    # ---- the inspector's SNR meter (oracle/SPEC_SN.md): before commit, after set_inspector
+    def set_snr(self, h, bins=256, sigma=1.0, alpha=None, enabled=True):
+        """Bin h's soft symbols into a `bins`-bin decision-space histogram and fit the comb model to it once per feed,
+        starting from `sigma`, with step `alpha` (None: 1 / 2^bits_per_symbol, the GUI's toggle); enabled=False: off"""
+        if not enabled:
+            _check(self._L.sdb_engine_set_snr(self._h, h, None))
+            self._snr_bins.pop(h, None)
+            return
+        if alpha is None:
+            alpha = 1.0 / (1 << (self._bps.get(h, 1) or 1))
+        p = SnrParams(bins, sigma, alpha)
+        _check(self._L.sdb_engine_set_snr(self._h, h, C.byref(p)))
+        self._snr_bins[h] = bins
+
+    def reset_snr(self, h, sigma=1.0):
+        """sigma of every stream from the next feed on; the histogram is kept"""
+        _check(self._L.sdb_engine_reset_snr(self._h, h, sigma))
+
+    def read_snr(self, h):
+        """-> (hist [n_streams, bins] uint32, model [n_streams, bins] float32, list of SnrStatus per stream)"""
+        if h not in self._snr_bins:
+            _check(self._L.sdb_engine_read_snr(self._h, h, None, None, None))   # the engine's refusal and its message
+            raise SdbError("the SNR meter is not on for this channel")
+        L = self._snr_bins[h]
+        hist = np.zeros((self.n_streams, L), np.uint32)
+        model = np.zeros((self.n_streams, L), np.float32)
+        st = (SnrStatus * self.n_streams)()
+        _check(self._L.sdb_engine_read_snr(self._h, h, hist.ctypes.data, model.ctypes.data, st))
+        return hist, model, list(st)
 
     # ---- inspector spectrum sources / estimators (SPEC U; Suscan/Analyzer.cpp:539-565)
     def set_spectrum_source(self, h, kind, size=1024):

@@ -6,7 +6,8 @@ import ctypes as C
 
 import numpy as np
 
-from . import INSP, WINDOW, FacParams, FacStatus, InspectorConfig, SdbError, last_error, load_library
+from . import (INSP, WINDOW, FacParams, FacStatus, InspectorConfig, SdbError, SnrParams, SnrStatus, last_error,
+               load_library)
 
 MSG = {"SOURCE_INFO": 0, "SOURCE_INIT": 1, "CHANNEL": 2, "EOS": 3, "READ_ERROR": 4, "INTERNAL": 5, "SAMPLES": 6,
        "INSPECTOR": 7, "PSD": 8, "PARAMS": 9, "HALT": 0xffffffff, "TIMEOUT": 0xfffffffe}
@@ -14,7 +15,8 @@ MSG_NAME = {v: k for k, v in MSG.items()}
 # sdb_analyzer_params.psd_detector (SPEC PK): which spectrum a PSD message carries
 PSD_DETECTOR = {"default": 0, "pos_peak": 1, "neg_peak": 2}
 KIND = {0: "OPEN", 1: "SET_ID", 2: "GET_CONFIG", 3: "SET_CONFIG", 4: "ESTIMATOR", 5: "SPECTRUM", 6: "CLOSE",
-        7: "INVALID_CHANNEL", 8: "WRONG_HANDLE", 9: "WRONG_OBJECT", 10: "WRONG_KIND", 11: "FAC"}
+        7: "INVALID_CHANNEL", 8: "WRONG_HANDLE", 9: "WRONG_OBJECT", 10: "WRONG_KIND", 11: "FAC",
+        12: "SNR"}
 
 
 class Timeval(C.Structure):
@@ -71,7 +73,8 @@ class InspectorMsg(C.Structure):
                 ("fs", C.c_float), ("equiv_fs", C.c_float), ("bandwidth", C.c_float), ("lo", C.c_float),
                 ("spectsrc_count", C.c_uint32), ("estimator_count", C.c_uint32), ("spectsrc_id", C.c_uint32),
                 ("spectrum_data", C.POINTER(C.c_float)), ("spectrum_size", C.c_uint64), ("samp_rate", C.c_uint64),
-                ("estimator_id", C.c_uint32), ("enabled", C.c_int32), ("value", C.c_float), ("fac", FacStatus)]
+                ("estimator_id", C.c_uint32), ("enabled", C.c_int32), ("value", C.c_float), ("fac", FacStatus),
+                ("snr", SnrStatus), ("snr_histogram", C.POINTER(C.c_uint32))]
 
 
 class ChannelMsg(C.Structure):
@@ -222,6 +225,19 @@ class Analyzer:
         p = FacParams(size, alpha, lo, hi, sigma)
         self._L.sdb_analyzer_inspector_set_fac_async(self._h, handle, C.byref(p), req_id)
 
+    def set_snr(self, handle, alpha, bins=256, sigma=1.0, enabled=True, req_id=0):
+        """the SNR meter of a psk / fsk / ask inspector (oracle/SPEC_SN.md), from the next block; enabled=False: off.
+        The GUI's toggle uses sigma = 1 and alpha = 1 / 2^bits_per_symbol of the inspector."""
+        if not enabled:
+            self._L.sdb_analyzer_inspector_set_snr_async(self._h, handle, None, req_id)
+            return
+        p = SnrParams(bins, sigma, alpha)
+        self._L.sdb_analyzer_inspector_set_snr_async(self._h, handle, C.byref(p), req_id)
+
+    def reset_snr(self, handle, sigma=1.0, req_id=0):
+        """the meter's sigma from the next block on; the histogram is kept"""
+        self._L.sdb_analyzer_inspector_reset_snr_async(self._h, handle, sigma, req_id)
+
     def estimator_cmd(self, handle, estimator_id, enabled=True, req_id=0):
         self._L.sdb_analyzer_inspector_estimator_cmd_async(self._h, handle, estimator_id, int(enabled), req_id)
 
@@ -284,6 +300,13 @@ class Analyzer:
                     f = m.fac
                     out["fac"] = dict(blocks=f.blocks, peak_lag=f.peak_lag, max=f.max, min=f.min, sigmas=f.sigmas,
                                       marker=f.marker)
+                if out["kind"] == "SNR":
+                    q = m.snr
+                    out["snr"] = dict(counted=q.counted, steps=q.steps, stepped=q.stepped, sigma=q.sigma, snr=q.snr,
+                                      delta=q.delta)
+                    out["histogram"] = None
+                    if m.snr_histogram and m.spectrum_size:
+                        out["histogram"] = np.ctypeslib.as_array(m.snr_histogram, shape=(m.spectrum_size,)).copy()
             elif name == "CHANNEL":
                 from . import DetectedChannel
                 m = C.cast(ptr, C.POINTER(ChannelMsg)).contents

@@ -39,7 +39,7 @@ namespace {
 struct Cmd {
   enum Kind { OPEN, SET_ID, SET_CONFIG, CLOSE, SET_PARAMS, SET_SPECTRUM, ESTIMATOR_CMD, SET_IQ_REVERSE, SET_THROTTLE, SET_WATERMARK,
               SET_FREQ, SET_BANDWIDTH, SEEK, SET_HOP_RANGE, SET_REL_BW, SET_BUFFERING, SET_STRATEGY,
-              SET_PARTITIONING, SET_HISTORY, REPLAY, SET_DC_REMOVE, SET_FAC } kind;
+              SET_PARTITIONING, SET_HISTORY, REPLAY, SET_DC_REMOVE, SET_FAC, SET_SNR, RESET_SNR } kind;
   double value2 = 0;
   uint32_t req_id = 0;
   uint32_t aux_id = 0; int enabled = 0;       // spectrum source id / estimator id + enable flag
@@ -53,6 +53,7 @@ struct Cmd {
   sdb_inspector_config cfg{};
   sdb_analyzer_params params{};
   sdb_fac_params fac{};                       // SET_FAC (enabled: on)
+  sdb_snr_params snr{};                       // SET_SNR (enabled: on); RESET_SNR: sigma
 };
 
 struct Insp {
@@ -74,6 +75,10 @@ struct Insp {
   bool spect_sched;       // emitting on the spectrum_update_int schedule (SPEC US) instead of once per block
   bool fac_on;            // the FAC tab (SPEC FC) with these parameters
   sdb_fac_params fac;
+  bool snr_on;            // the SNR meter (SPEC SN) with these parameters
+  sdb_snr_params snr;
+  bool snr_reset;         // a reset to snr_reset_sigma waits for the next block boundary
+  float snr_reset_sigma;
 };
 
 // class names in SDB_INSP_* order, as requests and inspector messages carry them
@@ -282,6 +287,7 @@ struct sdb_analyzer {
       i.bandwidth = (float) (i.channel.f_hi - i.channel.f_lo); i.lo = (float) i.channel.fc;
       sdb_engine_set_inspector(e.get(), h, &i.cfg);
       if (i.fac_on) sdb_engine_set_fac(e.get(), h, &i.fac);      // (checked when requested; the class cannot change)
+      if (i.snr_on) sdb_engine_set_snr(e.get(), h, &i.snr);      // (likewise)
       // spectrum source / estimators: the largest frame (<= 4096) a steady-state block can fill (SPEC U.1)
       i.spect_size = 0; i.spect_sched = false;
       if ((i.spectsrc_id || i.est_mask) && params.spectrum_update_int > 0) {
@@ -442,6 +448,8 @@ struct sdb_analyzer {
         case Cmd::SET_SPECTRUM:
         case Cmd::ESTIMATOR_CMD:
         case Cmd::SET_FAC:
+        case Cmd::SET_SNR:
+        case Cmd::RESET_SNR:
         case Cmd::CLOSE: {
           Insp *ip = open_insp(c.handle);
           if (!ip) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_HANDLE, c, nullptr); break; }
@@ -460,6 +468,17 @@ struct sdb_analyzer {
             if (c.enabled && sdb_fac_check(&c.fac)) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, c, nullptr); break; }
             i.fac_on = c.enabled != 0; i.fac = c.fac; plan_dirty = true;
             post_inspector(SDB_INSPECTOR_MSGKIND_FAC, c, &i);         // acknowledgement: data follows per block
+          } else if (c.kind == Cmd::SET_SNR) {
+            if (c.enabled && i.cls > SDB_INSP_ASK) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_KIND, c, nullptr); break; }
+            if (c.enabled && sdb_snr_check(&c.snr)) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, c, nullptr); break; }
+            i.snr_on = c.enabled != 0; i.snr = c.snr; i.snr_reset = false; plan_dirty = true;
+            post_inspector(SDB_INSPECTOR_MSGKIND_SNR, c, &i);         // acknowledgement: data follows per block
+          } else if (c.kind == Cmd::RESET_SNR) {
+            if (!i.snr_on || !(std::isfinite(c.snr.sigma) && c.snr.sigma > 0.0f)) {
+              post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, c, nullptr); break;
+            }
+            i.snr_reset = true; i.snr_reset_sigma = c.snr.sigma;      // no re-plan: applied before the next block
+            post_inspector(SDB_INSPECTOR_MSGKIND_SNR, c, &i);
           } else if (c.kind == Cmd::SET_ID) {
             i.inspector_id = c.inspector_id; i.has_id = true;
             post_inspector(SDB_INSPECTOR_MSGKIND_SET_ID, c, &i);
@@ -890,6 +909,40 @@ struct sdb_analyzer {
     }
   }
 
+  // SPEC SN.3: the resets requested since the last block, on the engines that run the next one
+  void apply_snr_resets()
+  {
+    for (auto &i : insps) {
+      if (!i.snr_reset) continue;
+      i.snr_reset = false;
+      sdb_engine_t *ie = engine_of(i);
+      if (i.open && i.snr_on && i.engine_handle >= 0 && ie) sdb_engine_reset_snr(ie, i.engine_handle, i.snr_reset_sigma);
+    }
+  }
+
+  // kind=SNR inspector messages (SPEC SN): one per block in which the meter stepped, after the block's SAMPLES
+  std::vector<float> snr_model;
+  std::vector<uint32_t> snr_hist;
+  void publish_snr()
+  {
+    for (auto &i : insps) {
+      sdb_engine_t *ie = engine_of(i);
+      if (!i.open || !i.snr_on || i.engine_handle < 0 || !ie) continue;
+      sdb_snr_status st;
+      snr_model.resize(i.snr.bins); snr_hist.resize(i.snr.bins);
+      if (sdb_engine_read_snr(ie, i.engine_handle, snr_hist.data(), snr_model.data(), &st) || !st.stepped) continue;
+      sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_SNR, i.handle, i.inspector_id,
+                                                    kClassNames[i.cls]);
+      m->spectrum_size = snr_model.size(); m->samp_rate = (uint64_t) i.fs;
+      m->fs = (float) rate; m->equiv_fs = i.fs; m->snr = st;
+      m->spectrum_data = (float *) malloc(snr_model.size() * sizeof(float));
+      memcpy(m->spectrum_data, snr_model.data(), snr_model.size() * sizeof(float));
+      m->snr_histogram = (uint32_t *) malloc(snr_hist.size() * sizeof(uint32_t));
+      memcpy(m->snr_histogram, snr_hist.data(), snr_hist.size() * sizeof(uint32_t));
+      post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
+    }
+  }
+
   // MESSAGE_TYPE_CHANNEL at channel_update_int cadence of signal time
   void publish_channels()
   {
@@ -943,12 +996,14 @@ struct sdb_analyzer {
       if (!dec) return init_failure();
     }
     if (plan_dirty && !rebuild()) return init_failure();
+    apply_snr_resets();
     bool on_device = false;                      // the decimated block is only in the decimator's device output
     if (!read_block(on_device) || !run_filters(on_device) || !feed(on_device)) return false;
     pace();
     publish_psd();
     publish_symbols();
     publish_fac();
+    publish_snr();
     publish_spectra();
     publish_channels();
     return true;
@@ -1054,7 +1109,8 @@ extern "C" void sdb_analyzer_dispose_message(uint32_t type, void *ptr)
       free(((sdb_analyzer_sample_batch_msg *) ptr)->symbols); break;
     case SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR:
       free(((sdb_analyzer_inspector_msg *) ptr)->class_name);
-      free(((sdb_analyzer_inspector_msg *) ptr)->spectrum_data); break;
+      free(((sdb_analyzer_inspector_msg *) ptr)->spectrum_data);
+      free(((sdb_analyzer_inspector_msg *) ptr)->snr_histogram); break;
     case SDB_ANALYZER_MESSAGE_TYPE_CHANNEL:
       free(((sdb_analyzer_channel_msg *) ptr)->channel_list);
       free(((sdb_analyzer_channel_msg *) ptr)->tracked_list); break;
@@ -1239,6 +1295,19 @@ extern "C" int sdb_analyzer_inspector_set_fac_async(sdb_analyzer_t *a, int32_t h
   Cmd c; c.kind = Cmd::SET_FAC; c.req_id = req_id; c.handle = handle;
   c.enabled = p ? 1 : 0;
   if (p) c.fac = *p;
+  return push_cmd(a, std::move(c));
+}
+extern "C" int sdb_analyzer_inspector_set_snr_async(sdb_analyzer_t *a, int32_t handle, const sdb_snr_params *p,
+                                                    uint32_t req_id)
+{
+  Cmd c; c.kind = Cmd::SET_SNR; c.req_id = req_id; c.handle = handle;
+  c.enabled = p ? 1 : 0;
+  if (p) c.snr = *p;
+  return push_cmd(a, std::move(c));
+}
+extern "C" int sdb_analyzer_inspector_reset_snr_async(sdb_analyzer_t *a, int32_t handle, float sigma, uint32_t req_id)
+{
+  Cmd c; c.kind = Cmd::RESET_SNR; c.req_id = req_id; c.handle = handle; c.snr.sigma = sigma;
   return push_cmd(a, std::move(c));
 }
 extern "C" int sdb_analyzer_inspector_estimator_cmd_async(sdb_analyzer_t *a, int32_t handle, uint32_t estimator_id,

@@ -21,6 +21,7 @@
 #include <vector>
 #include <cstdio>
 #include <cstring>
+#include <cstddef>
 #include <cmath>
 
 thread_local std::string g_err;
@@ -44,14 +45,16 @@ struct Channel {
   int spect_kind = 0; unsigned spect_size = 0, est_mask = 0;   // SPEC U
   uint64_t spect_interval = 0;                                    // SPEC US (0: once per feed, SPEC U.1)
   bool has_fac = false; sdb_fac_params fac{};                     // SPEC FC
+  bool has_snr = false; sdb_snr_params snr{};                     // SPEC SN
 };
 
 struct TimedSpan { int family; Event a, b; };
 enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_POWER, FAM_PSD_PEAK,
-       FAM_SPECTSCHED, FAM_CHAN_TRACK, FAM_FAC, FAM_COUNT };
+       FAM_SPECTSCHED, FAM_CHAN_TRACK, FAM_FAC, FAM_SNR,
+       FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
                                             "inspector", "psd_average", "power", "psd_peak", "spectsrc_sched",
-                                            "chan_track", "fac" };
+                                            "chan_track", "fac", "snr" };
 
 // SPEC PW: samples per mean of a power inspector (power.integrate-samples, 0 read as 1)
 static uint64_t power_m(const sdb_inspector_config &c) { return c.power_integrate_samples ? c.power_integrate_samples : 1; }
@@ -163,6 +166,12 @@ struct Plan {
     DevBuf<SdbFacTile> tiles; DevBuf<uint32_t> offs, nb; DevBuf<sdb_fac_status> status;
     int grid[SDB_FAC_KINDS] = {0, 0, 0, 0};
   } fac;
+  // the SNR meter (SPEC SN; snr_kernels.cu): one descriptor per channel with the meter on, first[k] its index or -1;
+  // per (channel, stream) chain, channel-major: h and the model [L] each, and the state / status of the latest feed
+  struct Snr {
+    std::vector<SdbSnrChan> h; std::vector<int> first; uint32_t max_L = 0;
+    DevBuf<SdbSnrChan> chans; DevBuf<uint32_t> hist; DevBuf<float> model; DevBuf<sdb_snr_status> status;
+  } snr;
   // frame averaging (SPEC A) and peak detection (SPEC PK), in the order they run
   FrameGroups avg{FAM_PSD_AVERAGE, 1}, peak{FAM_PSD_PEAK, 2};
   // running state
@@ -559,6 +568,72 @@ extern "C" const float *sdb_engine_fac_device(const sdb_engine_t *e, int handle)
     return nullptr;
   const Plan::Fac &f = e->plan->fac;
   return f.fac.get() + f.h[f.first[handle]].fac_off;
+}
+
+// SPEC SN: the meter's parameters
+int sdb_snr_check(const sdb_snr_params *p)
+{
+  if (p->bins < SDB_SNR_BINS_MIN || p->bins > SDB_SNR_BINS_MAX) return fail("SNR bins must be in [16, 1024]");
+  if (!(std::isfinite(p->sigma) && p->sigma > 0.0f)) return fail("SNR sigma must be finite and positive");
+  if (!(std::isfinite(p->alpha) && p->alpha > 0.0f)) return fail("SNR alpha must be finite and positive");
+  return 0;
+}
+
+// SN.2: K = 2^bps with bps 0 read as 1 (InspectorUI::getBps)
+static uint32_t snr_K(const sdb_inspector_config &c) { return 1u << (c.bits_per_symbol ? c.bits_per_symbol : 1u); }
+
+extern "C" int sdb_engine_set_snr(sdb_engine_t *e, int handle, const sdb_snr_params *p)
+{
+  if (!e) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (e->plan) return fail("engine already committed");
+  Channel &c = e->channels[handle];
+  if (!p) { c.has_snr = false; return 0; }
+  if (sdb_snr_check(p)) return -1;
+  if (!c.has_insp || c.cfg.insp_class > SDB_INSP_ASK) return fail("the SNR meter needs a psk, fsk or ask inspector");
+  c.snr = *p; c.has_snr = true;
+  return 0;
+}
+
+// SN.3: the state of the latest feed is the status; a reset writes sigma of every stream, in order with the feeds
+extern "C" int sdb_engine_reset_snr(sdb_engine_t *e, int handle, float sigma)
+{
+  if (!e) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (!e->plan) return fail("engine not committed");
+  const Plan::Snr &q = e->plan->snr;
+  if (q.first.empty() || q.first[handle] < 0) return fail("the SNR meter is not on for this channel");
+  if (!(std::isfinite(sigma) && sigma > 0.0f)) return fail("SNR sigma must be finite and positive");
+  const unsigned S = e->prm.n_streams;
+  std::vector<sdb_snr_status> st(S);
+  sdb_snr_status *d = q.status.get() + q.h[q.first[handle]].chain0;
+  CK(cudaSetDevice(e->prm.device));
+  CK(e->join());
+  CK(cudaStreamSynchronize(e->stream));
+  CK(cudaMemcpy(st.data(), d, S * sizeof(sdb_snr_status), cudaMemcpyDeviceToHost));
+  const uint32_t K = q.h[q.first[handle]].K;
+  for (auto &x : st) { x.sigma = sigma; x.snr = 1.0f / (K * sigma); }
+  CK(cudaMemcpy(d, st.data(), S * sizeof(sdb_snr_status), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+extern "C" int sdb_engine_read_snr(sdb_engine_t *e, int handle, uint32_t *hist, float *model, sdb_snr_status *st)
+{
+  if (!e) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (!e->plan) return fail("engine not committed");
+  const Plan::Snr &q = e->plan->snr;
+  if (q.first.empty() || q.first[handle] < 0) return fail("the SNR meter is not on for this channel");
+  const SdbSnrChan &h = q.h[q.first[handle]];
+  const size_t n = (size_t) e->prm.n_streams * h.L;
+  CK(cudaSetDevice(e->prm.device));
+  CK(e->join());
+  CK(cudaStreamSynchronize(e->stream));
+  if (hist) CK(cudaMemcpy(hist, q.hist.get() + h.hist_off, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  if (model) CK(cudaMemcpy(model, q.model.get() + h.hist_off, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (st) CK(cudaMemcpy(st, q.status.get() + h.chain0, e->prm.n_streams * sizeof(sdb_snr_status),
+                        cudaMemcpyDeviceToHost));
+  return 0;
 }
 
 extern "C" int sdb_engine_set_estimator(sdb_engine_t *e, int handle, int estimator_id, int enabled)
@@ -1021,6 +1096,57 @@ static int fac_feed(sdb_engine *e, Plan &p, Slot &sl, const SdbLaunchCtx &ictx)
   return 0;
 }
 
+// SPEC SN.3: every channel with the meter on starts with an empty h, a zero model and sigma from its parameters
+static int snr_commit(sdb_engine *e, Plan &p)
+{
+  const unsigned S = e->prm.n_streams;
+  const int K = (int) e->channels.size();
+  Plan::Snr &q = p.snr;
+  q.first.assign(K, -1);
+  size_t bins = 0;
+  std::vector<sdb_snr_status> st;
+  for (int k = 0; k < K; ++k) {
+    const Channel &c = e->channels[k];
+    if (!c.has_snr) continue;
+    if (!c.has_insp || c.cfg.insp_class > SDB_INSP_ASK) return fail("the SNR meter needs a psk, fsk or ask inspector");
+    SdbSnrChan h{};
+    h.L = c.snr.bins; h.K = snr_K(c.cfg); h.k = (uint32_t) k; h.chain0 = (uint32_t) st.size();
+    h.mode = c.cfg.insp_class == SDB_INSP_ASK ? 1 : 0;
+    if (h.mode) { h.dmin = 0.0f; h.dh = 1.0f - 0.0f; }          // SPEC D, as build_chain_cfg sets the decider
+    else { h.dmin = -3.14159265358979323846f; h.dh = 3.14159265358979323846f - (-3.14159265358979323846f); }
+    h.alpha = c.snr.alpha; h.hist_off = bins;
+    bins += (size_t) S * h.L;
+    q.max_L = std::max(q.max_L, h.L);
+    q.first[k] = (int) q.h.size();
+    q.h.push_back(h);
+    st.insert(st.end(), S, sdb_snr_status{ 0ull, 0u, 0u, c.snr.sigma, 1.0f / (h.K * c.snr.sigma), 0.0f });
+  }
+  if (q.h.empty()) return 0;
+  if (q.chans.alloc(q.h.size()) || q.hist.alloc(bins) || q.model.alloc(bins) || q.status.alloc(st.size()))
+    return fail("out of device memory (SNR meter)");
+  CK(cudaMemcpy(q.chans, q.h.data(), q.h.size() * sizeof(SdbSnrChan), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(q.status, st.data(), st.size() * sizeof(sdb_snr_status), cudaMemcpyHostToDevice));
+  CK(cudaMemset(q.hist, 0, bins * sizeof(uint32_t)));
+  CK(cudaMemset(q.model, 0, bins * sizeof(float)));
+  return 0;
+}
+
+// SPEC SN.2 for one feed, on the inspector stream after the chains (and the power and FAC launches)
+static int snr_feed(sdb_engine *e, Plan &p, Slot &sl, const SdbLaunchCtx &ictx)
+{
+  Plan::Snr &q = p.snr;
+  if (q.h.empty()) return 0;
+  SdbSnrArgs a{};
+  a.chans = q.chans; a.n_chans = (int) q.h.size(); a.n_streams = (int) e->prm.n_streams;
+  a.n_channels = (int) e->channels.size(); a.max_L = q.max_L;
+  a.soft = sl.soft; a.counts = sl.counts; a.sym_cap = p.sym_cap;
+  a.hist = q.hist; a.model = q.model; a.status = q.status;
+  e->span_begin(FAM_SNR, ictx.stream);
+  CK(sdb_launch_snr(ictx, a));
+  e->span_end(ictx.stream);
+  return 0;
+}
+
 extern "C" int sdb_engine_commit(sdb_engine_t *e)
 {
   if (!e) return fail("null engine");
@@ -1330,6 +1456,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
       CK(cudaMemset(p.power_carry, 0, chains * sizeof(SdbPowerCarry)));
     }
     if (fac_commit(e, p, max_hops)) return -1;
+    if (snr_commit(e, p)) return -1;
   }
   if (e->prm.flags & SDB_FLAG_DC_REMOVE) {
     p.d_dc_state = p.dalloc<float2>(S); p.d_dc_cur = p.dalloc<float2>(S);
@@ -1574,12 +1701,14 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
         e->span_end(ictx.stream);
       }
       if (fac_feed(e, p, sl, ictx)) return -1;
+      if (snr_feed(e, p, sl, ictx)) return -1;
       CK(sl.insp.record(ictx.stream));
     } else {
       std::fill(sl.sched_n.begin(), sl.sched_n.end(), 0u);   // no channel samples: no emission
       CK(sl.sym_read.wait_on(p.insp_stream));
       CK(cudaMemsetAsync(sl.counts, 0, (size_t) S * K * sizeof(uint32_t), p.insp_stream));
       if (fac_feed(e, p, sl, SdbLaunchCtx{ p.insp_stream.get(), &e->launches })) return -1;   // (a status of no blocks)
+      if (snr_feed(e, p, sl, SdbLaunchCtx{ p.insp_stream.get(), &e->launches })) return -1;   // (a status of no step)
       CK(sl.insp.record(p.insp_stream));
     }
     // keep the last half window of every stream as history for the next feed
@@ -1854,6 +1983,42 @@ extern "C" int sdb_engine_kernel_time(sdb_engine_t *e, const char *family, doubl
 // ---- tail and LO phase; if its inspector class and the sizes of its state lines are unchanged it also keeps the
 // ---- loop state of every chain (AGC, Costas / PLL, matched-filter line, Gardner, CMA...), whatever else of its
 // ---- configuration changed (loop bandwidths, gains, thresholds take effect at this block boundary).
+// SPEC SN.4: a channel that keeps its inspector class and L keeps h, the model and the state while its inspector
+// configuration is unchanged field by field; otherwise h is cleared (the new plan's h is empty) and sigma kept, and it
+// restarts at 1/8 when bps changed.  alpha is the new descriptor's.  Anything else keeps the new plan's fresh start.
+static bool same_inspector_config(const sdb_inspector_config &a, const sdb_inspector_config &b)
+{
+  return !memcmp(&a, &b, offsetof(sdb_inspector_config, eq_locked) + sizeof a.eq_locked) &&
+         a.power_integrate_samples == b.power_integrate_samples;
+}
+
+static int snr_migrate(Plan &to, const Plan &from, const Channel &cn, const Channel &co, int kn, int ko, unsigned S)
+{
+  const int qn = to.snr.first.empty() ? -1 : to.snr.first[kn], qo = from.snr.first.empty() ? -1 : from.snr.first[ko];
+  if (qn < 0 || qo < 0 || cn.cfg.insp_class != co.cfg.insp_class || cn.snr.bins != co.snr.bins) return 0;
+  const SdbSnrChan &hn = to.snr.h[qn], &ho = from.snr.h[qo];
+  std::vector<sdb_snr_status> st(S);
+  CK(cudaMemcpy(st.data(), from.snr.status.get() + ho.chain0, S * sizeof(sdb_snr_status), cudaMemcpyDeviceToHost));
+  if (same_inspector_config(cn.cfg, co.cfg)) {
+    const size_t n = (size_t) S * hn.L;
+    CK(cudaMemcpy(to.snr.hist.get() + hn.hist_off, from.snr.hist.get() + ho.hist_off, n * sizeof(uint32_t),
+                  cudaMemcpyDeviceToDevice));
+    CK(cudaMemcpy(to.snr.model.get() + hn.hist_off, from.snr.model.get() + ho.hist_off, n * sizeof(float),
+                  cudaMemcpyDeviceToDevice));
+  } else {
+    std::vector<sdb_snr_status> fresh(S);
+    CK(cudaMemcpy(fresh.data(), to.snr.status.get() + hn.chain0, S * sizeof(sdb_snr_status), cudaMemcpyDeviceToHost));
+    const bool bps_changed = cn.cfg.bits_per_symbol != co.cfg.bits_per_symbol;
+    for (unsigned s = 0; s < S; ++s) {
+      const float sigma = bps_changed ? 1.f / 8.f : st[s].sigma;
+      st[s] = fresh[s];
+      st[s].sigma = sigma; st[s].snr = 1.0f / (hn.K * sigma);
+    }
+  }
+  CK(cudaMemcpy(to.snr.status.get() + hn.chain0, st.data(), S * sizeof(sdb_snr_status), cudaMemcpyHostToDevice));
+  return 0;
+}
+
 static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<int> &old_of_new)
 {
   CK(cudaSetDevice(dst->prm.device));
@@ -1908,6 +2073,7 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
       CK(cudaMemcpy(to.fac.fac.get() + to.fac.h[fn].fac_off, from.fac.fac.get() + from.fac.h[fo].fac_off,
                     S * (L / 2) * sizeof(float), cudaMemcpyDeviceToDevice));
     }
+    if (snr_migrate(to, from, cn, co, kn, ko, S)) return -1;
     if (!cn.has_insp || !co.has_insp) continue;
     if (is_power(cn) || is_power(co)) {
       // SPEC PW: the partial group goes on while the inspector stays a power inspector with the same M

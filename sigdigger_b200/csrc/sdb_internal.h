@@ -521,6 +521,24 @@ struct SdbFacArgs {
 int sdb_fac_check(const sdb_fac_params *p);
 // grid[k]: CTAs of the persistent launches over units of kind k (0: no chain has that kind)
 cudaError_t sdb_launch_fac(const SdbLaunchCtx &c, const SdbFacArgs &a, const int grid[SDB_FAC_KINDS]);
+// snr_kernels.cu: the SNR meter (oracle/SPEC_SN.md).  One descriptor per channel with the meter on; its chains are
+// chain0 + s (s < n_streams), each with h and the model at hist_off + s L and its state in status[chain0 + s].
+#define SDB_SNR_BINS_MIN 16u
+#define SDB_SNR_BINS_MAX 1024u
+struct SdbSnrChan {
+  uint32_t L, K, k, chain0;           // bins, comb teeth 2^bps, channel (row s * n_channels + k), first chain
+  int32_t mode;                       // SPEC D: 0 argument, 1 modulus
+  float dmin, dh, alpha;              // SPEC D's min and max - min, the step size
+  size_t hist_off;
+};
+struct SdbSnrArgs {
+  const SdbSnrChan *chans; int n_chans, n_streams, n_channels; uint32_t max_L;
+  const float2 *soft; const uint32_t *counts; size_t sym_cap;
+  uint32_t *hist; float *model; sdb_snr_status *status;
+};
+// engine.cu: the parameter checks of sdb_engine_set_snr (0, or -1 with sdb_last_error() set), shared with the analyzer
+int sdb_snr_check(const sdb_snr_params *p);
+cudaError_t sdb_launch_snr(const SdbLaunchCtx &c, const SdbSnrArgs &a);
 // stream-ordered pieces of the panoramic sweep (panoramic.cu): caller-owned device buffers, no host copies, no
 // default-stream work.  engine.cu:
 int sdb_engine_pack_channels_device(sdb_engine_t *e, const double *centers_dev, sdb_detected_channel *out_dev, size_t cap,
