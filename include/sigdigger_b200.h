@@ -888,8 +888,8 @@ sdb_tv_processor_t *sdb_tv_processor_new(const sdb_tv_params *p, uint32_t batch,
 void sdb_tv_processor_destroy(sdb_tv_processor_t *t);
 int  sdb_tv_processor_set_params(sdb_tv_processor_t *t, const sdb_tv_params *p);
 int  sdb_tv_processor_geometry(const sdb_tv_processor_t *t, uint32_t *width, uint32_t *height);
-/* TVProcessorWorker::work (TVProcessorWorker.cpp:120-151) over the batch: x[batch][stride], n samples each;
- * frames_done[batch]; returns the frames completed in this call (-1 on error) */
+/* TVProcessorWorker::work (TVProcessorWorker.cpp:120-151) over the batch: x[batch][stride], n <= stride samples each
+ * (host or device memory); frames_done[batch]; returns the frames completed in this call (-1 on error) */
 long sdb_tv_processor_feed(sdb_tv_processor_t *t, const float *x, size_t stride, size_t n, uint32_t *frames_done);
 long sdb_tv_processor_feed_device(sdb_tv_processor_t *t, const float *x_dev, size_t stride, size_t n, uint32_t *frames_done);
 int  sdb_tv_processor_frames(sdb_tv_processor_t *t, uint64_t *counts);

@@ -4,10 +4,11 @@
  * (Default/GenericInspector/TVProcessorWorker.cpp:120-151 feed / take_frame loop, :186-239 start / setParams;
  * parameter block sigutils_tv_processor_params as filled at Default/GenericInspector/TVProcessorTab.cpp:549-597;
  * input conversion TVProcessorTab::feed, :601-620).  The processor itself lives in BatchDrake/sigutils (master,
- * unpinned, absent from /root/reference, no vectors): PARITY UNPINNED for the recurrence -- SPEC TV is this
- * project's statement of it; what pins it is behaviour (tests/test_oracle_tv.py: locks on a synthetic composite
- * signal at a non-integer line length, recovers the picture, follows a line-rate offset).  The input conversion is
- * in the reference and is restated value by value (sdo_tv_feed_transform).
+ * unpinned, absent from the reference, no vectors): PARITY UNPINNED for the recurrence -- SPEC TV is this
+ * project's statement of it.  What pins this file is tests/tv_stmt.py, an exact statement written from the SPEC text
+ * alone (tests/test_tv_stmt.py: bit for bit over a table of scenes), and behaviour (tests/test_oracle_tv.py: locks on
+ * a synthetic composite signal at a non-integer line length, recovers the picture, follows a line-rate offset).  The
+ * input conversion is in the reference and is restated value by value (sdo_tv_feed_transform).
  *
  * Plain C, one IEEE binary32 operation per source operation (built -O2 -ffp-contract=off). */
 #include "sd_oracle.h"

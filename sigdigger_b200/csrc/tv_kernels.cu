@@ -179,6 +179,7 @@ extern "C" long sdb_tv_processor_feed_device(sdb_tv_processor_t *t, const float 
 {
   if (!t || !x_dev) return fail("null argument");
   if (n == 0) return 0;
+  if (stride < n) return fail("stride < n");
   CK(cudaSetDevice(t->device));
   return tv_feed(t, x_dev, stride, n, frames_done);
 }

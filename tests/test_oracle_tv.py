@@ -1,6 +1,7 @@
 """CPU: analog-TV processor (SPEC TV; SURVEY 8(f) rank 4).  The recurrence is upstream's (sigutils, not in the
-reference, no vectors): what pins the oracle is behaviour -- it locks on a synthetic composite signal with a fractional
-line length, follows the vertical intervals, recovers the picture -- and the reference-shaped worker loop
+reference, no vectors): what pins the oracle is the exact statement of tests/tv_stmt.py (tests/test_tv_stmt.py) and
+behaviour -- it locks on a synthetic composite signal with a fractional line length, follows the vertical intervals,
+recovers the picture -- and the reference-shaped worker loop
 (tests/shim/reference_tu.cpp: TVProcessorWorker::work over <sigutils/tvproc.h>, whose per-sample entry point runs the
 GPU kernel's own step on the host) is held to the oracle bit for bit.  GPU batch: tests/test_gpu_tv.py."""
 import ctypes as C
