@@ -41,8 +41,9 @@
 //   8     11     out       x0.75, decision (atan2 / modulus quantiser), symbol stores            global
 //
 // Feed-forward work runs beside the recurrences, not in series with them.  Loop state lives in registers for the
-// whole feed, the per-chain lines in shared memory sized from the channel plan (SdbInspDyn).  Loops stay rolled:
-// unrolled or per-class variants grow the code several-fold and starve the role warps on instruction fetch.
+// whole feed, the per-chain lines in shared memory sized from the chains of the launch (SdbInspDyn).  Loops stay
+// rolled: unrolled variants grow the code several-fold and starve the role warps on instruction fetch.  Each inspector
+// class has its own instance of the kernel (ICtx<CLS>), which holds that class's branches only.
 #define CH 16
 enum { INSP_WARPS = 12 };              // role of each warp: see the dispatch at the end of k_inspectors
 #define INSP_STEPS 8          // pipeline depth after the load: a chunk loaded in iteration c leaves in iteration c + 8
@@ -144,14 +145,16 @@ struct ChainSmem {
   int    cnt[2][32];
 };
 
-// what every role needs to know about its lane's chain
-struct ICtx {
+// what every role needs to know about its lane's chain.  CLS is the inspector class (SDB_INSP_*) of every chain of the
+// CTA: each class has its own instance of the kernel, so the branches and the state of the other classes are not in it.
+template <int CLS> struct ICtx {
+  static constexpr int cls = CLS;
   ChainSmem *sm;
   float2 (*rb)[32]; unsigned rb_mask;         // ringB: carrier output, circular, doubles as the matched-filter line
   float  (*taps)[32];                         // per-lane matched-filter taps [t][lane]
   float  (*agc)[32]; int agc_rows;
   float2 (*eqw)[32]; float2 (*eqx)[32];
-  int lane, valid, cls, fresh;
+  int lane, valid, fresh;
   uint32_t n, nchunks;
   const SdbChainCfg *cp; SdbChainState *stp; float *bpool;
 };
@@ -188,7 +191,7 @@ static __device__ __forceinline__ float2 cma_step(float2 (*w)[32], float2 (*x)[3
 }
 
 // ---- steps 0 + 2: tile loader and AGC tracker (warp 0)
-static __device__ void role_track(const ICtx &c, const float2 *chan_row)
+template <int CLS> static __device__ void role_track(const ICtx<CLS> &c, const float2 *chan_row)
 {
   ChainSmem &sm = *c.sm;
   const int lane = c.lane;
@@ -294,7 +297,7 @@ static __device__ void role_track(const ICtx &c, const float2 *chan_row)
 }
 
 // ---- step 1: manual-offset LO + magnitude in dB (warps 1-2, half a chunk each)
-static __device__ void role_pre(const ICtx &c, int part)
+template <int CLS> static __device__ void role_pre(const ICtx<CLS> &c, int part)
 {
   ChainSmem &sm = *c.sm;
   const int lane = c.lane;
@@ -365,7 +368,7 @@ static __device__ void role_pre(const ICtx &c, int part)
 }
 
 // ---- step 3: gain (warps 3-4, half a chunk each)
-static __device__ void role_post(const ICtx &c, int part)
+template <int CLS> static __device__ void role_post(const ICtx<CLS> &c, int part)
 {
   ChainSmem &sm = *c.sm;
   const int lane = c.lane, cls = c.cls;
@@ -437,7 +440,7 @@ static __device__ void role_post(const ICtx &c, int part)
 }
 
 // ---- step 4: carrier stage (warp 5)
-static __device__ void role_carrier(const ICtx &c)
+template <int CLS> static __device__ void role_carrier(const ICtx<CLS> &c)
 {
   ChainSmem &sm = *c.sm;
   const int lane = c.lane, cls = c.cls;
@@ -604,7 +607,7 @@ static __device__ void role_carrier(const ICtx &c)
 // entries (the last mf_n - 1 samples of the previous feed are put back in front of position 0 at kernel start).
 // One thread produces 4 consecutive outputs of its chain from a sliding register window: per tap one ring load,
 // one tap load and four complex-by-real FMAs (complex sample x real tap, SPEC I.1: ascending taps, fused terms).
-static __device__ void role_filter(const ICtx &c, int part, const float *taps_pool)
+template <int CLS> static __device__ void role_filter(const ICtx<CLS> &c, int part, const float *taps_pool)
 {
   ChainSmem &sm = *c.sm;
   const int lane = c.lane;
@@ -750,7 +753,7 @@ static __device__ void role_filter(const ICtx &c, int part, const float *taps_po
 
 // ---- step 6: clock recovery / sampler / resampler, CMA (warp 10).  Emits the chunk's symbols (before the x0.75
 // and the decision) into sym[] and their number into cnt[]; the out role finishes them.
-static __device__ void role_clock(const ICtx &c)
+template <int CLS> static __device__ void role_clock(const ICtx<CLS> &c)
 {
   ChainSmem &sm = *c.sm;
   const int lane = c.lane, cls = c.cls;
@@ -844,7 +847,7 @@ static __device__ void role_clock(const ICtx &c)
 }
 
 // ---- step 7: -2.5 dB, decision, symbol stores (warp 11; feed-forward, off the clock recurrence)
-static __device__ void role_out(const ICtx &c, float2 *__restrict__ so, unsigned char *__restrict__ ho,
+template <int CLS> static __device__ void role_out(const ICtx<CLS> &c, float2 *__restrict__ so, unsigned char *__restrict__ ho,
                                 uint32_t *__restrict__ sym_count, size_t sym_cap)
 {
   ChainSmem &sm = *c.sm;
@@ -877,8 +880,12 @@ static __device__ void role_out(const ICtx &c, float2 *__restrict__ so, unsigned
   if (c.valid) *sym_count = nout;
 }
 
+// One instance per inspector class (CLS = SDB_INSP_*), launched over the CTAs [cta0, cta0 + gridDim.x) of a chain map
+// that holds chains of that class only (sdb_insp_grids).  Every instance keeps 2 CTAs of 384 threads per SM: 80
+// registers; the stack frames ptxas spills to at that bound are held in tests/test_inspector_resources.py.
+template <int CLS>
 __global__ void __launch_bounds__(INSP_WARPS * 32, 2) k_inspectors(const SdbChainCfg *__restrict__ cfgs, int n_channels,
-                                                     int n_streams, const int *__restrict__ chain_map,
+                                                     int n_streams, const int *__restrict__ chain_map, int cta0,
                                                      SdbChainState *__restrict__ states,
                                                      float *__restrict__ pool, size_t pool_stride,
                                                      const float *__restrict__ taps_pool,
@@ -890,7 +897,7 @@ __global__ void __launch_bounds__(INSP_WARPS * 32, 2) k_inspectors(const SdbChai
                                                      const SdbInspDyn dyn)
 {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  ICtx c;
+  ICtx<CLS> c;
   c.sm = reinterpret_cast<ChainSmem *>(smem_raw);
   unsigned char *dp = smem_raw + sizeof(ChainSmem);
   c.rb = reinterpret_cast<float2 (*)[32]>(dp); dp += (size_t) dyn.rb_slots * 32 * sizeof(float2);
@@ -900,18 +907,17 @@ __global__ void __launch_bounds__(INSP_WARPS * 32, 2) k_inspectors(const SdbChai
   c.agc_rows = dyn.agc_rows;
   c.eqw = reinterpret_cast<float2 (*)[32]>(dp); c.eqx = c.eqw + SDB_EQ_LEN;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int chains = n_channels * n_streams;
-  const int slot = blockIdx.x * 32 + lane;
+  const int cta = cta0 + (int) blockIdx.x;
+  const int slot = cta * 32 + lane;
   // chain_map: CTA slot -> channel-major chain index k * S + s, or -1 (padding so that a CTA holds one class)
-  const int g = chain_map ? chain_map[slot] : (slot < chains ? slot : -1);
+  const int g = chain_map[slot];
   const bool valid = g >= 0;
   const int k = valid ? g / n_streams : 0, s = valid ? g - k * n_streams : 0;
   const int chain = s * n_channels + k;                // index into states / outputs (stream-major)
   c.lane = lane; c.valid = valid ? 1 : 0; c.fresh = fresh;
   c.cp = cfgs + k; c.stp = states + chain;
-  c.cls = valid ? c.cp->cls : -1;
   c.n = valid ? n_hops * (uint32_t) chans[k].halfsz : 0;
-  c.bpool = pool + (size_t) blockIdx.x * 32 * pool_stride + lane;     // per-CTA pool, interleaved [slot][lane]
+  c.bpool = pool + (size_t) cta * 32 * pool_stride + lane;     // per-CTA pool, interleaved [slot][lane]
   __shared__ uint32_t s_nmax;
   if (threadIdx.x == 0) s_nmax = 0;
   __syncthreads();
@@ -968,28 +974,29 @@ size_t sdb_inspector_smem_bytes(const SdbInspDyn &dyn)
          (size_t) dyn.agc_rows * 32 * sizeof(float) + (dyn.use_eq ? 2 * (size_t) SDB_EQ_LEN * 32 * sizeof(float2) : 0);
 }
 
-cudaError_t sdb_launch_inspectors_n(const SdbLaunchCtx &c, const SdbChainCfg *cfg_dev, int n_channels,
-                                    int n_streams, const int *chain_map, int n_ctas, SdbChainState *state,
+cudaError_t sdb_launch_inspectors_n(const SdbLaunchCtx &c, const SdbInspGrid &grid, const SdbChainCfg *cfg_dev,
+                                    int n_channels, int n_streams, const int *chain_map, SdbChainState *state,
                                     float *pool, size_t pool_stride,
                                     const float *taps_pool, const SdbChannelDev *chans_dev,
                                     const float2 *chan_in, size_t chan_stream_stride, uint32_t n_hops,
-                                    float2 *soft, uint8_t *hard, uint32_t *sym_counts, size_t sym_cap, int fresh,
-                                    const SdbInspDyn &dyn)
+                                    float2 *soft, uint8_t *hard, uint32_t *sym_counts, size_t sym_cap, int fresh)
 {
-  const int chains = n_channels * n_streams;
-  if (chains == 0) return cudaSuccess;
+  if (grid.n_ctas == 0) return cudaSuccess;
+  using Kernel = decltype(&k_inspectors<SDB_INSP_PSK>);
+  static const Kernel inst[5] = { k_inspectors<SDB_INSP_PSK>, k_inspectors<SDB_INSP_FSK>, k_inspectors<SDB_INSP_ASK>,
+                                  k_inspectors<SDB_INSP_AUDIO>, k_inspectors<SDB_INSP_RAW> };
+  if (grid.cls < 0 || grid.cls >= 5) return cudaErrorInvalidValue;
   static std::atomic<unsigned long long> attr_done{ 0 };   // one bit per device: function attributes are per context
   if (sdb_first_on_device(attr_done))
-    cudaFuncSetAttribute(k_inspectors, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);   // + static < 227 KB
-  const size_t smem = sdb_inspector_smem_bytes(dyn);
-  if (!chain_map) n_ctas = (chains + 31) / 32;
+    for (Kernel k : inst) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);   // + static < 227 KB
+  const size_t smem = sdb_inspector_smem_bytes(grid.dyn);
   // SDB_INSP_PLACEMENT=linear: roles in warp order (track, pre x2, post x2, carrier, filter x4, clock, out), the
   // placement of the first builds -- kept for A/B measurements
   static const bool linear = getenv("SDB_INSP_PLACEMENT") && !strcmp(getenv("SDB_INSP_PLACEMENT"), "linear");
-  SdbInspDyn d2 = dyn;
+  SdbInspDyn d2 = grid.dyn;
   if (linear) { d2.role_lut = 0x653333244110ull; d2.part_lut = 0x3210010100ull; }
-  k_inspectors<<<n_ctas, INSP_WARPS * 32, smem, c.stream>>>(
-      cfg_dev, n_channels, n_streams, chain_map, state, pool, pool_stride, taps_pool, chans_dev, chan_in,
+  inst[grid.cls]<<<grid.n_ctas, INSP_WARPS * 32, smem, c.stream>>>(
+      cfg_dev, n_channels, n_streams, chain_map, grid.cta0, state, pool, pool_stride, taps_pool, chans_dev, chan_in,
       chan_stream_stride, n_hops, soft, hard, sym_counts, sym_cap, fresh, d2);
   if (c.launch_counter) ++*c.launch_counter;
   return cudaGetLastError();

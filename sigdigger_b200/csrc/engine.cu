@@ -126,6 +126,10 @@ struct Plan {
   SdbChainState *d_state = nullptr;
   float *d_pool = nullptr; size_t pool_stride = 0;
   int *d_chain_map = nullptr; int insp_ctas = 0; std::vector<int> h_chain_map;
+  // one inspector grid per class run of the chain map, launched in the map's order on the inspector stream.  They do
+  // not run concurrently: two classes' kernels on one SM fetch from two code images, and every role of both slowed
+  // down (DESIGN.md section 5); the next feed's transforms fill the SMs a grid's last wave leaves free.
+  std::vector<SdbInspGrid> insp_grids;
   float *d_taps = nullptr;
   size_t sym_cap = 0;
   // power inspectors (SPEC PW; power_kernels.cu): one integrator per (power channel, stream), channel-major, and the
@@ -1410,6 +1414,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
     p.d_chain_map = p.dalloc<int>(p.h_chain_map.size());
     if (!p.d_chain_map) return fail("out of device memory (chain map)");
     CK(cudaMemcpy(p.d_chain_map, p.h_chain_map.data(), p.h_chain_map.size() * sizeof(int), cudaMemcpyHostToDevice));
+    p.insp_grids = sdb_insp_grids(p.h_cfg.data(), (int) S, p.h_chain_map);
     const size_t pool_floats = (size_t) p.insp_ctas * 32 * pool;   // per-CTA interleaved [slot][lane]
     p.d_pool = p.dalloc<float>(pool_floats);
     p.d_taps = p.dalloc<float>(taps_pool.size());
@@ -1686,12 +1691,12 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
                                p.chan_stride, (uint32_t) wps, p.d_spect, p.spect_stride, p.d_spect_size,
                                p.d_est, p.d_est_valid));
       if (!p.sched.empty() && sched_feed(e, p, sl, ictx, (uint64_t) wps)) return -1;
-      if (p.insp_ctas > 0) {                      // (every channel a power inspector: no chain)
+      if (!p.insp_grids.empty()) {                // (every channel a power inspector: no chain)
         e->span_begin(FAM_INSPECTOR, ictx.stream);
-        CK(sdb_launch_inspectors_n(ictx, p.d_cfg, K, (int) S, p.d_chain_map, p.insp_ctas, p.d_state, p.d_pool,
-                                   p.pool_stride, p.d_taps,
-                                   p.d_chans, sl.chan, p.chan_stride, (uint32_t) wps, sl.soft, sl.hard,
-                                   sl.counts, p.sym_cap, 0, sdb_insp_dyn(p.h_cfg.data(), K)));
+        for (const SdbInspGrid &g : p.insp_grids)
+          CK(sdb_launch_inspectors_n(ictx, g, p.d_cfg, K, (int) S, p.d_chain_map, p.d_state, p.d_pool, p.pool_stride,
+                                     p.d_taps, p.d_chans, sl.chan, p.chan_stride, (uint32_t) wps, sl.soft, sl.hard,
+                                     sl.counts, p.sym_cap, 0));
         e->span_end(ictx.stream);
       }
       if (p.n_power) {
@@ -2166,10 +2171,15 @@ extern "C" long sdb_task_inspector(const sdb_inspector_config *cfg, const sdb_co
   const std::vector<SdbChainState> st(batch, chain_layout(c));
   const size_t pool = (size_t) std::max(1, c.st_pool);
   SdbChannelDev cd; memset(&cd, 0, sizeof(cd)); cd.halfsz = 1; cd.out_off = 0;
-  const size_t pool_floats = ((batch + 31) / 32) * 32 * pool;
+  std::vector<int> map;
+  const int n_ctas = sdb_build_chain_map(&c, 1, (int) batch, map);
+  const std::vector<SdbInspGrid> grids = sdb_insp_grids(&c, (int) batch, map);   // (one class: one grid)
+  const size_t pool_floats = (size_t) n_ctas * 32 * pool;
   DevBuf<float2> d_src, d_soft; DevBuf<uint8_t> d_hard; DevBuf<uint32_t> d_cnt; DevBuf<SdbChainCfg> d_cfg;
-  DevBuf<SdbChainState> d_st; DevBuf<float> d_pool, d_taps; DevBuf<SdbChannelDev> d_cd;
+  DevBuf<SdbChainState> d_st; DevBuf<float> d_pool, d_taps; DevBuf<SdbChannelDev> d_cd; DevBuf<int> d_map;
   CK(d_src.alloc(n * batch)); CK(d_soft.alloc(cap * batch)); CK(d_hard.alloc(cap * batch)); CK(d_cnt.alloc(batch));
+  CK(d_map.alloc(map.size()));
+  CK(cudaMemcpy(d_map, map.data(), map.size() * sizeof(int), cudaMemcpyHostToDevice));
   CK(d_cfg.alloc(1)); CK(d_st.alloc(batch)); CK(d_pool.alloc(pool_floats));
   CK(d_taps.alloc(std::max<size_t>(1, taps.size()))); CK(d_cd.alloc(1));
   CK(cudaMemcpy(d_src, src, n * batch * sizeof(float2), cudaMemcpyHostToDevice));
@@ -2180,8 +2190,9 @@ extern "C" long sdb_task_inspector(const sdb_inspector_config *cfg, const sdb_co
   CK(cudaMemcpy(d_cd, &cd, sizeof(cd), cudaMemcpyHostToDevice));
   SdbLaunchCtx ctx{ 0, nullptr };
   // every chain is "stream s, channel 0"; chan_stream_stride = n
-  CK(sdb_launch_inspectors_n(ctx, d_cfg, 1, (int) batch, nullptr, 0, d_st, d_pool, pool, d_taps, d_cd, d_src, n,
-                             (uint32_t) n, d_soft, d_hard, d_cnt, cap, 1, sdb_insp_dyn(&c, 1)));
+  for (const SdbInspGrid &g : grids)
+    CK(sdb_launch_inspectors_n(ctx, g, d_cfg, 1, (int) batch, d_map, d_st, d_pool, pool, d_taps, d_cd, d_src, n,
+                               (uint32_t) n, d_soft, d_hard, d_cnt, cap, 1));
   CK(cudaDeviceSynchronize());
   CK(cudaMemcpy(counts, d_cnt, batch * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   if (soft) CK(cudaMemcpy(soft, d_soft, cap * batch * sizeof(float2), cudaMemcpyDeviceToHost));

@@ -388,6 +388,28 @@ static inline int sdb_build_chain_map(const SdbChainCfg *cfgs, int K, int S, std
   while (map.size() % 32) map.push_back(-1);
   return (int) (map.size() / 32);
 }
+
+// One launch of k_inspectors: the CTAs [cta0, cta0 + n_ctas) of a chain map, every chain of them of inspector class
+// cls, with the shared-memory lines of those chains alone.  sdb_insp_grids cuts a map from sdb_build_chain_map into
+// one grid per run of CTAs of one class, in the map's order (slowest class first).
+struct SdbInspGrid { int cls, cta0, n_ctas; SdbInspDyn dyn; };
+static inline std::vector<SdbInspGrid> sdb_insp_grids(const SdbChainCfg *cfgs, int S, const std::vector<int> &map)
+{
+  std::vector<SdbInspGrid> out;
+  std::vector<SdbChainCfg> run;                     // the channels of the current grid, once each
+  int last_k = -1;
+  auto close = [&]() { if (!out.empty()) out.back().dyn = sdb_insp_dyn(run.data(), (int) run.size()); run.clear(); };
+  for (size_t q = 0; q < map.size(); q += 32) {
+    const int g = map[q];                           // a CTA's first slot always holds a chain
+    const int cta = (int) (q / 32), cls = cfgs[g / S].cls;
+    if (out.empty() || out.back().cls != cls) { close(); out.push_back(SdbInspGrid{ cls, cta, 0, {} }); last_k = -1; }
+    ++out.back().n_ctas;
+    for (size_t l = q; l < q + 32; ++l)
+      if (map[l] >= 0 && map[l] / S != last_k) { last_k = map[l] / S; run.push_back(cfgs[last_k]); }
+  }
+  close();
+  return out;
+}
 #endif
 
 // host-callable launchers ----------------------------------------------------------------------
@@ -418,15 +440,14 @@ cudaError_t sdb_launch_sym_pack(cudaStream_t stream, const uint32_t *counts, uns
                                 const float2 *soft, const unsigned char *hard, size_t cap, void *out_soft,
                                 void *out_hard, unsigned long long cap_total, uint64_t *launch_counter);
 size_t sdb_inspector_smem_bytes(const SdbInspDyn &dyn);
-// chain_map / n_ctas from sdb_build_chain_map (null: identity, (chains + 31) / 32 CTAs); the pool holds
-// n_ctas * 32 * pool_stride floats
-cudaError_t sdb_launch_inspectors_n(const SdbLaunchCtx &c, const SdbChainCfg *cfg_dev, int n_channels,
-                                    int n_streams, const int *chain_map, int n_ctas, SdbChainState *state,
+// one grid of sdb_insp_grids over chain_map (from sdb_build_chain_map); the pool holds 32 * pool_stride floats per CTA
+// of the whole map
+cudaError_t sdb_launch_inspectors_n(const SdbLaunchCtx &c, const SdbInspGrid &grid, const SdbChainCfg *cfg_dev,
+                                    int n_channels, int n_streams, const int *chain_map, SdbChainState *state,
                                     float *pool, size_t pool_stride,
                                     const float *taps_pool, const SdbChannelDev *chans_dev,
                                     const float2 *chan_in, size_t chan_stream_stride, uint32_t n_hops,
-                                    float2 *soft, uint8_t *hard, uint32_t *sym_counts, size_t sym_cap,
-                                    int fresh, const SdbInspDyn &dyn);
+                                    float2 *soft, uint8_t *hard, uint32_t *sym_counts, size_t sym_cap, int fresh);
 cudaError_t sdb_launch_spectsrc(const SdbLaunchCtx &c, const SdbSpectCfg *cfg_dev, const SdbChannelDev *chans_dev,
                                 int n_channels, int n_streams, int max_ns, const float2 *chan_in,
                                 size_t chan_stream_stride, uint32_t n_hops, float *spect, size_t spect_stream_stride,
