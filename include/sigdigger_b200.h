@@ -310,6 +310,49 @@ int  sdb_engine_set_snr(sdb_engine_t *e, int handle, const sdb_snr_params *p);
 int  sdb_engine_reset_snr(sdb_engine_t *e, int handle, float sigma);
 int  sdb_engine_read_snr(sdb_engine_t *e, int handle, uint32_t *hist, float *model, sdb_snr_status *st);
 
+/* ---- the inspector's Analog TV tab (TVProcessorTab::feed, Default/GenericInspector/TVProcessorTab.cpp:601-620;
+ * TVProcessorWorker::work, TVProcessorWorker.cpp:120-158; oracle/SPEC_TI.md) ----
+ * One TV processor per stream of a psk / fsk / ask inspector, run by the engine over every feed's soft symbols (what
+ * SAMPLES carries): each symbol becomes k |x| + dc (ask) or k arg(x) / pi + dc (psk, fsk), with k = -1 when
+ * invert_sync is set and +1 otherwise, and dc as given (the tab passes its DC value / 100), and runs one step of SPEC
+ * TV, in order.  A feed
+ * without symbols changes nothing.  Per feed the processor reports how many frames it completed and posts the first of
+ * them, exactly as it stood when it completed, however many frames the feed completed.  Every symbol is processed: the
+ * worker's frame acknowledgement and its maxProcessingBlock truncation are not reproduced.
+ * set_tv: before commit; NULL turns the tab off.  Commit refuses another class, parameters sdb_tv_processor_new refuses
+ * and an allocation that does not fit.  Device memory per (channel, stream): (SDB_TV_RING + 1) W H + W + delay_len
+ * floats (W = floor(line_len), H = frame_lines, delay_len = ceil(line_len), the ring of 4 frames and the posted frame)
+ * plus 168 bytes of state and status; PAL at 8 MS/s (W 512, H 625) is 6.4 MB per stream.
+ * set_tv_params: between feeds, from the next feed on; the state is kept.  Refused with the tab off or when the
+ * geometry (W, H, delay_len, interlace) would change: that needs a new plan.
+ * read_tv: frames[n_streams][H][W] (the posted frames, valid where completed > 0; may be NULL) and st[n_streams] after
+ * the latest feed (waits for it).
+ * Migration: a channel that keeps its inspector class and the geometry keeps the whole processor (state, comb delay
+ * line, row being drawn, ring, posted frame and frame count), whatever else of its configuration changed; the new
+ * parameters apply from the next feed.  Anything else starts afresh. */
+/* the analog-TV processor's parameters (SPEC.md section TV; the stand-alone processor sdb_tv_processor_* is below):
+ * the fields of struct sigutils_tv_processor_params as the reference fills them (lengths in samples) */
+typedef struct {
+  int32_t  enable_sync, reverse, interlace, enable_agc;
+  float    x_off;
+  int32_t  dominance;
+  uint32_t frame_lines;
+  float    frame_spacing;                     /* fractional lines per frame beyond frame_lines (TVProcessorTab.cpp:559) */
+  int32_t  enable_comb, comb_reverse;
+  float    hsync_len, vsync_len, line_len;    /* samples */
+  uint32_t vsync_odd_trigger;                 /* equalising pulses that end a field */
+  float    t_tol, l_tol, g_tol;
+  float    hsync_huge_err, hsync_max_err, hsync_min_err;
+  float    hsync_len_tau, line_len_tau, agc_tau, hsync_fast_track_tau, hsync_slow_track_tau;
+} sdb_tv_params;
+typedef struct { sdb_tv_params tv; int32_t invert_sync; float dc; } sdb_tv_tab_params;
+/* frames: completed since the start; posted_no: the posted frame's number (1 = the first frame), 0 before any;
+ * completed: frames the latest feed completed; width, height: W, H; line_len, hsync_len, agc_gain: the estimates */
+typedef struct { uint64_t frames, posted_no; uint32_t completed, width, height; float line_len, hsync_len, agc_gain; } sdb_tv_status;
+int  sdb_engine_set_tv(sdb_engine_t *e, int handle, const sdb_tv_tab_params *p);
+int  sdb_engine_set_tv_params(sdb_engine_t *e, int handle, const sdb_tv_tab_params *p);
+int  sdb_engine_read_tv(sdb_engine_t *e, int handle, float *frames, sdb_tv_status *st);
+
 /* ---- channel detector on the main PSD (SURVEY.md 8(f) rank 3; SPEC.md section K) ----
  * struct suscan_analyzer_params.detector_params.{alpha, beta, gamma, snr} + channel_update_int
  * (Suscan/AnalyzerParams.cpp:27-66) -> SUSCAN_ANALYZER_MESSAGE_TYPE_CHANNEL lists of struct sigutils_channel
@@ -386,7 +429,8 @@ uint64_t sdb_engine_launch_count(const sdb_engine_t *e);
  * "psd_peak" (the group extremes) none while peak detection is off, "spectsrc_sched" (the scheduled spectra: frame
  * gather, transforms and ring update) none in a feed that neither emits nor keeps samples, "fac" (the FAC tab's
  * launches, sdb_engine_set_fac) none while no channel has the FAC on, "snr" (the SNR meter's k_snr, sdb_engine_set_snr)
- * none while no channel has the meter on */
+ * none while no channel has the meter on, "tv" (the TV tab's k_tv_insp, sdb_engine_set_tv) none while no channel has
+ * the TV on */
 int      sdb_engine_kernel_time(sdb_engine_t *e, const char *family, double *avg_ms, uint64_t *launches);
 void     sdb_engine_timing(sdb_engine_t *e, int enable);
 /* inspector-kernel stage balance since the last reset: out[0..3] = busy SM cycles of the gain / carrier /
@@ -563,7 +607,8 @@ enum {   /* SUSCAN_ANALYZER_INSPECTOR_MSGKIND_* (Suscan/AnalyzerRequestTracker.c
   SDB_INSPECTOR_MSGKIND_CLOSE, SDB_INSPECTOR_MSGKIND_INVALID_CHANNEL, SDB_INSPECTOR_MSGKIND_WRONG_HANDLE,
   SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, SDB_INSPECTOR_MSGKIND_WRONG_KIND,
   SDB_INSPECTOR_MSGKIND_FAC,         /* this project's: the FAC tab (oracle/SPEC_FC.md); suscan has no such kind */
-  SDB_INSPECTOR_MSGKIND_SNR          /* this project's: the SNR meter (oracle/SPEC_SN.md); suscan has no such kind */
+  SDB_INSPECTOR_MSGKIND_SNR,         /* this project's: the SNR meter (oracle/SPEC_SN.md); suscan has no such kind */
+  SDB_INSPECTOR_MSGKIND_TV           /* this project's: the Analog TV tab (oracle/SPEC_TI.md); suscan has no such kind */
 };
 enum { SDB_ANALYZER_MODE_CHANNEL = 0, SDB_ANALYZER_MODE_WIDE_SPECTRUM = 1 };
 
@@ -657,6 +702,11 @@ typedef struct {                  /* suscan_analyzer_inspector_msg, fields this 
    * and h[bins] in snr_histogram (freed with the message) (sdb_engine_read_snr) */
   sdb_snr_status snr;
   uint32_t *snr_histogram;
+  /* kind = TV: the acknowledgement of sdb_analyzer_inspector_set_tv_async (no data), or, after the SAMPLES (and the FAC
+   * and SNR messages) of every block whose feed completed a frame, the status here and the posted frame
+   * [height][width] in tv_frame (freed with the message) (sdb_engine_read_tv) */
+  sdb_tv_status tv;
+  float *tv_frame;
 } sdb_analyzer_inspector_msg;
 /* suscan_analyzer_channel_msg (Suscan/Messages/ChannelMessage.cpp:25-70): posted every channel_update_int seconds
  * of signal time when channel_update_int > 0 */
@@ -704,6 +754,13 @@ int    sdb_analyzer_inspector_set_fac_async(sdb_analyzer_t *a, int32_t handle, c
  * sdb_engine_set_snr refuses, or a reset with the meter off or a sigma that is not finite and positive) otherwise. */
 int    sdb_analyzer_inspector_set_snr_async(sdb_analyzer_t *a, int32_t handle, const sdb_snr_params *p, uint32_t req_id);
 int    sdb_analyzer_inspector_reset_snr_async(sdb_analyzer_t *a, int32_t handle, float sigma, uint32_t req_id);
+/* the Analog TV tab of a psk / fsk / ask inspector (sdb_engine_set_tv; p NULL = off).  Turning it on or off, or a
+ * change of the picture geometry, takes effect through the re-plan, which keeps the processor as sdb_engine_migrate
+ * says; a change that keeps the geometry while the tab is on is applied at the next block boundary without a re-plan
+ * (sdb_engine_set_tv_params).  A frame is posted once per block, not once per SAMPLES batch.  Acknowledged by an
+ * INSPECTOR message of kind TV; WRONG_HANDLE, WRONG_KIND (another class) or WRONG_OBJECT (parameters sdb_engine_set_tv
+ * refuses) otherwise. */
+int    sdb_analyzer_inspector_set_tv_async(sdb_analyzer_t *a, int32_t handle, const sdb_tv_tab_params *p, uint32_t req_id);
 int    sdb_analyzer_inspector_estimator_cmd_async(sdb_analyzer_t *a, int32_t handle, uint32_t estimator_id,
                                                   int enabled, uint32_t req_id);
 int    sdb_analyzer_set_params_async(sdb_analyzer_t *a, const sdb_analyzer_params *p, uint32_t req_id);
@@ -866,19 +923,7 @@ int      sdb_sview_feed_view(sdb_sview_t *v, const sdb_sview_t *detail);
  * The input is the TV tab's real-valued signal with the sync tips HIGH (TVProcessorTab::feed, :601-620:
  * sdb_tv_feed_transform).  The sigutils-named per-sample interface (su_tv_processor_feed ...) is <sigutils/tvproc.h>.
  * ---------------------------------------------------------------------------------------------- */
-typedef struct {
-  int32_t  enable_sync, reverse, interlace, enable_agc;
-  float    x_off;
-  int32_t  dominance;
-  uint32_t frame_lines;
-  float    frame_spacing;                     /* fractional lines per frame beyond frame_lines (TVProcessorTab.cpp:559) */
-  int32_t  enable_comb, comb_reverse;
-  float    hsync_len, vsync_len, line_len;    /* samples */
-  uint32_t vsync_odd_trigger;                 /* equalising pulses that end a field */
-  float    t_tol, l_tol, g_tol;
-  float    hsync_huge_err, hsync_max_err, hsync_min_err;
-  float    hsync_len_tau, line_len_tau, agc_tau, hsync_fast_track_tau, hsync_slow_track_tau;
-} sdb_tv_params;
+/* sdb_tv_params: with the engine's Analog TV tab, above */
 typedef struct sdb_tv_processor sdb_tv_processor_t;
 /* su_tv_processor_params_pal / _ntsc (TVProcessorTab.cpp:629,633) */
 void sdb_tv_params_pal(sdb_tv_params *p, float samp_rate);

@@ -331,6 +331,9 @@ _PROTOS = {
     "sdb_engine_set_snr": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "sdb_engine_reset_snr": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
     "sdb_engine_read_snr": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sdb_engine_set_tv": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "sdb_engine_set_tv_params": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "sdb_engine_read_tv": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_read_spectrum": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_read_estimate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "sdb_engine_set_spectrum_interval": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
@@ -407,6 +410,7 @@ _PROTOS = {
     "sdb_analyzer_inspector_set_fac_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32]),
     "sdb_analyzer_inspector_set_snr_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32]),
     "sdb_analyzer_inspector_reset_snr_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.c_uint32]),
+    "sdb_analyzer_inspector_set_tv_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32]),
     "sdb_analyzer_inspector_estimator_cmd_async": (C.c_int, [C.c_void_p, C.c_int32, C.c_uint32, C.c_int, C.c_uint32]),
     "sdb_analyzer_get_samp_rate": (C.c_uint64, [C.c_void_p]),
     "sdb_analyzer_get_measured_samp_rate": (C.c_float, [C.c_void_p]),
@@ -575,6 +579,7 @@ class Engine:
         self._fac_size = {}                 # FAC block size of every channel with the FAC on (set_fac)
         self._snr_bins = {}                 # histogram bins of every channel with the SNR meter on (set_snr)
         self._bps = {}                      # bits_per_symbol of every channel's inspector (set_inspector)
+        self._baud = {}                     # baud of every channel's inspector (set_inspector)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -605,6 +610,7 @@ class Engine:
             setattr(cfg, k, v)
         _check(self._L.sdb_engine_set_inspector(self._h, h, C.byref(cfg)))
         self._bps[h] = cfg.bits_per_symbol
+        self._baud[h] = cfg.baud
 
     def commit(self):
         _check(self._L.sdb_engine_commit(self._h))
@@ -768,6 +774,34 @@ class Engine:
         st = (SnrStatus * self.n_streams)()
         _check(self._L.sdb_engine_read_snr(self._h, h, hist.ctypes.data, model.ctypes.data, st))
         return hist, model, list(st)
+
+    # ---- the inspector's Analog TV tab (oracle/SPEC_TI.md): before commit, after set_inspector
+    def set_tv(self, h, params=None, invert=False, dc=0.0, enabled=True):
+        """Run a TV processor over h's soft symbols in every stream (k |x| + dc for ask, k arg(x) / pi + dc for psk and
+        fsk, k = -1 with invert); params: a tv_params(...) block, None: PAL at the inspector's symbol rate (one sample
+        per symbol); dc: the tab's DC value / 100; enabled=False: off"""
+        if not enabled:
+            _check(self._L.sdb_engine_set_tv(self._h, h, None))
+            return
+        _check(self._L.sdb_engine_set_tv(self._h, h, C.byref(self._tv_tab(h, params, invert, dc))))
+
+    def set_tv_params(self, h, params=None, invert=False, dc=0.0):
+        """between feeds, from the next feed on; the picture geometry must stay (else a new plan is needed)"""
+        _check(self._L.sdb_engine_set_tv_params(self._h, h, C.byref(self._tv_tab(h, params, invert, dc))))
+
+    def _tv_tab(self, h, params, invert, dc):
+        if params is None:
+            params = tv_params("pal", self._baud[h])
+        return TvTabParams(params, int(bool(invert)), dc)
+
+    def read_tv(self, h):
+        """-> (frames [n_streams, H, W] float32: each stream's posted frame, valid where completed > 0, list of TvStatus
+        per stream) after the latest feed"""
+        st = (TvStatus * self.n_streams)()
+        _check(self._L.sdb_engine_read_tv(self._h, h, None, st))
+        frames = np.zeros((self.n_streams, st[0].height, st[0].width), np.float32)
+        _check(self._L.sdb_engine_read_tv(self._h, h, frames.ctypes.data, None))
+        return frames, list(st)
 
     # ---- inspector spectrum sources / estimators (SPEC U; Suscan/Analyzer.cpp:539-565)
     def set_spectrum_source(self, h, kind, size=1024):
@@ -1394,6 +1428,17 @@ class TvProcessor:
         a, b, g = C.c_float(), C.c_float(), C.c_float()
         _check(self._L.sdb_tv_processor_estimates(self._h, which, C.byref(a), C.byref(b), C.byref(g)))
         return a.value, b.value, g.value
+
+
+class TvTabParams(C.Structure):
+    """sdb_tv_tab_params: the Analog TV tab of one inspector (oracle/SPEC_TI.md)."""
+    _fields_ = [("tv", TvParams), ("invert_sync", C.c_int32), ("dc", C.c_float)]
+
+
+class TvStatus(C.Structure):
+    """sdb_tv_status: one stream's TV processor after the latest feed."""
+    _fields_ = [("frames", C.c_uint64), ("posted_no", C.c_uint64), ("completed", C.c_uint32), ("width", C.c_uint32),
+                ("height", C.c_uint32), ("line_len", C.c_float), ("hsync_len", C.c_float), ("agc_gain", C.c_float)]
 
 
 def tv_feed_transform(x, mode, k=1.0, dc=0.0):

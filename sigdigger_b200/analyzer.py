@@ -6,8 +6,8 @@ import ctypes as C
 
 import numpy as np
 
-from . import (INSP, WINDOW, FacParams, FacStatus, InspectorConfig, SdbError, SnrParams, SnrStatus, last_error,
-               load_library)
+from . import (INSP, WINDOW, FacParams, FacStatus, InspectorConfig, SdbError, SnrParams, SnrStatus, TvStatus,
+               TvTabParams, last_error, load_library)
 
 MSG = {"SOURCE_INFO": 0, "SOURCE_INIT": 1, "CHANNEL": 2, "EOS": 3, "READ_ERROR": 4, "INTERNAL": 5, "SAMPLES": 6,
        "INSPECTOR": 7, "PSD": 8, "PARAMS": 9, "HALT": 0xffffffff, "TIMEOUT": 0xfffffffe}
@@ -16,7 +16,7 @@ MSG_NAME = {v: k for k, v in MSG.items()}
 PSD_DETECTOR = {"default": 0, "pos_peak": 1, "neg_peak": 2}
 KIND = {0: "OPEN", 1: "SET_ID", 2: "GET_CONFIG", 3: "SET_CONFIG", 4: "ESTIMATOR", 5: "SPECTRUM", 6: "CLOSE",
         7: "INVALID_CHANNEL", 8: "WRONG_HANDLE", 9: "WRONG_OBJECT", 10: "WRONG_KIND", 11: "FAC",
-        12: "SNR"}
+        12: "SNR", 13: "TV"}
 
 
 class Timeval(C.Structure):
@@ -74,7 +74,8 @@ class InspectorMsg(C.Structure):
                 ("spectsrc_count", C.c_uint32), ("estimator_count", C.c_uint32), ("spectsrc_id", C.c_uint32),
                 ("spectrum_data", C.POINTER(C.c_float)), ("spectrum_size", C.c_uint64), ("samp_rate", C.c_uint64),
                 ("estimator_id", C.c_uint32), ("enabled", C.c_int32), ("value", C.c_float), ("fac", FacStatus),
-                ("snr", SnrStatus), ("snr_histogram", C.POINTER(C.c_uint32))]
+                ("snr", SnrStatus), ("snr_histogram", C.POINTER(C.c_uint32)), ("tv", TvStatus),
+                ("tv_frame", C.POINTER(C.c_float))]
 
 
 class ChannelMsg(C.Structure):
@@ -238,6 +239,16 @@ class Analyzer:
         """the meter's sigma from the next block on; the histogram is kept"""
         self._L.sdb_analyzer_inspector_reset_snr_async(self._h, handle, sigma, req_id)
 
+    def set_tv(self, handle, params=None, invert=False, dc=0.0, enabled=True, req_id=0):
+        """the Analog TV tab of a psk / fsk / ask inspector (oracle/SPEC_TI.md): params a tv_params(...) block at the
+        inspector's symbol rate, invert the tab's "invert sync", dc its DC value / 100; enabled=False (or params None):
+        off.  A change that keeps the picture geometry applies at the next block without a re-plan."""
+        if not enabled or params is None:
+            self._L.sdb_analyzer_inspector_set_tv_async(self._h, handle, None, req_id)
+            return
+        p = TvTabParams(params, int(bool(invert)), dc)
+        self._L.sdb_analyzer_inspector_set_tv_async(self._h, handle, C.byref(p), req_id)
+
     def estimator_cmd(self, handle, estimator_id, enabled=True, req_id=0):
         self._L.sdb_analyzer_inspector_estimator_cmd_async(self._h, handle, estimator_id, int(enabled), req_id)
 
@@ -307,6 +318,13 @@ class Analyzer:
                     out["histogram"] = None
                     if m.snr_histogram and m.spectrum_size:
                         out["histogram"] = np.ctypeslib.as_array(m.snr_histogram, shape=(m.spectrum_size,)).copy()
+                if out["kind"] == "TV":
+                    q = m.tv
+                    out["tv"] = dict(frames=q.frames, posted_no=q.posted_no, completed=q.completed, width=q.width,
+                                     height=q.height, line_len=q.line_len, hsync_len=q.hsync_len, agc_gain=q.agc_gain)
+                    out["frame"] = None
+                    if m.tv_frame and q.width and q.height:
+                        out["frame"] = np.ctypeslib.as_array(m.tv_frame, shape=(q.height, q.width)).copy()
             elif name == "CHANNEL":
                 from . import DetectedChannel
                 m = C.cast(ptr, C.POINTER(ChannelMsg)).contents

@@ -39,7 +39,7 @@ namespace {
 struct Cmd {
   enum Kind { OPEN, SET_ID, SET_CONFIG, CLOSE, SET_PARAMS, SET_SPECTRUM, ESTIMATOR_CMD, SET_IQ_REVERSE, SET_THROTTLE, SET_WATERMARK,
               SET_FREQ, SET_BANDWIDTH, SEEK, SET_HOP_RANGE, SET_REL_BW, SET_BUFFERING, SET_STRATEGY,
-              SET_PARTITIONING, SET_HISTORY, REPLAY, SET_DC_REMOVE, SET_FAC, SET_SNR, RESET_SNR } kind;
+              SET_PARTITIONING, SET_HISTORY, REPLAY, SET_DC_REMOVE, SET_FAC, SET_SNR, RESET_SNR, SET_TV } kind;
   double value2 = 0;
   uint32_t req_id = 0;
   uint32_t aux_id = 0; int enabled = 0;       // spectrum source id / estimator id + enable flag
@@ -54,6 +54,7 @@ struct Cmd {
   sdb_analyzer_params params{};
   sdb_fac_params fac{};                       // SET_FAC (enabled: on)
   sdb_snr_params snr{};                       // SET_SNR (enabled: on); RESET_SNR: sigma
+  sdb_tv_tab_params tv{};                     // SET_TV (enabled: on)
 };
 
 struct Insp {
@@ -79,6 +80,9 @@ struct Insp {
   sdb_snr_params snr;
   bool snr_reset;         // a reset to snr_reset_sigma waits for the next block boundary
   float snr_reset_sigma;
+  bool tv_on;             // the Analog TV tab (SPEC TI) with these parameters
+  sdb_tv_tab_params tv;
+  bool tv_live;           // a change of tv that keeps the geometry waits for the next block boundary
 };
 
 // class names in SDB_INSP_* order, as requests and inspector messages carry them
@@ -288,6 +292,7 @@ struct sdb_analyzer {
       sdb_engine_set_inspector(e.get(), h, &i.cfg);
       if (i.fac_on) sdb_engine_set_fac(e.get(), h, &i.fac);      // (checked when requested; the class cannot change)
       if (i.snr_on) sdb_engine_set_snr(e.get(), h, &i.snr);      // (likewise)
+      if (i.tv_on) sdb_engine_set_tv(e.get(), h, &i.tv);         // (likewise)
       // spectrum source / estimators: the largest frame (<= 4096) a steady-state block can fill (SPEC U.1)
       i.spect_size = 0; i.spect_sched = false;
       if ((i.spectsrc_id || i.est_mask) && params.spectrum_update_int > 0) {
@@ -450,6 +455,7 @@ struct sdb_analyzer {
         case Cmd::SET_FAC:
         case Cmd::SET_SNR:
         case Cmd::RESET_SNR:
+        case Cmd::SET_TV:
         case Cmd::CLOSE: {
           Insp *ip = open_insp(c.handle);
           if (!ip) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_HANDLE, c, nullptr); break; }
@@ -479,6 +485,14 @@ struct sdb_analyzer {
             }
             i.snr_reset = true; i.snr_reset_sigma = c.snr.sigma;      // no re-plan: applied before the next block
             post_inspector(SDB_INSPECTOR_MSGKIND_SNR, c, &i);
+          } else if (c.kind == Cmd::SET_TV) {
+            if (c.enabled && i.cls > SDB_INSP_ASK) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_KIND, c, nullptr); break; }
+            if (c.enabled && sdb_tv_tab_check(&c.tv)) { post_inspector(SDB_INSPECTOR_MSGKIND_WRONG_OBJECT, c, nullptr); break; }
+            // SPEC TI.4: the same geometry while on is a live change at the next block boundary; anything else re-plans
+            if (c.enabled && i.tv_on && sdb_tv_same_geometry(i.tv.tv, c.tv.tv)) i.tv_live = true;
+            else { i.tv_on = c.enabled != 0; i.tv_live = false; plan_dirty = true; }
+            i.tv = c.tv;
+            post_inspector(SDB_INSPECTOR_MSGKIND_TV, c, &i);          // acknowledgement: frames follow per block
           } else if (c.kind == Cmd::SET_ID) {
             i.inspector_id = c.inspector_id; i.has_id = true;
             post_inspector(SDB_INSPECTOR_MSGKIND_SET_ID, c, &i);
@@ -920,6 +934,37 @@ struct sdb_analyzer {
     }
   }
 
+  // SPEC TI.4: the live changes requested since the last block, on the engines that run the next one
+  void apply_tv_params()
+  {
+    for (auto &i : insps) {
+      if (!i.tv_live) continue;
+      i.tv_live = false;
+      sdb_engine_t *ie = engine_of(i);
+      if (i.open && i.tv_on && i.engine_handle >= 0 && ie) sdb_engine_set_tv_params(ie, i.engine_handle, &i.tv);
+    }
+  }
+
+  // kind=TV inspector messages (SPEC TI.3): one per block whose feed completed a frame, after the block's SAMPLES, FAC
+  // and SNR messages
+  void publish_tv()
+  {
+    for (auto &i : insps) {
+      sdb_engine_t *ie = engine_of(i);
+      if (!i.open || !i.tv_on || i.engine_handle < 0 || !ie) continue;
+      sdb_tv_status st;
+      if (sdb_engine_read_tv(ie, i.engine_handle, nullptr, &st) || !st.completed) continue;
+      const size_t px = (size_t) st.width * st.height;
+      float *frame = (float *) malloc(px * sizeof(float));
+      if (!frame || sdb_engine_read_tv(ie, i.engine_handle, frame, nullptr)) { free(frame); continue; }
+      sdb_analyzer_inspector_msg *m = inspector_msg(SDB_INSPECTOR_MSGKIND_TV, i.handle, i.inspector_id,
+                                                    kClassNames[i.cls]);
+      m->samp_rate = (uint64_t) i.fs; m->fs = (float) rate; m->equiv_fs = i.fs;
+      m->tv = st; m->tv_frame = frame;
+      post(SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR, m);
+    }
+  }
+
   // kind=SNR inspector messages (SPEC SN): one per block in which the meter stepped, after the block's SAMPLES
   std::vector<float> snr_model;
   std::vector<uint32_t> snr_hist;
@@ -997,6 +1042,7 @@ struct sdb_analyzer {
     }
     if (plan_dirty && !rebuild()) return init_failure();
     apply_snr_resets();
+    apply_tv_params();
     bool on_device = false;                      // the decimated block is only in the decimator's device output
     if (!read_block(on_device) || !run_filters(on_device) || !feed(on_device)) return false;
     pace();
@@ -1004,6 +1050,7 @@ struct sdb_analyzer {
     publish_symbols();
     publish_fac();
     publish_snr();
+    publish_tv();
     publish_spectra();
     publish_channels();
     return true;
@@ -1110,7 +1157,8 @@ extern "C" void sdb_analyzer_dispose_message(uint32_t type, void *ptr)
     case SDB_ANALYZER_MESSAGE_TYPE_INSPECTOR:
       free(((sdb_analyzer_inspector_msg *) ptr)->class_name);
       free(((sdb_analyzer_inspector_msg *) ptr)->spectrum_data);
-      free(((sdb_analyzer_inspector_msg *) ptr)->snr_histogram); break;
+      free(((sdb_analyzer_inspector_msg *) ptr)->snr_histogram);
+      free(((sdb_analyzer_inspector_msg *) ptr)->tv_frame); break;
     case SDB_ANALYZER_MESSAGE_TYPE_CHANNEL:
       free(((sdb_analyzer_channel_msg *) ptr)->channel_list);
       free(((sdb_analyzer_channel_msg *) ptr)->tracked_list); break;
@@ -1308,6 +1356,14 @@ extern "C" int sdb_analyzer_inspector_set_snr_async(sdb_analyzer_t *a, int32_t h
 extern "C" int sdb_analyzer_inspector_reset_snr_async(sdb_analyzer_t *a, int32_t handle, float sigma, uint32_t req_id)
 {
   Cmd c; c.kind = Cmd::RESET_SNR; c.req_id = req_id; c.handle = handle; c.snr.sigma = sigma;
+  return push_cmd(a, std::move(c));
+}
+extern "C" int sdb_analyzer_inspector_set_tv_async(sdb_analyzer_t *a, int32_t handle, const sdb_tv_tab_params *p,
+                                                   uint32_t req_id)
+{
+  Cmd c; c.kind = Cmd::SET_TV; c.req_id = req_id; c.handle = handle;
+  c.enabled = p ? 1 : 0;
+  if (p) c.tv = *p;
   return push_cmd(a, std::move(c));
 }
 extern "C" int sdb_analyzer_inspector_estimator_cmd_async(sdb_analyzer_t *a, int32_t handle, uint32_t estimator_id,

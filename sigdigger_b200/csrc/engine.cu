@@ -13,6 +13,7 @@
 #include "../../include/sigdigger_b200.h"
 #include "sdb_internal.h"
 #include "host_design.h"
+#include "sdb_tv_steps.h"
 
 #include <algorithm>
 #include <map>
@@ -46,15 +47,16 @@ struct Channel {
   uint64_t spect_interval = 0;                                    // SPEC US (0: once per feed, SPEC U.1)
   bool has_fac = false; sdb_fac_params fac{};                     // SPEC FC
   bool has_snr = false; sdb_snr_params snr{};                     // SPEC SN
+  bool has_tv = false; sdb_tv_tab_params tv{};                    // SPEC TI
 };
 
 struct TimedSpan { int family; Event a, b; };
 enum { FAM_COLS = 0, FAM_ROWS_PSD, FAM_ROWS_CHAN, FAM_CHAN_IFFT, FAM_INSPECTOR, FAM_PSD_AVERAGE, FAM_POWER, FAM_PSD_PEAK,
-       FAM_SPECTSCHED, FAM_CHAN_TRACK, FAM_FAC, FAM_SNR,
+       FAM_SPECTSCHED, FAM_CHAN_TRACK, FAM_FAC, FAM_SNR, FAM_TV,
        FAM_COUNT };
 static const char *kFamNames[FAM_COUNT] = { "fft_cols", "fft_rows_psd", "fft_rows_chan", "chan_ifft",
                                             "inspector", "psd_average", "power", "psd_peak", "spectsrc_sched",
-                                            "chan_track", "fac", "snr" };
+                                            "chan_track", "fac", "snr", "tv" };
 
 // SPEC PW: samples per mean of a power inspector (power.integrate-samples, 0 read as 1)
 static uint64_t power_m(const sdb_inspector_config &c) { return c.power_integrate_samples ? c.power_integrate_samples : 1; }
@@ -176,6 +178,13 @@ struct Plan {
     std::vector<SdbSnrChan> h; std::vector<int> first; uint32_t max_L = 0;
     DevBuf<SdbSnrChan> chans; DevBuf<uint32_t> hist; DevBuf<float> model; DevBuf<sdb_snr_status> status;
   } snr;
+  // the Analog TV tab (SPEC TI; k_tv_insp in tv_kernels.cu): one descriptor per channel with the TV on, first[k] its
+  // index or -1; per (channel, stream) processor, channel-major: state, delay line, row, ring, posted frame and status
+  struct Tv {
+    std::vector<SdbTvInspChan> h; std::vector<int> first; size_t smem = 0;
+    DevBuf<SdbTvInspChan> chans; DevBuf<SdbTvState> state; DevBuf<float> delay, line, ring, post;
+    DevBuf<sdb_tv_status> status;
+  } tv;
   // frame averaging (SPEC A) and peak detection (SPEC PK), in the order they run
   FrameGroups avg{FAM_PSD_AVERAGE, 1}, peak{FAM_PSD_PEAK, 2};
   // running state
@@ -637,6 +646,81 @@ extern "C" int sdb_engine_read_snr(sdb_engine_t *e, int handle, uint32_t *hist, 
   if (model) CK(cudaMemcpy(model, q.model.get() + h.hist_off, n * sizeof(float), cudaMemcpyDeviceToHost));
   if (st) CK(cudaMemcpy(st, q.status.get() + h.chain0, e->prm.n_streams * sizeof(sdb_snr_status),
                         cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// SPEC TI.4: the tab's parameters, and what a running processor cannot change (TV.7)
+int sdb_tv_tab_check(const sdb_tv_tab_params *p)
+{
+  if (!sdb_tv_params_valid(p->tv)) return fail("TV: invalid parameters (the sample rate may be too low for them)");
+  return 0;
+}
+
+bool sdb_tv_same_geometry(const sdb_tv_params &a, const sdb_tv_params &b)
+{
+  SdbTvCfg x, y;
+  sdb_tv_derive(a, x); sdb_tv_derive(b, y);
+  return x.W == y.W && x.H == y.H && x.delay_len == y.delay_len && x.interlace == y.interlace;
+}
+
+// SPEC TI.1: the processor's constants and the conversion of the channel's class
+static void tv_describe(const Channel &c, SdbTvInspChan &h)
+{
+  sdb_tv_derive(c.tv.tv, h.c);
+  h.mode = c.cfg.insp_class == SDB_INSP_ASK ? 0 : 1;
+  h.gain = c.tv.invert_sync ? -1.0f : 1.0f; h.dc = c.tv.dc;
+}
+
+extern "C" int sdb_engine_set_tv(sdb_engine_t *e, int handle, const sdb_tv_tab_params *p)
+{
+  if (!e) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (e->plan) return fail("engine already committed");
+  Channel &c = e->channels[handle];
+  if (!p) { c.has_tv = false; return 0; }
+  if (sdb_tv_tab_check(p)) return -1;
+  if (!c.has_insp || c.cfg.insp_class > SDB_INSP_ASK) return fail("the TV needs a psk, fsk or ask inspector");
+  c.tv = *p; c.has_tv = true;
+  return 0;
+}
+
+// SPEC TI.4: from the next feed on, in order with the feeds; the state is kept
+extern "C" int sdb_engine_set_tv_params(sdb_engine_t *e, int handle, const sdb_tv_tab_params *p)
+{
+  if (!e || !p) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (!e->plan) return fail("engine not committed");
+  Plan::Tv &q = e->plan->tv;
+  if (q.first.empty() || q.first[handle] < 0) return fail("the TV is not on for this channel");
+  if (sdb_tv_tab_check(p)) return -1;
+  Channel &c = e->channels[handle];
+  if (!sdb_tv_same_geometry(c.tv.tv, p->tv))
+    return fail("TV: the picture geometry (width, height, delay line, interlacing) cannot change without a re-plan");
+  SdbTvInspChan &h = q.h[q.first[handle]];
+  CK(cudaSetDevice(e->prm.device));
+  CK(e->join());
+  CK(cudaStreamSynchronize(e->stream));
+  c.tv = *p;
+  tv_describe(c, h);
+  CK(cudaMemcpy(q.chans.get() + q.first[handle], &h, sizeof(h), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+extern "C" int sdb_engine_read_tv(sdb_engine_t *e, int handle, float *frames, sdb_tv_status *st)
+{
+  if (!e) return fail("null argument");
+  if (handle < 0 || handle >= (int) e->channels.size()) return fail("wrong handle");
+  if (!e->plan) return fail("engine not committed");
+  const Plan::Tv &q = e->plan->tv;
+  if (q.first.empty() || q.first[handle] < 0) return fail("the TV is not on for this channel");
+  const SdbTvInspChan &h = q.h[q.first[handle]];
+  const unsigned S = e->prm.n_streams;
+  CK(cudaSetDevice(e->prm.device));
+  CK(e->join());
+  CK(cudaStreamSynchronize(e->stream));
+  if (frames) CK(cudaMemcpy(frames, q.post.get() + h.post_off, (size_t) S * h.c.H * h.c.W * sizeof(float),
+                            cudaMemcpyDeviceToHost));
+  if (st) CK(cudaMemcpy(st, q.status.get() + h.chain0, S * sizeof(sdb_tv_status), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1135,6 +1219,66 @@ static int snr_commit(sdb_engine *e, Plan &p)
   return 0;
 }
 
+// SPEC TI: every channel with the TV on starts from sdb_tv_state_init with every buffer zero
+static int tv_commit(sdb_engine *e, Plan &p)
+{
+  const unsigned S = e->prm.n_streams;
+  const int K = (int) e->channels.size();
+  Plan::Tv &q = p.tv;
+  q.first.assign(K, -1);
+  size_t nd = 0, nl = 0, nr = 0, np = 0;
+  std::vector<SdbTvState> st;
+  std::vector<sdb_tv_status> status;
+  for (int k = 0; k < K; ++k) {
+    const Channel &c = e->channels[k];
+    if (!c.has_tv) continue;
+    if (!c.has_insp || c.cfg.insp_class > SDB_INSP_ASK) return fail("the TV needs a psk, fsk or ask inspector");
+    if (sdb_tv_tab_check(&c.tv)) return -1;
+    SdbTvInspChan h{};
+    tv_describe(c, h);
+    const size_t px = (size_t) h.c.H * h.c.W;
+    h.k = (uint32_t) k; h.chain0 = (uint32_t) st.size();
+    h.delay_off = nd; h.line_off = nl; h.ring_off = nr; h.post_off = np;
+    nd += (size_t) S * h.c.delay_len; nl += (size_t) S * h.c.W; nr += (size_t) S * SDB_TV_RING * px; np += S * px;
+    q.smem = std::max(q.smem, (size_t) (h.c.W + h.c.delay_len) * sizeof(float));
+    q.first[k] = (int) q.h.size();
+    q.h.push_back(h);
+    SdbTvState s0;
+    sdb_tv_state_init(h.c, s0);
+    st.insert(st.end(), S, s0);
+    status.insert(status.end(), S, sdb_tv_status{ 0ull, 0ull, 0u, (uint32_t) h.c.W, (uint32_t) h.c.H, s0.est_line_len,
+                                                  s0.est_hsync_len, s0.agc_gain });
+  }
+  if (q.h.empty()) return 0;
+  if (q.chans.alloc(q.h.size()) || q.state.alloc(st.size()) || q.status.alloc(st.size()) || q.delay.alloc(nd) ||
+      q.line.alloc(nl) || q.ring.alloc(nr) || q.post.alloc(np))
+    return fail("out of device memory (TV)");
+  CK(cudaMemcpy(q.chans, q.h.data(), q.h.size() * sizeof(SdbTvInspChan), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(q.state, st.data(), st.size() * sizeof(SdbTvState), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(q.status, status.data(), status.size() * sizeof(sdb_tv_status), cudaMemcpyHostToDevice));
+  CK(cudaMemset(q.delay, 0, nd * sizeof(float)));
+  CK(cudaMemset(q.line, 0, nl * sizeof(float)));
+  CK(cudaMemset(q.ring, 0, nr * sizeof(float)));
+  CK(cudaMemset(q.post, 0, np * sizeof(float)));
+  return 0;
+}
+
+// SPEC TI.1-TI.3 for one feed, on the inspector stream after the SNR meter
+static int tv_feed(sdb_engine *e, Plan &p, Slot &sl, const SdbLaunchCtx &ictx)
+{
+  Plan::Tv &q = p.tv;
+  if (q.h.empty()) return 0;
+  SdbTvInspArgs a{};
+  a.chans = q.chans; a.n_chans = (int) q.h.size(); a.n_streams = (int) e->prm.n_streams;
+  a.n_channels = (int) e->channels.size(); a.smem = q.smem;
+  a.soft = sl.soft; a.counts = sl.counts; a.sym_cap = p.sym_cap;
+  a.state = q.state; a.delay = q.delay; a.line = q.line; a.ring = q.ring; a.post = q.post; a.status = q.status;
+  e->span_begin(FAM_TV, ictx.stream);
+  CK(sdb_launch_tv_insp(ictx, a));
+  e->span_end(ictx.stream);
+  return 0;
+}
+
 // SPEC SN.2 for one feed, on the inspector stream after the chains (and the power and FAC launches)
 static int snr_feed(sdb_engine *e, Plan &p, Slot &sl, const SdbLaunchCtx &ictx)
 {
@@ -1462,6 +1606,7 @@ extern "C" int sdb_engine_commit(sdb_engine_t *e)
     }
     if (fac_commit(e, p, max_hops)) return -1;
     if (snr_commit(e, p)) return -1;
+    if (tv_commit(e, p)) return -1;
   }
   if (e->prm.flags & SDB_FLAG_DC_REMOVE) {
     p.d_dc_state = p.dalloc<float2>(S); p.d_dc_cur = p.dalloc<float2>(S);
@@ -1707,6 +1852,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
       }
       if (fac_feed(e, p, sl, ictx)) return -1;
       if (snr_feed(e, p, sl, ictx)) return -1;
+      if (tv_feed(e, p, sl, ictx)) return -1;
       CK(sl.insp.record(ictx.stream));
     } else {
       std::fill(sl.sched_n.begin(), sl.sched_n.end(), 0u);   // no channel samples: no emission
@@ -1714,6 +1860,7 @@ extern "C" int sdb_engine_feed_device(sdb_engine_t *e, const sdb_complex *xv, si
       CK(cudaMemsetAsync(sl.counts, 0, (size_t) S * K * sizeof(uint32_t), p.insp_stream));
       if (fac_feed(e, p, sl, SdbLaunchCtx{ p.insp_stream.get(), &e->launches })) return -1;   // (a status of no blocks)
       if (snr_feed(e, p, sl, SdbLaunchCtx{ p.insp_stream.get(), &e->launches })) return -1;   // (a status of no step)
+      if (tv_feed(e, p, sl, SdbLaunchCtx{ p.insp_stream.get(), &e->launches })) return -1;    // (no frame completed)
       CK(sl.insp.record(p.insp_stream));
     }
     // keep the last half window of every stream as history for the next feed
@@ -2024,6 +2171,29 @@ static int snr_migrate(Plan &to, const Plan &from, const Channel &cn, const Chan
   return 0;
 }
 
+// SPEC TI.5: a channel that keeps its class and the picture geometry keeps the whole processor; its new descriptor
+// (parameters, invert_sync, dc) applies from the next feed
+static int tv_migrate(Plan &to, const Plan &from, const Channel &cn, const Channel &co, int kn, int ko, unsigned S)
+{
+  const int qn = to.tv.first.empty() ? -1 : to.tv.first[kn], qo = from.tv.first.empty() ? -1 : from.tv.first[ko];
+  if (qn < 0 || qo < 0 || cn.cfg.insp_class != co.cfg.insp_class || !sdb_tv_same_geometry(cn.tv.tv, co.tv.tv)) return 0;
+  const SdbTvInspChan &hn = to.tv.h[qn], &ho = from.tv.h[qo];
+  const size_t px = (size_t) hn.c.H * hn.c.W;
+  CK(cudaMemcpy(to.tv.state.get() + hn.chain0, from.tv.state.get() + ho.chain0, S * sizeof(SdbTvState),
+                cudaMemcpyDeviceToDevice));
+  CK(cudaMemcpy(to.tv.status.get() + hn.chain0, from.tv.status.get() + ho.chain0, S * sizeof(sdb_tv_status),
+                cudaMemcpyDeviceToDevice));
+  CK(cudaMemcpy(to.tv.delay.get() + hn.delay_off, from.tv.delay.get() + ho.delay_off,
+                (size_t) S * hn.c.delay_len * sizeof(float), cudaMemcpyDeviceToDevice));
+  CK(cudaMemcpy(to.tv.line.get() + hn.line_off, from.tv.line.get() + ho.line_off, (size_t) S * hn.c.W * sizeof(float),
+                cudaMemcpyDeviceToDevice));
+  CK(cudaMemcpy(to.tv.ring.get() + hn.ring_off, from.tv.ring.get() + ho.ring_off, S * SDB_TV_RING * px * sizeof(float),
+                cudaMemcpyDeviceToDevice));
+  CK(cudaMemcpy(to.tv.post.get() + hn.post_off, from.tv.post.get() + ho.post_off, S * px * sizeof(float),
+                cudaMemcpyDeviceToDevice));
+  return 0;
+}
+
 static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<int> &old_of_new)
 {
   CK(cudaSetDevice(dst->prm.device));
@@ -2079,6 +2249,7 @@ static int migrate_impl(sdb_engine_t *dst, sdb_engine_t *src, const std::vector<
                     S * (L / 2) * sizeof(float), cudaMemcpyDeviceToDevice));
     }
     if (snr_migrate(to, from, cn, co, kn, ko, S)) return -1;
+    if (tv_migrate(to, from, cn, co, kn, ko, S)) return -1;
     if (!cn.has_insp || !co.has_insp) continue;
     if (is_power(cn) || is_power(co)) {
       // SPEC PW: the partial group goes on while the inspector stays a power inspector with the same M

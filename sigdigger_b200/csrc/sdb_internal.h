@@ -560,6 +560,10 @@ struct SdbSnrArgs {
 // engine.cu: the parameter checks of sdb_engine_set_snr (0, or -1 with sdb_last_error() set), shared with the analyzer
 int sdb_snr_check(const sdb_snr_params *p);
 cudaError_t sdb_launch_snr(const SdbLaunchCtx &c, const SdbSnrArgs &a);
+// engine.cu: the parameter checks of sdb_engine_set_tv (0, or -1 with sdb_last_error() set) and whether two parameter
+// blocks give the same picture geometry (W, H, delay line, interlacing), shared with the analyzer
+int sdb_tv_tab_check(const sdb_tv_tab_params *p);
+bool sdb_tv_same_geometry(const sdb_tv_params &a, const sdb_tv_params &b);
 // stream-ordered pieces of the panoramic sweep (panoramic.cu): caller-owned device buffers, no host copies, no
 // default-stream work.  engine.cu:
 int sdb_engine_pack_channels_device(sdb_engine_t *e, const double *centers_dev, sdb_detected_channel *out_dev, size_t cap,

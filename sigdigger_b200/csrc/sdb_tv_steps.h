@@ -190,6 +190,23 @@ SDB_HD int sdb_tv_step(const SdbTvCfg &c, SdbTvState &s, float *delay, float *li
   return flags;
 }
 
+// ---- the engine's Analog TV tab (oracle/SPEC_TI.md; k_tv_insp in tv_kernels.cu).  One descriptor per channel with
+// the TV on; its processors are chain0 + s (s < n_streams), each with its delay line, row, ring and posted frame at
+// the channel's offset + s times their size.
+struct SdbTvInspChan {
+  SdbTvCfg c;
+  uint32_t k, chain0;                 // channel (symbol row s * n_channels + k), first processor
+  int32_t mode;                       // TI.1: 0 modulus (ask), 1 argument (psk, fsk), as k_tv_feed_transform
+  float gain, dc;                     // TI.1: k = -1 (invert_sync) or +1, and dc
+  size_t delay_off, line_off, ring_off, post_off;
+};
+struct SdbTvInspArgs {
+  const SdbTvInspChan *chans; int n_chans, n_streams, n_channels; size_t smem;
+  const float2 *soft; const uint32_t *counts; size_t sym_cap;
+  SdbTvState *state; float *delay, *line, *ring, *post; sdb_tv_status *status;
+};
+cudaError_t sdb_launch_tv_insp(const SdbLaunchCtx &ctx, const SdbTvInspArgs &a);
+
 // ---- host-side: validity and derived constants (SPEC TV.0 / TV.1).  P has the fields of sigutils_tv_processor_params
 // (sdb_tv_params in the C-ABI, struct sigutils_tv_processor_params in <sigutils/tvproc.h>).
 #include <math.h>

@@ -10,6 +10,8 @@
 // line and the row being drawn in shared memory; the warp loads the input 32 samples at a time (coalesced) and hands
 // them to lane 0 by shuffle, and all 32 lanes store a finished row into the frame ring (coalesced) and clear it.
 // Bound: serial latency of the step (one processor advances a few MS/s; a batch scales with the SM count).
+// k_tv_insp runs the same warp over an engine inspector's device-side soft symbols: the inspector panel's Analog TV
+// tab (InspectorUI.cpp:851-852, oracle/SPEC_TI.md), one processor per (TV channel, stream), launched by engine.cu.
 // Compiled with -fmad=false: bit-identical to oracle/tvproc.c and to the host step of <sigutils/tvproc.h>.
 #include "sdb_tv_steps.h"
 #include <vector>
@@ -68,6 +70,93 @@ __global__ void k_tv_feed_transform(const float2 *__restrict__ x, size_t n, int 
   const float2 v = x[i];
   out[i] = mode == 0 ? k * sqrtf(v.x * v.x + v.y * v.y) + dc
                      : k * d_atan2f(v.y, v.x) / 3.14159265358979323846f + dc;
+}
+
+// The engine's Analog TV tab (oracle/SPEC_TI.md): one warp per (TV channel, stream), grid (n_streams, n_chans), on
+// the inspector stream after the feed's chains.  As k_tv_feed, but the input is the row's soft symbols and their
+// device-side count, converted in the coalesced load with k_tv_feed_transform's expression (TI.1), and the feed's
+// first completed frame is copied from its ring slot to the posted frame as soon as it completes (TI.3: four more
+// frames of the same feed would overwrite the slot).  Dynamic shared memory: the largest W + delay_len.
+__global__ void __launch_bounds__(32) k_tv_insp(const SdbTvInspChan *__restrict__ chans, int n_channels,
+                                                const float2 *__restrict__ soft, const uint32_t *__restrict__ counts,
+                                                size_t sym_cap, SdbTvState *__restrict__ states,
+                                                float *__restrict__ delays, float *__restrict__ lines,
+                                                float *__restrict__ rings, float *__restrict__ posts,
+                                                sdb_tv_status *__restrict__ status)
+{
+  const SdbTvInspChan &ch = chans[blockIdx.y];
+  const int s = blockIdx.x, lane = threadIdx.x;
+  const unsigned p = ch.chain0 + s;
+  const size_t row = (size_t) s * n_channels + ch.k;
+  const unsigned n = counts[row];
+  if (n == 0) {                                    // TI.2: nothing changes
+    if (lane == 0) status[p].completed = 0;
+    return;
+  }
+  const SdbTvCfg c = ch.c;
+  const int mode = ch.mode;
+  const float gain = ch.gain, dc = ch.dc;
+  extern __shared__ float s_tv[];                  // [W] row being drawn | [delay_len] comb delay line
+  float *s_line = s_tv, *s_delay = s_tv + c.W;
+  const size_t px = (size_t) c.H * c.W;
+  float *g_line = lines + ch.line_off + (size_t) s * c.W, *g_delay = delays + ch.delay_off + (size_t) s * c.delay_len;
+  float *ring = rings + ch.ring_off + (size_t) s * SDB_TV_RING * px;
+  float *__restrict__ post = posts + ch.post_off + (size_t) s * px;
+  for (int k = lane; k < c.W; k += 32) s_line[k] = g_line[k];
+  for (int k = lane; k < c.delay_len; k += 32) s_delay[k] = g_delay[k];
+  SdbTvState st;
+  if (lane == 0) st = states[p];
+  __syncwarp();
+  const float2 *__restrict__ xs = soft + row * sym_cap;
+  unsigned done = 0;
+  for (unsigned i0 = 0; i0 < n; i0 += 32) {
+    float xv = 0.0f;
+    if (i0 + lane < n) {
+      const float2 v = xs[i0 + lane];
+      xv = mode == 0 ? gain * sqrtf(v.x * v.x + v.y * v.y) + dc
+                     : gain * d_atan2f(v.y, v.x) / 3.14159265358979323846f + dc;
+    }
+    const int cnt = n - i0 < 32 ? (int) (n - i0) : 32;
+    for (int j = 0; j < cnt; ++j) {
+      const float xj = __shfl_sync(0xffffffffu, xv, j);
+      int flags = 0, frow = -1, fslot = 0;
+      if (lane == 0) flags = sdb_tv_step(c, st, s_delay, s_line, xj, &frow, &fslot);
+      flags = __shfl_sync(0xffffffffu, flags, 0);
+      if (flags & SDB_TV_LINE_DONE) {
+        frow = __shfl_sync(0xffffffffu, frow, 0);
+        fslot = __shfl_sync(0xffffffffu, fslot, 0);
+        float *__restrict__ slot = ring + (size_t) fslot * px;
+        if (frow >= 0)
+          for (int k = lane; k < c.W; k += 32) slot[(size_t) frow * c.W + k] = s_line[k];
+        for (int k = lane; k < c.W; k += 32) s_line[k] = 0.0f;
+        __syncwarp();
+        if ((flags & SDB_TV_FRAME_DONE) && ++done == 1) {
+          for (size_t k = lane; k < px; k += 32) post[k] = slot[k];
+          __syncwarp();
+        }
+      }
+    }
+  }
+  __syncwarp();
+  for (int k = lane; k < c.W; k += 32) g_line[k] = s_line[k];
+  for (int k = lane; k < c.delay_len; k += 32) g_delay[k] = s_delay[k];
+  if (lane == 0) {
+    states[p] = st;
+    sdb_tv_status o = status[p];
+    if (done) o.posted_no = st.frames - done + 1;
+    o.frames = st.frames; o.completed = done; o.width = (uint32_t) c.W; o.height = (uint32_t) c.H;
+    o.line_len = st.est_line_len; o.hsync_len = st.est_hsync_len; o.agc_gain = st.agc_gain;
+    status[p] = o;
+  }
+}
+
+cudaError_t sdb_launch_tv_insp(const SdbLaunchCtx &ctx, const SdbTvInspArgs &a)
+{
+  if (a.n_chans <= 0) return cudaSuccess;
+  k_tv_insp<<<dim3((unsigned) a.n_streams, (unsigned) a.n_chans), 32, a.smem, ctx.stream>>>(
+      a.chans, a.n_channels, a.soft, a.counts, a.sym_cap, a.state, a.delay, a.line, a.ring, a.post, a.status);
+  if (ctx.launch_counter) ++*ctx.launch_counter;
+  return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------
